@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Headline benchmark: env steps/sec of the PPO hot path (BASELINE.json metric) on N B200s.
+"""Headline benchmark: env steps/sec of the PPO hot path (BASELINE.json metric) on N H100s.
 
     python bench.py --gpus 1 --steps K --warmup W            # our arm (libb200rl kernels)
     python bench.py --impl reference --gpus N --steps K ...  # reference arm: the reference's CPU path
@@ -42,7 +42,7 @@ def bench_config(N, T, world):
     return {"workload": "ppo_atari_envpool Breakout-shaped synthetic vec env; per GPU num_envs=%d num_steps=%d, "
                         "4 epochs x 4 minibatches of %d, NatureCNN A=4; one step = one PPO iteration" % (N, T, N * T // 4),
             "global_num_envs": N * world, "parallelism": f"dp{world}",
-            "timing": "inputs_larger_than_L2 (3.7 GB uint8 rollout + 2.8 GB activations per minibatch vs 126 MB L2)",
+            "timing": "inputs_larger_than_L2 (3.7 GB uint8 rollout + 2.8 GB activations per minibatch vs 50 MB L2)",
             "gae_kernel": "scan"}
 
 
@@ -59,7 +59,7 @@ def ppo_args(num_envs, num_steps, num_iterations, precision):
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons during the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -72,9 +72,9 @@ class ClockSampler:
         self.t0 = self.t1 = None
 
     def start(self):
-        """Start sampling (nvidia-smi needs ~0.5 s to deliver its first line: start it BEFORE the warm-up).  200 ms is the
-        recipe's period (B200_PROFILING.md); every query takes driver locks, and at 50 ms the end-to-end rollout -- which is
-        bound by host-side CUDA API calls -- measurably slowed down."""
+        """Start sampling (nvidia-smi needs ~0.5 s to deliver its first line: start it BEFORE the warm-up).  Every query takes
+        driver locks, and at 50 ms the end-to-end rollout -- which is bound by host-side CUDA API calls -- measurably slowed
+        down; the default period is 200 ms."""
         period = os.environ.get("BENCH_CLOCK_SAMPLE_MS", "200")
         if period == "0":
             self.proc = None
@@ -135,7 +135,7 @@ def pin_to_gpu_cores(gpu_index):
     local to the GPU, so that pinned staging memory, the env buffers and the upload path sit on the GPU's NUMA node.  One
     process per GPU: every rank pins to its own GPU's cores.  OFF by default (BENCH_CPU_AFFINITY=1 turns it on): on the
     shared hosts this was measured on, the GPU-local socket is where every other tenant's processes sit as well, and the
-    pinned run was 2x slower than letting the scheduler pick idle cores (profiles/r2_host_sensitivity.md)."""
+    pinned run was slower than letting the scheduler pick idle cores."""
     if os.environ.get("BENCH_CPU_AFFINITY", "0") != "1" or not hasattr(os, "sched_setaffinity"):
         return None
     try:
@@ -157,8 +157,8 @@ def measured_peaks():
     p = ROOT / "MEASURED_PEAKS.json"
     if p.exists():
         z = json.loads(p.read_text())
-        return z.get("bf16_tflops_sustained", 1400.0), z.get("hbm_gbs", 6650.0), "measured"
-    return 1400.0, 6650.0, "fallback"
+        return z.get("bf16_tflops_sustained", 989.0), z.get("hbm_gbs", 3350.0), "measured"
+    return 989.0, 3350.0, "H100 SXM data sheet (dense bf16, HBM3)"
 
 
 # --------------------------------------------------------------------------------- our arm
@@ -245,7 +245,7 @@ def run_ours(opt):
         return env_sets[mode]
 
     # frame-stacked observations only pay off through the delta upload; where the engine uploads whole observations (several
-    # ranks per host by default, CLEANRL_B200_DELTA_UPLOAD=0) the e2e arm hands it dense pinned batches as rounds 1-2 did
+    # ranks per host by default, CLEANRL_B200_DELTA_UPLOAD=0) the e2e arm hands it dense pinned batches
     obs_mode = opt.env_obs if (opt.env_obs == "pool" or eng.delta_upload) else "pool"
     if G > 1:
         env_parts, state = use_envs(obs_mode)
@@ -343,6 +343,8 @@ def run_ours(opt):
 
     replica_trace("init")
     res = timed(iteration_resident)                 # `value`: update replayed as per-epoch CUDA graphs, no profiling events
+    if opt.dump_outputs and rank == 0:
+        dump_outputs(opt.dump_outputs, eng, res["stats"])
     replica_trace("after resident loop")
     eng.update_graphs = False                       # per-kernel CUDA-event brackets cannot live inside a captured graph:
     prof_run = timed(iteration_resident, profile=True)      # the kernel table comes from an eager pass of the same iteration
@@ -459,19 +461,11 @@ def run_ours(opt):
     secs = top["ms"] * 1e-3
     ach_tf = top["flops"] / secs / 1e12 if secs > 0 else 0.0
     ach_gb = top["bytes"] / secs / 1e9 if secs > 0 else 0.0
-    traffic = None
-    for name in ("r2_traffic.json", "r1_traffic.json"):      # the newest ncu --set full capture that has this kernel
-        tp = ROOT / "profiles" / name
-        tr = json.loads(tp.read_text()).get(top["name"]) if tp.exists() else None
-        if tr:
-            traffic = {"dram_bytes_per_launch": tr["dram_bytes"], "algorithmic_bytes_per_launch": tr["algorithmic_bytes"],
-                       "at_n": tr["n"], "from": f"profiles/{name} (ncu --set full)"}
-            break
     roofline = {
         "bound": "hbm" if hbm_bound else "tensor", "kernel": top["name"],
         "achieved": round(ach_gb if hbm_bound else ach_tf, 2), "peak": peak_hbm if hbm_bound else peak_tf,
         "unit": "GB/s" if hbm_bound else "TFLOP/s",
-        "frac": round(ach_gb / peak_hbm if hbm_bound else ach_tf / peak_tf, 4), "traffic": traffic,
+        "frac": round(ach_gb / peak_hbm if hbm_bound else ach_tf / peak_tf, 4),
         "peak_source": f"{which} " + ("hbm_gbps" if hbm_bound else "bf16_tflops_sustained"),
         "arithmetic_intensity_flop_per_byte": round(intensity, 1), "ridge_flop_per_byte": round(ridge, 1),
         "achieved_tflops": round(ach_tf, 2), "achieved_gbs": round(ach_gb, 1),
@@ -533,6 +527,37 @@ def run_ours(opt):
         out["extra"] = extra_configs()
     print(json.dumps(out), flush=True)
     shutdown()
+
+
+DUMP_BUDGET_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, eng, stats):
+    """What the timed iteration's caller receives, from its last step: the rollout's sampled actions, log-probabilities,
+    values, GAE advantages and returns ([num_steps, num_envs] each) and the parameters after the update as float32, and
+    the update's scalar statistics as float64.  Everything stays within 64 MB: when the five rollout arrays would not fit
+    beside the parameters, they keep a fixed, seeded sample of env columns (the same for every run with the same
+    num_envs), whose indices are written as env_index.npy."""
+    import torch
+    torch.cuda.synchronize()
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    params = eng.flat.flat.detach().float().cpu().numpy()
+    rollout = {"actions": eng.actions, "logprobs": eng.logprobs, "values": eng.values, "advantages": eng.advantages,
+               "returns": eng.returns}
+    T, N = eng.actions.shape[0], eng.actions.shape[1]
+    cols = (DUMP_BUDGET_BYTES - params.nbytes - (1 << 20)) // (len(rollout) * T * 4)    # 1 MB for env_index and statistics
+    keep = None
+    if cols < N:
+        keep = np.sort(np.random.default_rng(0).choice(N, size=max(int(cols), 1), replace=False))
+        np.save(d / "env_index.npy", keep.astype(np.float64))
+    for name, t in rollout.items():
+        a = t.detach().float().cpu().numpy().reshape(T, N)
+        np.save(d / f"{name}.npy", a if keep is None else a[:, keep])
+    np.save(d / "params.npy", params)
+    for k, v in (stats or {}).items():
+        if isinstance(v, (int, float)):
+            np.save(d / f"stat_{k}.npy", np.array(float(v), dtype=np.float64))
 
 
 # ------------------------------------------------------------------ BASELINE.json configs[3] and configs[4]
@@ -639,7 +664,7 @@ def cpu_baseline(opt):
 def gpu_eager_baseline(opt):
     """SURVEY 8(d)(ii): what `python cleanrl/ppo_atari_envpool.py --cuda` executes on this same GPU -- fp32 rollout
     storage on the device, eager torch / cuDNN / cuBLAS ops, autograd, foreach Adam, per-step action sync -- restated
-    by oracle/ppo_port.py with device="cuda" (no /root/reference on the GPU box).  2 iterations, the second is timed."""
+    by oracle/ppo_port.py with device="cuda" (the reference is not installed on the GPU machine).  2 iterations, the second is timed."""
     import torch
     from oracle import ppo_port
     try:
@@ -656,7 +681,7 @@ def gpu_eager_baseline(opt):
 
 def run_reference(opt):
     """--impl reference: the reference's own CPU implementation of the path (torch CPU loop, all host threads it can
-    use) -- the oracle port, because /root/reference does not exist on the GPU box.  Same `config` as our arm; every
+    use) -- the oracle port, because the reference is not installed on the GPU machine.  Same `config` as our arm; every
     step is a bounded sample of that workload: one 1/16-iteration slice at full tensor shapes (see cpu_sample)."""
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
@@ -698,6 +723,8 @@ def main():
     ap.add_argument("--no-extra", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-gpu-eager-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the timed iteration computed in its last step as DIR/<name>.npy")
     opt = ap.parse_args()
     if opt.impl == "reference":
         run_reference(opt)

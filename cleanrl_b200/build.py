@@ -1,4 +1,4 @@
-"""Compile libb200rl.so in-tree with nvcc for sm_100a (no JIT cache, no torch headers).
+"""Compile libb200rl.so in-tree with nvcc for sm_90a (no JIT cache, no torch headers).
 
 ``python -m cleanrl_b200.build`` or ``__graft_entry__.build()``.
 """
@@ -17,8 +17,8 @@ LIB = PKG / "libb200rl.so"
 STAMP = PKG / ".libb200rl.stamp"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
-    "-Xcompiler", "-fPIC", "-shared", "-DB200RL_ARCH=100",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
+    "-Xcompiler", "-fPIC", "-shared", "-DB200RL_ARCH=90",
 ]
 
 

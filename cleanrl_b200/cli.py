@@ -53,7 +53,7 @@ _RUNTIME = [
 _EXTRA = [
     ("precision", Literal["fp32", "bf16"], "fp32",
      "[b200] network arithmetic: fp32 = exact CUDA-core kernels (reference numerics), "
-     "bf16 = tcgen05 tensor-core kernels with fp32 accumulation"),
+     "bf16 = wgmma tensor-core kernels with fp32 accumulation"),
     ("gae_kernel", Literal["sequential", "scan"], "sequential",
      "[b200] GAE kernel: sequential = bit-identical to the reference loop, scan = chunked affine scan"),
     ("synthetic_env", bool, False,

@@ -71,9 +71,5 @@ extern "C" int b200rl_profile_summary(char* buf, size_t cap) {
 extern "C" int b200rl_version(void) { return 100; }  // 0.1.0
 extern "C" const char* b200rl_last_error(void) { return b200rl::err_buf(); }
 extern "C" int b200rl_compiled_arch(void) {
-#ifdef B200RL_ARCH
     return B200RL_ARCH;
-#else
-    return 100;
-#endif
 }

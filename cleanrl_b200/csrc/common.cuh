@@ -1,4 +1,4 @@
-// Shared host/device helpers for libb200rl.so (sm_100a).
+// Shared host/device helpers for libb200rl.so (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdarg>

@@ -139,7 +139,7 @@ extern "C" int b200rl_gae_f32(const float* rewards, const float* values, const f
     cudaStream_t s = (cudaStream_t)stream;
     ProfScope ps(s, mode == 0 ? "gae_seq" : "gae_scan", 0, 20.0 * T * N + 8.0 * N);
     if (mode == 0) {
-        const int threads = (N >= 148 * 64) ? 64 : 32;
+        const int threads = (N >= 132 * 64) ? 64 : 32;
         const unsigned blocks = (unsigned)ceil_div(N, threads);
         gae_seq_kernel<8><<<blocks, threads, 0, s>>>(rewards, values, dones, next_value, next_done,
                                                      advantages, returns, T, N, g, gl);

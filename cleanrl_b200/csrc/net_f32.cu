@@ -9,7 +9,7 @@
 // This is the fp32 validation path of the NatureCNN (reference:
 // cleanrl/ppo_atari_envpool.py:123-139) and the production path of the 64-wide
 // MLPs of ppo.py / ppo_continuous_action.py, which are launch-latency bound.
-// The bf16 tcgen05 path (net_tc.cu) is the throughput path for the CNN.
+// The bf16 wgmma path (net_tc.cu) is the throughput path for the CNN.
 //
 // Tile: 64x64 outputs per CTA, K-step 16, 256 threads, 4x4 outputs/thread.
 // Weight-grad problems split the (huge) reduction over grid.z into a partial
@@ -259,7 +259,7 @@ static int launch(const P& p, int64_t M, int64_t N, int64_t R, int splits, cudaS
 }
 
 static int split_count(int64_t tiles, int64_t R) {
-    int64_t want = ceil_div(148 * 4, tiles > 0 ? tiles : 1);
+    int64_t want = ceil_div(132 * 4, tiles > 0 ? tiles : 1);
     int64_t maxs = ceil_div(R, 256);     // keep >= 256 reduction steps per split
     if (want > maxs) want = maxs;
     if (want < 1) want = 1;

@@ -1,4 +1,4 @@
-// NatureCNN on the 5th-gen tensor cores (tcgen05.mma, accumulators in TMEM), bf16 operands,
+// NatureCNN on the Hopper tensor cores (wgmma, accumulators in registers), bf16 operands,
 // fp32 accumulation.  Reference network: cleanrl/ppo_atari_envpool.py:123-139.
 //
 // Data layout in HBM (all activations are LINEAR PIXEL GRIDS: row = grid position, 128 bytes = 64 channels)
@@ -18,11 +18,10 @@
 //   tc_conv_win<BN,CPR,STAGES,NTAPS>   stride-1 "window" convolution (conv1/2/3 forward, conv3/conv2 data-gradient):
 //       GEMM rows enumerate grid positions, so tap (dy,dx) of row r is row r + dy*Wp + dx.  A persistent CTA
 //       stages ONE window of 128+maxshift rows per tile as a TMA box (cp.async.bulk.tensor; for conv1 a 3-D box
-//       whose image coordinate is the minibatch gather) and every tap is a UMMA descriptor whose start address is
+//       whose image coordinate is the minibatch gather) and every tap is a wgmma descriptor whose start address is
 //       shifted by whole 128-byte rows (legal for SWIZZLE_128B: the pattern is a function of the smem address
-//       bits; tools/experiments/umma_shift_test.cu).  Weights stay resident in smem.  Warp 0 = TMA producer, warp 1 issues tcgen05.mma
-//       (warp-uniform loop, elected lane); warps 2-9 = two epilogue groups that own alternate tiles and drain
-//       double-buffered accumulators; ReLU masks are exchanged between forward and backward as bits.
+//       bits).  Weights stay resident in smem.  Warp 0 = TMA producer, two warpgroups run wgmma on 64 rows each and
+//       the epilogue; ReLU masks are exchanged between forward and backward as bits.
 //   tc_wgrad_win                 conv weight gradients: dW^T[(tap,c), co] = sum_r X[r+shift_tap, c] * dY[r, co]; the same
 //       row images are read as MN-major operands (rows = reduction index), taps again by row shifts; the bias
 //       gradient (column sums of dY) is accumulated by the four dY warps from the staged tiles.
@@ -136,7 +135,8 @@ static WPlan wgrad_plan(int64_t M, int target_ctas, int quantum = 32) {
     if (w.splits < 1) w.splits = 1;
     return w;
 }
-static const int kC1Ctas = 296, kC2Ctas = 148, kC3Ctas = 148, kFcSplits = 8;
+// row splits of the weight gradients: one or two waves of CTAs on the 132 SMs of an H100
+static const int kC1Ctas = 264, kC2Ctas = 132, kC3Ctas = 132, kFcSplits = 8;
 
 static int launch_wgrad_win(const WGradWinParams& p, int ctas, cudaStream_t s, const char* what) {
     const size_t smem = (size_t)kWgradWinStages * ((size_t)p.WRX * 128 * p.cpr + 128 * 128) + 4096 + 1024;
@@ -158,12 +158,13 @@ static int launch_wgrad_win(const WGradWinParams& p, int ctas, cudaStream_t s, c
         if ((128 << p.tpi_shift) < p.G) return fail(B200RL_ERR_INVALID_ARGUMENT, "%s: steps per image too small", what);
         if ((rc = make_tmap_3d(&tmX, p.X, p.n_images, p.G, (int64_t)p.cpr * 64, p.WRX, what))) return rc;
     }
-    tc_wgrad_win<<<ctas, kWgradWinThreads, smem, s>>>(tmX, tmY, p, use_tma);
+    const dim3 grid(ctas, (unsigned)ceil_div(p.nslots / 2, kWgradWinTilesPerCta));
+    tc_wgrad_win<<<grid, kWgradWinThreads, smem, s>>>(tmX, tmY, p, use_tma);
     return check_launch(what);
 }
 
 static int colsum(const bf16* Y, int64_t M, int ld, int ncols, float* part, float* db, cudaStream_t s) {
-    int64_t rpb = ceil_div(M, 148 * 3);
+    int64_t rpb = ceil_div(M, 132 * 3);
     if (rpb < 64) rpb = 64;
     const int nb = (int)ceil_div(M, rpb);
     tc_colsum_partial<<<nb, 256, 0, s>>>(Y, M, ld, ncols, rpb, part);
@@ -171,7 +172,7 @@ static int colsum(const bf16* Y, int64_t M, int ld, int ncols, float* part, floa
     return check_launch("colsum", 2);
 }
 static size_t colsum_ws(int64_t M, int ncols) {
-    int64_t rpb = ceil_div(M, 148 * 3);
+    int64_t rpb = ceil_div(M, 132 * 3);
     if (rpb < 64) rpb = 64;
     return (size_t)ceil_div(M, rpb) * ncols * sizeof(float);
 }
@@ -288,7 +289,7 @@ extern "C" int b200rl_naturecnn_bf16_forward(const void* obs, int obs_format, co
     wp.Bw = P + L.w2f; wp.N = 64; wp.vH = 9; wp.vW = 9; wp.out_mode = WOUT_DENSE; wp.out = act + Q.act2;
     wp.bias = params + L.c2b; wp.relu = 1; wp.mask_out = reinterpret_cast<uint32_t*>(act + Q.m2);
     { ProfScope ps(s, "conv2_fwd", 2.0 * n * 81 * 64 * 512, (double)n * ((12800 + 5184) * 2 + 648));
-      if ((rc = launch_conv_win<64, 2, 4, 4>(wp, s, "naturecnn/conv2"))) return rc; }
+      if ((rc = launch_conv_win<64, 2, 3, 4>(wp, s, "naturecnn/conv2"))) return rc; }
     // conv3: 3x3 window conv -> act3 [n,7,7,64]
     win_defaults(wp); win_conv3(wp, act + Q.act2, n);
     wp.Bw = P + L.w3f; wp.N = 64; wp.vH = 7; wp.vW = 7; wp.out_mode = WOUT_DENSE; wp.out = act + Q.act3;
@@ -301,8 +302,8 @@ extern "C" int b200rl_naturecnn_bf16_forward(const void* obs, int obs_format, co
     p.mask_out = reinterpret_cast<uint32_t*>(act + Q.m4);
     { ProfScope ps(s, "fc_fwd", 2.0 * n * 512 * 3136, (double)n * (3136 + 512) * 2 + 512.0 * 3136 * 2);
       // small batches (rollout step): narrower N tiles => 4x more CTAs for the same work
-      if (n <= 8192) { if ((rc = launch_gemm_tma<64, 8>(p, s, "naturecnn/fc"))) return rc; }
-      else if ((rc = launch_gemm_tma<256, 4>(p, s, "naturecnn/fc"))) return rc; }
+      if (n <= 8192) { if ((rc = launch_gemm_tma<64, 6>(p, s, "naturecnn/fc"))) return rc; }
+      else if ((rc = launch_gemm_tma<128, 4>(p, s, "naturecnn/fc"))) return rc; }
     // heads (fp32 math on CUDA cores): head_out [n, A+1] = [logits | value]
     { ProfScope ps(s, "heads_fwd", 2.0 * n * 512 * (A + 1), (double)n * (1024 + 4 * (A + 1)));
       int hb = (int)ceil_div(n, 8); if (hb > num_sms() * 8) hb = num_sms() * 8;
@@ -366,10 +367,12 @@ extern "C" int b200rl_naturecnn_bf16_backward(const void* obs, const void* obs_a
           CUtensorMap tmX, tmY;
           if ((rc = make_tmap_2d(&tmX, act + Q.dhid, n, 512, 64, "naturecnn/fc_wgrad"))) return rc;
           if ((rc = make_tmap_2d(&tmY, act + Q.act3, n, 3136, 64, "naturecnn/fc_wgrad"))) return rc;
-          const size_t smem = (size_t)4 * (2 + 4) * 64 * 128 + 1024;
+          const size_t smem = (size_t)4 * (kFcWgradXChunks + kFcWgradYChunks) * 64 * 128 + 1024;
           static SmemAttrCache attr;
           if ((rc = attr.ensure(tc_wgrad_tma, smem, "naturecnn/fc_wgrad"))) return rc;
-          tc_wgrad_tma<<<dim3(pl.splits, 4, 13), 160, smem, s>>>(tmX, tmY, n, pl.rows_per_cta, 2, 4, wsbig);
+          // X = dhid (512 columns), Y = act3 (3136 columns, the last Y group partly past the end: zero-filled by TMA)
+          const dim3 grid(pl.splits, 512 / (64 * kFcWgradXChunks), (unsigned)ceil_div(3136, 64 * kFcWgradYChunks));
+          tc_wgrad_tma<<<grid, kWgradTmaThreads, smem, s>>>(tmX, tmY, n, pl.rows_per_cta, wsbig);
           if ((rc = check_launch("naturecnn/fc_wgrad"))) return rc; }
         { ProfScope ps(s, "wgrad_fold_bias", 0, 0);
           note_launches(1); tc_fold_fc<<<(unsigned)ceil_div((int64_t)512 * 3136, 256), 256, 0, s>>>(wsbig, pl.splits, 512, 13 * 256, 512, 3136, 64, 49, 1.f, grads + L.fcw);
@@ -384,7 +387,7 @@ extern "C" int b200rl_naturecnn_bf16_backward(const void* obs, const void* obs_a
         p.Bw = P + L.wfcdg; p.N = 3136; p.out = act + Q.dact3a; p.out2 = act + Q.dact3b; p.dual_dact3 = 1;
         p.ldo = 3136; p.mask_bits = reinterpret_cast<const uint32_t*>(act + Q.m3);
         { ProfScope ps(s, "fc_dgrad", 2.0 * n * 512 * 3136, (double)n * ((3136 + 512) * 2 + 392) + 512.0 * 3136 * 2);
-          if ((rc = launch_gemm_tma<256, 4>(p, s, "naturecnn/fc_dgrad"))) return rc; }
+          if ((rc = launch_gemm_tma<128, 4>(p, s, "naturecnn/fc_dgrad"))) return rc; }
     }
     WGradWinParams gw;
     WinParams wp;
@@ -442,13 +445,13 @@ extern "C" int b200rl_naturecnn_bf16_backward(const void* obs, const void* obs_a
         wp.WR = round8(128 + 12);
         wp.Bw = P + L.w2dg; wp.N = 128; wp.vH = 10; wp.vW = 10; wp.out_mode = WOUT_DACT1;
         wp.out = act + Q.dact1; wp.mask_bits = reinterpret_cast<const uint32_t*>(act + Q.m1);
-        if (obs_format == B200RL_OBS_S2D_U8) { wp.out_f16 = 1; wp.scale = kDact1Scale; }     // fp16 x 2^12 for the TMEM-fed conv1 wgrad
+        if (obs_format == B200RL_OBS_S2D_U8) { wp.out_f16 = 1; wp.scale = kDact1Scale; }     // fp16 x 2^12 for the uint8 conv1 wgrad
         { ProfScope ps(s, "conv2_dgrad", 2.0 * n * 400 * 32 * 256, (double)n * ((7744 + 14112) * 2 + 1600));
-          if ((rc = launch_conv_win<128, 1, 6, 4>(wp, s, "naturecnn/conv2_dgrad"))) return rc; }
+          if ((rc = launch_conv_win<128, 1, 4, 4>(wp, s, "naturecnn/conv2_dgrad"))) return rc; }
     }
     // ---- conv1 (no data gradient: the input is the observation)
     if (obs_format == B200RL_OBS_S2D_U8) {
-        // uint8 channel-major frames -> fp16 in registers -> tensor memory (tc_conv1_u8.cuh); 1 CTA per SM (512 TMEM columns)
+        // uint8 channel-major frames -> fp16 wgmma operands in registers (tc_conv1_u8.cuh); 1 CTA per SM
         Conv1WgradU8Params cw;
         memset(&cw, 0, sizeof(cw));
         const WPlan pl = wgrad_plan(n * 512, kC2Ctas, 512);          // whole images per CTA

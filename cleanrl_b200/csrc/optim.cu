@@ -13,7 +13,7 @@
 namespace b200rl {
 
 constexpr int kOptThreads = 256;
-constexpr int kOptMaxBlocks = 148 * 8;
+constexpr int kOptMaxBlocks = 132 * 8;
 
 struct OptScratch {      // lives at the head of the caller's workspace
     float norm;          // pre-clip global L2 norm

@@ -1,4 +1,4 @@
-// Shared types and host helpers of the tcgen05 NatureCNN kernels (included by net_tc.cu and the tc_*.cuh kernel files).
+// Shared types and host helpers of the wgmma NatureCNN kernels (included by net_tc.cu and the tc_*.cuh kernel files).
 #pragma once
 #include <cuda.h>            // CUtensorMap types only; the encoder is resolved at run time (no libcuda link)
 #include <cstring>
@@ -117,7 +117,7 @@ static int num_sms() {
     if (g_num_sms == 0) {
         int dev = 0;
         cudaGetDevice(&dev);
-        if (cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || g_num_sms <= 0) g_num_sms = 148;
+        if (cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || g_num_sms <= 0) g_num_sms = 132;
     }
     return g_num_sms;
 }

@@ -1,7 +1,7 @@
-// tcgen05 / TMEM / mbarrier primitives for sm_100a (inline PTX; no CUTLASS dependency).
+// wgmma / TMA / mbarrier primitives for sm_90a (inline PTX; no CUTLASS dependency).
 //
-// Shared-memory operand images follow the UMMA canonical SWIZZLE_128B layouts
-// (bit fields as in CUTLASS cute/arch/mma_sm100_desc.hpp, restated here):
+// Shared-memory operand images follow the wgmma canonical SWIZZLE_128B layouts
+// (bit fields as in the PTX ISA's matrix-descriptor format, restated here):
 //   one "row" = 128 bytes = 64 bf16, rows 128 B apart, 8 rows = one 1024-B swizzle atom,
 //   the 16-byte chunk c of row r is stored at chunk position (c ^ (r & 7)).
 // The SAME image serves as
@@ -12,6 +12,7 @@
 #pragma once
 #include <cuda_bf16.h>
 #include <cstdint>
+#include "tc_wgmma.cuh"
 
 namespace b200rl { namespace tc {
 
@@ -38,9 +39,8 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
     return ok != 0;
 }
 // Bounded wait: a protocol bug must surface as a launch failure (trap), never as a hung GPU.  The bound is counted on the
-// SM's own cycle counter: reading %globaltimer inside the spin loop (round 1) costs several hundred cycles per poll, which
-// became the period of every tight producer/consumer handshake (stage knock-outs of tc_conv1_wgrad_u8: 850 cycles per step
-// with every stage switched off).
+// SM's own cycle counter: reading %globaltimer inside the spin loop costs several hundred cycles per poll, which would
+// become the period of every tight producer/consumer handshake.
 #ifndef B200RL_WAIT_MODE
 #define B200RL_WAIT_MODE 0
 #endif
@@ -78,97 +78,47 @@ __device__ __forceinline__ void mbar_wait2(uint64_t* bar_a, uint32_t parity_a, u
     if (!b) mbar_wait(bar_b, parity_b);
 }
 
-// 256-bit global store (sm_100: STG.E.ENL2.256): half the store instructions -- and L1 wavefronts -- of two 16-byte stores
-// when every lane writes its own line.  `p` must be 32-byte aligned.
-__device__ __forceinline__ void st_global_256(void* p, const int4& a, const int4& b) {
-    asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(a.x), "r"(a.y), "r"(a.z), "r"(a.w), "r"(b.x),
-                 "r"(b.y), "r"(b.z), "r"(b.w)
-                 : "memory");
+// 32 bytes to global memory as two 16-byte stores
+__device__ __forceinline__ void st_global_32b(void* p, const int4& a, const int4& b) {
+    reinterpret_cast<int4*>(p)[0] = a;
+    reinterpret_cast<int4*>(p)[1] = b;
 }
 
-// one lane of the (converged) warp
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "elect.sync _|p, 0xFFFFFFFF;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}\n"
-        : "=r"(pred));
-    return pred != 0;
-}
-
-// generic-proxy smem writes -> visible to the async proxy (tcgen05.mma operand reads)
+// generic-proxy smem writes -> visible to the async proxy (wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
-// -------------------------------------------------------------------- TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {  // one full warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // same warp
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem]; bf16 inputs, fp32 accumulate; issued by ONE thread
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrive on an mbarrier when all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-
-// TMEM -> registers: this warp's 32 lanes x 16 consecutive fp32 columns
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr));
-}
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive fp32 columns
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-          "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-          "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
 // ------------------------------------------------------------- descriptors
-constexpr uint64_t kDescVersion = 1ull << 46;        // Blackwell descriptor version
-constexpr uint64_t kDescSwizzle128 = 2ull << 61;     // LayoutType::SWIZZLE_128B
+// wgmma shared-memory matrix descriptor: start address >> 4 (bits 0-13), leading byte offset >> 4 (16-29), stride byte
+// offset >> 4 (32-45), base offset 0 (the swizzle is applied to absolute address bits, so a start address shifted by whole
+// rows inside a swizzled image addresses the shifted rows), layout type in bits 62-63.
+constexpr uint64_t kDescSwizzle128 = 1ull << 62;     // SWIZZLE_128B
+constexpr uint64_t kDescSwizzle64 = 2ull << 62;      // SWIZZLE_64B
 
 // K-major SW128 operand: rows (M or N index) 128 B apart, 8-row atoms 1024 B apart (SBO), LBO unused (=1)
 __device__ __forceinline__ uint64_t desc_kmajor(uint32_t smem_addr) {
-    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | kDescVersion | kDescSwizzle128;
+    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | kDescSwizzle128;
 }
 // MN-major SW128 operand: 64-element MN atoms `lbo_bytes` apart, 8-row K groups 1024 B apart (SBO)
 __device__ __forceinline__ uint64_t desc_mnmajor(uint32_t smem_addr, uint32_t lbo_bytes) {
     return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) | (64ull << 32) |
-           kDescVersion | kDescSwizzle128;
+           kDescSwizzle128;
 }
-// instruction descriptor: bf16 x bf16 -> fp32, M x N tile, operand majors (0 = K-major, 1 = MN-major)
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N, int a_mn_major, int b_mn_major) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) |
-           ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+
+// Accumulator hand-off from a warpgroup's 64 x N fp32 fragment (tc_wgmma.cuh) to a row-major shared-memory tile
+// st[64][ld] (ld = N + 4: conflict-free row-wise float4 reads), so that an epilogue thread can own a whole row.
+template <int R>
+__device__ __forceinline__ void stage_acc(float* st, int ld, int wg_tid, const float (&d)[R]) {
+    const int row = ((wg_tid >> 5) << 4) + ((wg_tid & 31) >> 2), col = (wg_tid & 3) * 2;
+#pragma unroll
+    for (int j = 0; j < R / 4; ++j) {
+        *reinterpret_cast<float2*>(st + row * ld + 8 * j + col) = make_float2(d[4 * j], d[4 * j + 1]);
+        *reinterpret_cast<float2*>(st + (row + 8) * ld + 8 * j + col) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+    }
 }
+// named barrier over `n` threads (warpgroups synchronise among themselves without stalling the producer warps)
+__device__ __forceinline__ void named_bar(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 // byte offset of 16-byte chunk `c` of row `r` inside an operand image (rows stacked 128 B apart)
 __device__ __forceinline__ uint32_t img_off(int r, int c) { return (uint32_t)(r * 128 + ((c ^ (r & 7)) << 4)); }

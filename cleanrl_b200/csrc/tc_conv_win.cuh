@@ -1,4 +1,4 @@
-// tcgen05 "window" convolution kernel + launcher (see net_tc.cu for the layer plan).
+// wgmma "window" convolution kernel + launcher (see net_tc.cu for the layer plan).
 #pragma once
 #include "tc_base.cuh"
 
@@ -9,9 +9,8 @@ using namespace tc;
 // Stride-1 convolutions over activations stored as a LINEAR pixel grid [n*G rows, CPR*64 channels]
 // (G = Hp*Wp grid positions per image).  GEMM rows enumerate grid positions, so tap (dy,dx) of a row is
 // simply the row `dy*Wp+dx` further down: the CTA stages ONE window of 128+maxshift rows per tile and
-// every tap is a tcgen05 operand descriptor whose start address is shifted by whole 128-byte rows
-// (the SWIZZLE_128B pattern is a function of the shared-memory address bits, so any row shift is legal:
-// tools/experiments/umma_shift_test.cu).  Each activation row is therefore read from L2 once per tile
+// every tap is a wgmma operand descriptor whose start address is shifted by whole 128-byte rows
+// (the SWIZZLE_128B pattern is a function of the shared-memory address bits, so any row shift is legal).  Each activation row is therefore read from L2 once per tile
 // instead of once per tap, and the producers do no im2col index arithmetic at all.  Grid positions whose
 // window would leave the image (X >= vW or Y >= vH) are computed but not stored.
 enum { WOUT_DENSE = 0, WOUT_S2D2 = 1, WOUT_DACT2 = 2, WOUT_DACT1 = 3 };
@@ -50,29 +49,20 @@ __device__ __forceinline__ uint32_t pack_f16x2_sat(float lo, float hi) {
     return d;
 }
 
-// Thread roles (576 threads): warp 0 = TMA producer; warp 1 = MMA issuer; warps 2-17 = FOUR epilogue groups of four warps
-// (one warp per TMEM lane quadrant).  Group h owns accumulator buffer h and drains tiles h, h + 4, ...
-// Why four groups: an epilogue warp runs a ~250-500 instruction dependent chain per tile (tcgen05.ld, scale/bias, ReLU
-// mask, bf16 packing, stores); with two groups every scheduler held two such warps and ncu showed 0.2-0.4 instructions per
-// cycle and scheduler with the tensor pipe at 25-45 % -- the epilogue's LATENCY was the tile period.  Four warps per scheduler
-// hide it.  Measured and dropped: a second MMA-issuer warp (no gain: the issuing thread is not the limit).
-constexpr int kConvWinThreads = 576;                     // the widest instance (4 groups); see conv_win_groups
-// N = 128 tiles (conv2 data gradient) keep two groups: their epilogue holds 4 x 32 accumulator columns per row and was
-// measured 10 % slower with four groups (register pressure at 576 threads); the narrower kernels gain 0-12 %.
-__host__ __device__ constexpr int conv_win_groups(int BN) { return BN >= 128 ? 2 : 4; }
-__host__ __device__ constexpr int conv_win_threads(int BN) { return 64 + conv_win_groups(BN) * 128; }
-__host__ __device__ constexpr int conv_win_acc_bufs(int BN) { return BN <= 128 ? 4 : 2; }
+// Thread roles (384 threads): warpgroup 0 = TMA producer (warp 0; warps 1-3 only hold the warpgroup alignment that wgmma
+// requires); warpgroups 1 and 2 each run wgmma on 64 rows of every 128-row tile (accumulators in registers), hand the
+// accumulators to a row-major shared-memory tile and run the epilogue with one thread per row (a second thread per row
+// takes the odd 32-column groups).
+constexpr int kConvWinThreads = 384;
+template <int BN>
+__host__ __device__ constexpr size_t conv_win_acc_bytes() { return (size_t)128 * (BN + 4) * sizeof(float); }
 template <int BN, int CPR, int STAGES, int NTAPS>
-__global__ void __launch_bounds__(conv_win_threads(BN), 1) tc_conv_win(const __grid_constant__ CUtensorMap tmA, const WinParams p,
-                                                      int total_tiles) {
+__global__ void __launch_bounds__(kConvWinThreads, 1) tc_conv_win(const __grid_constant__ CUtensorMap tmA, const WinParams p,
+                                                                  int total_tiles) {
     constexpr int B_CHUNK = BN * 128;
-    constexpr int NB = conv_win_acc_bufs(BN);
-    constexpr int NG = conv_win_groups(BN);
-    static_assert(NB % NG == 0, "every epilogue group owns NB / NG accumulator buffers");
-    constexpr uint32_t TMEM_COLS = (NB * BN) < 32 ? 32 : NB * BN;
+    constexpr int LDA = BN + 4;                          // fp32 accumulator tile row pitch (conflict-free row reads)
     extern __shared__ uint8_t smem_raw[];
-    __shared__ uint64_t full_bar[STAGES], empty_bar[STAGES], tfull_bar[NB], tempty_bar[NB];
-    __shared__ uint32_t tmem_base_smem;
+    __shared__ uint64_t full_bar[STAGES], empty_bar[STAGES];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     const int tid = threadIdx.x, warp = tid >> 5;
     const int nchunks = p.ntaps * CPR;
@@ -81,14 +71,13 @@ __global__ void __launch_bounds__(conv_win_threads(BN), 1) tc_conv_win(const __g
     const int STAGE_BYTES = IMG * CPR;
     uint8_t* sW = smem;
     uint8_t* sRing = smem + (size_t)nchunks * B_CHUNK;
+    float* sAcc = reinterpret_cast<float*>(sRing + (size_t)STAGES * STAGE_BYTES);
 
     if (tid == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        for (int a = 0; a < NB; ++a) { mbar_init(&tfull_bar[a], 1); mbar_init(&tempty_bar[a], 4); }
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }   // 8 consumer warps
         fence_barrier_init();
         tma_prefetch_desc(&tmA);
     }
-    if (warp == 1) tmem_alloc(&tmem_base_smem, TMEM_COLS);
     for (int idx = tid; idx < nchunks * BN * 8; idx += blockDim.x) {
         const int c16 = idx & 7;
         int t = idx >> 3;
@@ -98,10 +87,7 @@ __global__ void __launch_bounds__(conv_win_threads(BN), 1) tc_conv_win(const __g
         *reinterpret_cast<int4*>(sW + (size_t)j * B_CHUNK + img_off(r, c16)) = v;
     }
     fence_proxy_async_smem();
-    tc_fence_before_sync();
     __syncthreads();
-    tc_fence_after_sync();
-    const uint32_t tmem_d = tmem_base_smem;
     // each CTA walks a CONTIGUOUS range of tiles: with the minibatch gather every image (3-4 tiles) is then
     // touched by one SM only (TLB / L2 locality), and the image indices of tile+1 can be prefetched
     const int tile_begin = (int)(((int64_t)total_tiles * blockIdx.x) / gridDim.x);
@@ -138,68 +124,47 @@ __global__ void __launch_bounds__(conv_win_threads(BN), 1) tc_conv_win(const __g
                 }
             }
         }
-    } else if (warp == 1) {
-        // ======================= MMA issuer: the WHOLE warp walks the tile loop (uniform control flow keeps the
-        // descriptor arithmetic in uniform registers), one elected lane issues.  Descriptors differ from a per-stage /
-        // per-tap base only in their 14-bit start-address field, so each MMA costs two 32-bit adds.
-        const bool leader = elect_one();
-        constexpr uint32_t idesc = make_idesc(128, BN, 0, 0);
-        const uint64_t desc_hi = desc_kmajor(0) & 0xFFFFFFFF00000000ull;
-        const uint32_t desc_lo_flags = (uint32_t)(desc_kmajor(0) & 0xFFFFFFFFull);       // LBO field
-        const uint32_t w_lo = ((smem_u32(sW) & 0x3FFFFu) >> 4) | desc_lo_flags;
-        for (uint32_t q = 0; (int)q < tile_end - tile_begin; ++q) {
-            const uint32_t acc = q % NB, s = q % STAGES;
-            if (q >= (uint32_t)NB) mbar_wait(&tempty_bar[acc], ((q / NB) - 1) & 1);
-            mbar_wait(&full_bar[s], (q / STAGES) & 1);
-            tc_fence_after_sync();
-            if (leader) {
-                const uint32_t d_addr = tmem_d + acc * BN;
-                const uint32_t win_lo = ((smem_u32(sRing + (size_t)s * STAGE_BYTES) & 0x3FFFFu) >> 4) | desc_lo_flags;
-#pragma unroll
-                for (int t = 0; t < NTAPS; ++t) {
-#pragma unroll
-                    for (int c = 0; c < CPR; ++c) {
-                        const uint32_t a_lo = win_lo + (uint32_t)((c * IMG) >> 4) + (uint32_t)p.shift[t] * 8u;
-                        const uint32_t b_lo = w_lo + (uint32_t)(((t * CPR + c) * B_CHUNK) >> 4);
-#pragma unroll
-                        for (int kk = 0; kk < 4; ++kk)
-                            umma_bf16(d_addr, desc_hi | (uint64_t)(a_lo + 2 * kk), desc_hi | (uint64_t)(b_lo + 2 * kk), idesc,
-                                      (t | c | kk) != 0 ? 1u : 0u);
-                    }
-                }
-                umma_commit(&empty_bar[s]);
-                umma_commit(&tfull_bar[acc]);
-            }
-            __syncwarp();
-        }
-    } else {
-        // ======================= epilogue: warps 2-17 = two groups of four (one warp per TMEM lane quadrant).
-        // Group h owns accumulator buffer h, i.e. every other tile of the CTA's range, and handles ALL BN columns
-        // of its rows: the row -> (image, Y, X) -> output offset arithmetic is paid once per tile and thread, and
-        // is incremental (a tile step is 256 grid rows; Y = rem / Wp by multiply-shift, exact for G*Wp < 65536).
-        const int ew = warp & 3;
-        const int h = (warp - 2) >> 2;                       // epilogue group 0..3
-        const int lrow = ew * 32 + (tid & 31);
+    } else if (warp >= 4) {
+        // ======================= consumer warpgroup wg: rows 64 wg .. 64 wg + 63 of every tile.  Every tap is a descriptor
+        // of the staged window whose start address is shifted by whole 128-byte rows.
+        const int wg = (warp - 4) >> 2, wt = tid & 127;
+        float* st = sAcc + wg * 64 * LDA;
+        const uint32_t w_base = smem_u32(sW);
+        const int lr = wt & 63, half = wt >> 6;
+        const int lrow = wg * 64 + lr;
         const uint32_t mW = (65536u + (uint32_t)p.Wp - 1u) / (uint32_t)p.Wp;
-        constexpr int TSTEP = NG * 128;                      // grid rows between two tiles of one group
-        const int step_i = TSTEP / p.G, step_rem = TSTEP % p.G;
-        int64_t r = ((int64_t)tile_begin + h) * 128 + lrow;      // linear-grid mode state (unused when image-aligned)
-        int i_lin = (int)(r / p.G);
-        int rem_lin = (int)(r - (int64_t)i_lin * p.G);
         const int tmask = (1 << p.tpi_shift) - 1;
-        const uint32_t lane_base = tmem_d + ((uint32_t)(ew * 32) << 16);
         constexpr int NW = BN / 32;                          // 32-column groups = mask words per row
-        uint32_t k = 0;                                      // tiles this group has drained
-        for (int tile = tile_begin + h; tile < tile_end; tile += NG, ++k) {
-            const uint32_t acc = (uint32_t)(tile - tile_begin) % NB;           // group h drains buffers h, h + NG, ...
-            const uint32_t lane_addr = lane_base + acc * BN;
-            int i = i_lin, rem = rem_lin;
+        float d[BN / 2];
+#pragma unroll
+        for (int e = 0; e < BN / 2; ++e) d[e] = 0.f;
+        for (int tile = tile_begin; tile < tile_end; ++tile) {
+            const uint32_t q = (uint32_t)(tile - tile_begin), s = q % STAGES;
+            // the row -> (image, Y, X) -> output offset arithmetic, done while the tile's MMAs run
+            const int64_t r = (int64_t)tile * 128 + lrow;
+            int i = (int)(r / p.G);
+            int rem = (int)(r - (int64_t)i * p.G);
             bool inside = r < p.M;
             if (p.tpi_shift) {                               // image-aligned tiles: rows >= G of an image are padding
                 i = tile >> p.tpi_shift;
                 rem = ((tile & tmask) << 7) + lrow;
                 inside = rem < p.G;
             }
+            mbar_wait(&full_bar[s], (q / STAGES) & 1);
+            wgmma_fence();
+            const uint32_t win = smem_u32(sRing + (size_t)s * STAGE_BYTES) + (uint32_t)(wg * 64 * 128);
+#pragma unroll
+            for (int t = 0; t < NTAPS; ++t) {
+#pragma unroll
+                for (int c = 0; c < CPR; ++c) {
+                    const uint64_t a = desc_kmajor(win + (uint32_t)(c * IMG) + (uint32_t)p.shift[t] * 128u);
+                    const uint64_t b = desc_kmajor(w_base + (uint32_t)((t * CPR + c) * B_CHUNK));
+#pragma unroll
+                    for (int kk = 0; kk < 4; ++kk)
+                        WgmmaBf16<BN, 0, 0>::mma(d, a + 2 * kk, b + 2 * kk, (t | c | kk) != 0 ? 1u : 0u);
+                }
+            }
+            wgmma_commit();
             const int Y = (int)(((uint32_t)rem * mW) >> 16), X = rem - Y * p.Wp;
             const bool valid = inside && (Y < p.vH) && (X < p.vW);
             int64_t o1 = 0, o2 = 0, ob = 0;
@@ -232,19 +197,23 @@ __global__ void __launch_bounds__(conv_win_threads(BN), 1) tc_conv_win(const __g
                     mb[0] = __ldg(p.mask_bits + ob);
                 }
             }
-            mbar_wait(&tfull_bar[acc], ((uint32_t)(tile - tile_begin) / NB) & 1);
-            tc_fence_after_sync();
+            wgmma_wait<0>();
+            wgmma_fence_operands(d);
+            if ((tid & 31) == 0) mbar_arrive(&empty_bar[s]);              // this warp's operand reads are complete
+            named_bar(1 + wg, 128);                                         // the previous tile's rows have been read
+            stage_acc(st, LDA, wt, d);
+            named_bar(1 + wg, 128);
 #pragma unroll
             for (int g = 0; g < NW; ++g) {
-                uint32_t v[32];
-                tmem_ld32(lane_addr + g * 32, v);
-                tmem_ld_wait();
-                if (g == NW - 1) {             // accumulator drained: hand the buffer back before the global stores
-                    tc_fence_before_sync();
-                    __syncwarp();
-                    if ((tid & 31) == 0) mbar_arrive(&tempty_bar[acc]);
-                }
+                if ((g & 1) != half) continue;
                 if (!valid || g * 32 >= p.N) continue;
+                uint32_t v[32];
+#pragma unroll
+                for (int e = 0; e < 8; ++e) {
+                    const float4 f = *reinterpret_cast<const float4*>(st + lr * LDA + g * 32 + 4 * e);
+                    v[4 * e] = __float_as_uint(f.x); v[4 * e + 1] = __float_as_uint(f.y);
+                    v[4 * e + 2] = __float_as_uint(f.z); v[4 * e + 3] = __float_as_uint(f.w);
+                }
                 if (p.bias) {
                     const float4* bp = reinterpret_cast<const float4*>(p.bias + g * 32);
 #pragma unroll
@@ -298,12 +267,7 @@ __global__ void __launch_bounds__(conv_win_threads(BN), 1) tc_conv_win(const __g
                     w[e].w = (int)pack_bf16x2(__uint_as_float(v[8 * e + 6]), __uint_as_float(v[8 * e + 7]));
                 }
                 }
-                // Stores: a lane owns one output row, so every store instruction of the warp touches 32 different lines = 32 L1
-                // wavefronts; on the N = 128 conv2 data gradient they were ~70 % of the tile period.  256-bit stores halve
-                // the instructions (conv2 data gradient 338 -> 288 us, conv3 data gradient 308 -> 256, conv2 forward -5 %).
-                // Measured against it: coalescing through a shared-memory tile (4 or 8 lanes per row) -- conv3 data gradient 263,
-                // conv2 forward equal, conv3 forward +5 %, conv2 data gradient +18..23 % (extra warp syncs in a latency-bound
-                // epilogue) -- so the direct form stays.
+                // a thread owns one output row: 64 contiguous bytes per 32-column group
                 bf16* dst;
                 if (p.out_mode == WOUT_DACT1) {
                     // column group g = (py,px) of the cell -> input pixel (2Y+py, 2X+px) of the 21-grid, 32 channels
@@ -311,27 +275,22 @@ __global__ void __launch_bounds__(conv_win_threads(BN), 1) tc_conv_win(const __g
                 } else {
                     dst = p.out + o1 + g * 32;
                 }
-                st_global_256(dst, w[0], w[1]);
-                st_global_256(dst + 16, w[2], w[3]);
+                st_global_32b(dst, w[0], w[1]);
+                st_global_32b(dst + 16, w[2], w[3]);
                 if (p.out_mode == WOUT_DACT2) {
                     bf16* dst2 = p.out2 + o2 + g * 32;
-                    st_global_256(dst2, w[0], w[1]);
-                    st_global_256(dst2 + 16, w[2], w[3]);
+                    st_global_32b(dst2, w[0], w[1]);
+                    st_global_32b(dst2 + 16, w[2], w[3]);
                 }
             }
-            r += TSTEP; i_lin += step_i; rem_lin += step_rem;
-            if (rem_lin >= p.G) { rem_lin -= p.G; ++i_lin; }
         }
     }
-    tc_fence_before_sync();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_d, TMEM_COLS);
 }
 
 template <int BN, int CPR, int STAGES, int NTAPS>
 static int launch_conv_win(const WinParams& p, cudaStream_t s, const char* what) {
     if (p.ntaps != NTAPS) return fail(B200RL_ERR_INVALID_ARGUMENT, "%s: %d taps, kernel instance has %d", what, p.ntaps, NTAPS);
-    const size_t smem = (size_t)p.ntaps * CPR * BN * 128 + (size_t)STAGES * p.WR * 128 * CPR + 1024;
+    const size_t smem = (size_t)p.ntaps * CPR * BN * 128 + (size_t)STAGES * p.WR * 128 * CPR + conv_win_acc_bytes<BN>() + 1024;
     static SmemAttrCache attr;
     if (int rc = attr.ensure(tc_conv_win<BN, CPR, STAGES, NTAPS>, smem, what)) return rc;
     if ((int64_t)p.G * p.Wp >= 65536 || p.G < 1 || p.N % 32 != 0)
@@ -348,7 +307,7 @@ static int launch_conv_win(const WinParams& p, cudaStream_t s, const char* what)
     if (p.tpi_shift) rc = make_tmap_3d(&tmA, p.A, p.n_images, p.G, (int64_t)CPR * 64, p.WR, what);
     else rc = make_tmap_2d(&tmA, p.A, p.M, (int64_t)CPR * 64, p.WR, what);
     if (rc) return rc;
-    tc_conv_win<BN, CPR, STAGES, NTAPS><<<grid, conv_win_threads(BN), smem, s>>>(tmA, p, total);
+    tc_conv_win<BN, CPR, STAGES, NTAPS><<<grid, kConvWinThreads, smem, s>>>(tmA, p, total);
     return check_launch(what);
 }
 

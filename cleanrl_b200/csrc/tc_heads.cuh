@@ -9,7 +9,7 @@ using namespace tc;
 // ------------------------------------------------------------------ policy/value heads (tiny: CUDA cores, fp32 math)
 // A1 = A + 1 head outputs (logits | value), 1 <= A1 <= kMaxHeads.  Head weights live in dynamic shared memory.
 constexpr int kMaxHeads = 24;              // (A+1) * 2 KB of head weights must fit the 48 KB default dynamic shared memory
-constexpr int kHeadsPartialBlocks = 296;     // row blocks of the head weight gradient (x2 row lanes = partial slabs)
+constexpr int kHeadsPartialBlocks = 264;     // 2 x 132 SMs: row blocks of the head weight gradient (x2 row lanes = partial slabs)
 // rows per block of tc_heads_bwd_weight: its dhead rows are staged in (static-limit) shared memory, <= 256 x 32 floats
 static inline int64_t heads_rows_per_block(int64_t n) {
     int64_t rpb = (n + kHeadsPartialBlocks - 1) / kHeadsPartialBlocks;

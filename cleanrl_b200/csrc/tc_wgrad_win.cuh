@@ -1,4 +1,4 @@
-// tcgen05 window weight-gradient kernel (conv layers).
+// wgmma window weight-gradient kernel (conv layers).
 #pragma once
 #include "tc_base.cuh"
 
@@ -10,7 +10,7 @@ using namespace tc;
 // SAME linear grid (dY is zero at positions that are not valid outputs).  Per step of 128 rows the CTA
 // stages one X window (128 + max shift rows) and 128 dY rows; every tap is an MN-major descriptor shifted by
 // whole rows.  Output tile t pairs the 64-channel chunks slot[2t], slot[2t+1].
-constexpr int kWgradWinStages = 3;       // stage = X window (<= 37 KB) + 16 KB of dY rows; 3 stages keep conv1 at 2 CTAs per SM (4 were measured 40 % slower)
+constexpr int kWgradWinStages = 3;       // stage = X window (<= 37 KB) + 16 KB of dY rows
 struct WGradWinParams {
     const bf16* X; const int64_t* rows; int64_t M; int n, G;
     int tpi_shift;           // > 0: image-aligned steps (2^tpi_shift steps of 128 rows per image, M = n << (7 + tpi_shift))
@@ -26,39 +26,34 @@ struct WGradWinParams {
     float* wsb;              // [gridDim.x][64] bias-gradient partials: sum_r dY[r, co]
 };
 
-// 224 threads: warps 0-3 = dY warps (bias sums, final TMEM drain), warps 4 and 6 = MMA issuers (output tiles of even /
-// odd index: independent accumulators, see tc_conv_win.cuh for why one issuing thread is not enough), warp 5 = TMA.
-constexpr int kWgradWinThreads = 224;
-constexpr int kWgradWinIssuers = 1;      // 2 = warps 4 and 6 issue alternate output tiles; measured: no gain (shared-memory operand bound)
+// 512 threads: warps 0-3 = dY warps (bias sums; in image-aligned mode they also stage dY with cp.async), warp 4 = TMA
+// producer (warps 5-7 only keep the consumers warpgroup-aligned), warpgroups 2 and 3 = wgmma: warpgroup w accumulates slot
+// 2 t + w of every output tile t this CTA owns.  A CTA owns at most kWgradWinTilesPerCta output tiles (64 accumulator
+// registers per thread); blockIdx.y selects them, so the slots of one row split are spread over gridDim.y CTAs.
+constexpr int kWgradWinThreads = 512;
+constexpr int kWgradWinTilesPerCta = 2;
 __global__ void __launch_bounds__(kWgradWinThreads, 1) tc_wgrad_win(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmY,
                                                        const WGradWinParams p, int use_tma) {
-    constexpr int R = 128, STAGES = kWgradWinStages, LOOKAHEAD = 1, NY = 64;
+    constexpr int R = 128, STAGES = kWgradWinStages, LOOKAHEAD = 1, NY = 64, TT = kWgradWinTilesPerCta;
     extern __shared__ uint8_t smem_raw[];
-    __shared__ uint64_t full_bar[STAGES], empty_bar[STAGES], done_bar;
-    __shared__ uint32_t tmem_base_smem;
+    __shared__ uint64_t full_bar[STAGES], empty_bar[STAGES];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     const int tid = threadIdx.x, warp = tid >> 5;
     const int IMGX = p.WRX * 128;
     const int XBYTES = IMGX * p.cpr;
     const int stage_bytes = XBYTES + R * 128;
     const int xt = p.nslots / 2;
-    uint32_t tmem_cols = 32;
-    while ((int)tmem_cols < xt * NY) tmem_cols <<= 1;
+    const int t0 = blockIdx.y * TT;                       // first output tile of this CTA
     float* sRed = reinterpret_cast<float*>(smem + (size_t)STAGES * stage_bytes);     // [16][64] bias partials (4 KB)
     if (tid == 0) {
         // full:  one expect_tx arrival (TMA) [+ the four cp.async warps that stage dY in image-aligned mode]
-        // empty: the MMA commit [+ the four dY-summing warps when they read the stage after the TMA landed]
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], use_tma ? 1 : 5); mbar_init(&empty_bar[s], (use_tma ? 4 : 0) + kWgradWinIssuers); }
-        mbar_init(&done_bar, kWgradWinIssuers);
+        // empty: the eight wgmma warps [+ the four dY-summing warps when they read the stage after the TMA landed]
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], use_tma ? 1 : 5); mbar_init(&empty_bar[s], (use_tma ? 4 : 0) + 8); }
         fence_barrier_init();
         tma_prefetch_desc(&tmX);
         if (use_tma) tma_prefetch_desc(&tmY);
     }
-    if (warp == 4) tmem_alloc(&tmem_base_smem, tmem_cols);
-    tc_fence_before_sync();
     __syncthreads();
-    tc_fence_after_sync();
-    const uint32_t tmem_d = tmem_base_smem;
     const int64_t m_begin = (int64_t)blockIdx.x * p.rows_per_cta;
     int64_t m_end = m_begin + p.rows_per_cta;
     if (m_end > p.M) m_end = p.M;
@@ -66,7 +61,7 @@ __global__ void __launch_bounds__(kWgradWinThreads, 1) tc_wgrad_win(const __grid
     const int tmask = (1 << p.tpi_shift) - 1;
     const int64_t g0 = m_begin / R;                       // first global step of this CTA (image-aligned mode)
 
-    if (warp == 5) {
+    if (warp == 4) {
         // ======================= TMA producer (one lane): X window [+ dY rows when they are 128 bytes wide] =========
         if ((tid & 31) == 0) {
             int z_next = 0;
@@ -169,83 +164,54 @@ __global__ void __launch_bounds__(kWgradWinThreads, 1) tc_wgrad_win(const __grid
             float t = 0.f;
 #pragma unroll
             for (int l = 0; l < 16; ++l) t += sRed[l * 64 + tid];
-            p.wsb[(int64_t)blockIdx.x * NY + tid] = t;
+            if (blockIdx.y == 0) p.wsb[(int64_t)blockIdx.x * NY + tid] = t;
         }
-    } else {
-        // ======================= MMA issuers (warps 4 and 6): the whole warp walks the step loop (uniform control flow),
-        // one elected lane issues the output tiles of its parity.  Everything that does not depend on the stage is hoisted: per output tile the X operand's offset
-        // inside the stage and its LBO field; descriptors then differ only in the 14-bit start-address field.
-        const bool leader = elect_one();
-        const int ih = warp == 4 ? 0 : 1;
-        if (ih < kWgradWinIssuers) {
-        constexpr uint32_t idesc = make_idesc(128, NY, 1, 1);
-        const uint64_t desc_hi = desc_mnmajor(0, 0) & 0xFFFFFFFF00000000ull;
-        uint32_t arel[8], albo[8];
+    } else if (warp >= 8) {
+        // ======================= wgmma warpgroups: X slot (MN-major, rows = reduction index, shifted by whole rows per tap)
+        // x dY rows (MN-major); 8 K-steps of 16 rows per step
+        const int w = (warp - 8) >> 2, wt = tid & 127;
+        uint32_t arel[TT];
 #pragma unroll
-        for (int t = 0; t < 8; ++t) {
-            arel[t] = 0; albo[t] = 0;
-            if (t < xt) {
-                const uint32_t r0 = (uint32_t)(p.slot_cc[2 * t] * IMGX + p.shift[p.slot_tap[2 * t]] * 128);
-                const uint32_t r1 = (uint32_t)(p.slot_cc[2 * t + 1] * IMGX + p.shift[p.slot_tap[2 * t + 1]] * 128);
-                arel[t] = r0 >> 4;
-                albo[t] = (((r1 - r0) >> 4) & 0x3FFFu) << 16;
-            }
+        for (int tt = 0; tt < TT; ++tt) {
+            const int slot = 2 * (t0 + tt) + w;
+            arel[tt] = t0 + tt < xt ? (uint32_t)(p.slot_cc[slot] * IMGX + p.shift[p.slot_tap[slot]] * 128) : 0u;
         }
-        const uint32_t ylbo = (uint32_t)(((R * 128) >> 4) & 0x3FFF) << 16;
+        float d[TT][NY / 2];
+#pragma unroll
+        for (int tt = 0; tt < TT; ++tt)
+#pragma unroll
+            for (int e = 0; e < NY / 2; ++e) d[tt][e] = 0.f;
         for (int it = 0; it < nsteps; ++it) {
             const int s = it % STAGES;
             mbar_wait(&full_bar[s], (it / STAGES) & 1);
-            tc_fence_after_sync();
-            if (leader) {
-                const uint32_t xa = smem_u32(smem + (size_t)s * stage_bytes);
-                const uint32_t xa16 = (xa & 0x3FFFFu) >> 4, ya16 = (((xa + XBYTES) & 0x3FFFFu) >> 4) | ylbo;
-                const uint32_t accum = it != 0 ? 1u : 0u;
+            wgmma_fence();
+            const uint32_t xa = smem_u32(smem + (size_t)s * stage_bytes), ya = xa + XBYTES;
 #pragma unroll
-                for (int t = 0; t < 8; ++t) {
-                    if (t < xt && (kWgradWinIssuers == 1 || (t & 1) == ih)) {
-                        const uint32_t a_lo = (xa16 + arel[t]) | albo[t];
+            for (int tt = 0; tt < TT; ++tt) {
+                if (t0 + tt >= xt) continue;
 #pragma unroll
-                        for (int kk = 0; kk < R / 16; ++kk)
-                            umma_bf16(tmem_d + t * NY, desc_hi | (uint64_t)(a_lo + kk * 128), desc_hi | (uint64_t)(ya16 + kk * 128),
-                                      idesc, kk != 0 ? 1u : accum);
-                    }
-                }
-                umma_commit(&empty_bar[s]);
+                for (int kk = 0; kk < R / 16; ++kk)
+                    WgmmaBf16<NY, 1, 1>::mma(d[tt], desc_mnmajor(xa + arel[tt] + kk * 2048, 0), desc_mnmajor(ya + kk * 2048, 0),
+                                             (it | kk) != 0 ? 1u : 0u);
             }
-            __syncwarp();
+            wgmma_commit();
+            wgmma_wait<0>();
+            if ((tid & 31) == 0) mbar_arrive(&empty_bar[s]);
         }
-        if (leader) umma_commit(&done_bar);
-        __syncwarp();
-        }
-    }
-    if (warp < 4) {
-        if (nsteps > 0) {
-            mbar_wait(&done_bar, 0);
-            tc_fence_after_sync();
-        }
+        const int row = ((wt >> 5) << 4) + ((wt & 31) >> 2), col = (wt & 3) * 2;
         float* wsb = p.ws + (int64_t)blockIdx.x * (p.nslots * 64) * NY;
-        const uint32_t lane_addr = tmem_d + ((uint32_t)(warp * 32) << 16);
-        for (int t = 0; t < xt; ++t) {
-            float* dst = wsb + (int64_t)(t * 128 + tid) * NY;
-            for (int c0 = 0; c0 < NY; c0 += 16) {
-                uint32_t v[16];
-                if (nsteps > 0) {
-                    tmem_ld16(lane_addr + t * NY + c0, v);
-                    tmem_ld_wait();
-                } else {
 #pragma unroll
-                    for (int e = 0; e < 16; ++e) v[e] = 0u;
-                }
+        for (int tt = 0; tt < TT; ++tt) {
+            if (t0 + tt >= xt) continue;
+            wgmma_fence_operands(d[tt]);
+            float* d0 = wsb + (int64_t)((2 * (t0 + tt) + w) * 64 + row) * NY + col;
 #pragma unroll
-                for (int e = 0; e < 16; e += 4)
-                    *reinterpret_cast<float4*>(dst + c0 + e) = make_float4(__uint_as_float(v[e]), __uint_as_float(v[e + 1]),
-                                                                             __uint_as_float(v[e + 2]), __uint_as_float(v[e + 3]));
+            for (int j = 0; j < NY / 8; ++j) {
+                *reinterpret_cast<float2*>(d0 + 8 * j) = make_float2(d[tt][4 * j], d[tt][4 * j + 1]);
+                *reinterpret_cast<float2*>(d0 + 8 * NY + 8 * j) = make_float2(d[tt][4 * j + 2], d[tt][4 * j + 3]);
             }
         }
     }
-    tc_fence_before_sync();
-    __syncthreads();
-    if (warp == 4) tmem_dealloc(tmem_d, tmem_cols);
 }
 
 }  // namespace b200rl

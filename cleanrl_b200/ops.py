@@ -445,7 +445,7 @@ def lstm_cell_bwd(dh_heads, dh_rec_raw, done_next, dc_rec, save, c_masked, done,
     _lib.check(rc, "lstm_cell_bwd")
 
 
-# ------------------------------------------------------ NatureCNN bf16 (tcgen05) plan
+# ------------------------------------------------------ NatureCNN bf16 (wgmma) plan
 class NatureCNNBf16:
     """Owns the packed bf16 weights and activation workspaces of the tensor-core NatureCNN path."""
 

@@ -1,4 +1,4 @@
-"""Drop-in for cleanrl/ppo_atari_envpool.py on the B200-native PPO engine.
+"""Drop-in for cleanrl/ppo_atari_envpool.py on the H100-native PPO engine.
 
 Same CLI flags (``Args``), same ``Agent`` surface / ``state_dict`` keys, same
 TensorBoard tags and stdout lines as the reference script

@@ -1,4 +1,4 @@
-"""B200-native PPO iteration engine: rollout storage, policy step, GAE, minibatch update.
+"""H100-native PPO iteration engine: rollout storage, policy step, GAE, minibatch update.
 
 This is the loop body of the reference scripts (cleanrl/ppo.py:185-310 and its
 twins in ppo_atari_envpool.py / ppo_atari_multigpu.py) re-designed around
@@ -162,9 +162,10 @@ class PPOEngine:
         # frame-stack delta upload (grouped loop, uint8 rollout): only the newest frame plane of every env crosses PCIe, the
         # device rebuilds slot t from slot t-1, a host worker pool verifies the shifted-stack property (csrc/frame_stack.cu)
         # Default: on for a single process per host, off when several ranks share the host (LOCAL_WORLD_SIZE > 1): the
-        # verification and the leaner launch path make the rollout HOST-bound instead of PCIe-bound, which wins on an idle host
-        # (1.39 M vs 1.03 M env-steps/s) and loses when the ranks' worker pools compete for the same cores and memory
-        # bandwidth (profiles/r2_host_sensitivity.md).  CLEANRL_B200_DELTA_UPLOAD=1 / 0 overrides either way.
+        # verification and the leaner launch path make the rollout HOST-bound instead of PCIe-bound, so which path is faster
+        # depends on the host's free cores and memory bandwidth; with several ranks the worker pools compete for them.  On the
+        # H100 host of README.md whole uploads were the faster single-process path (0.63-0.65 M vs 0.47-0.50 M env-steps/s,
+        # bench.py `e2e_whole_upload` vs `e2e`).  CLEANRL_B200_DELTA_UPLOAD=1 / 0 overrides either way.
         want_delta = os.environ.get("CLEANRL_B200_DELTA_UPLOAD")
         if want_delta is None:
             want_delta = "1" if int(os.environ.get("LOCAL_WORLD_SIZE", "1") or 1) <= 1 else "0"
@@ -736,7 +737,7 @@ class PPOEngine:
             self.hyper.copy_(self.hyper_h, non_blocking=True)
         for epoch in range(E):
             # numpy global RNG, in-place and cumulative across epochs as the reference (ppo.py:245).  A shuffle of 131 072
-            # indices costs the host 1.5-3 ms: it is drawn per epoch, right before that epoch's launches, so that every
+            # indices costs the host milliseconds: it is drawn per epoch, right before that epoch's launches, so that every
             # shuffle but the first runs while the device is still busy with the previous epoch's minibatches.
             t_sh = time.perf_counter()
             self._shuffle(b_inds_np)
@@ -835,7 +836,7 @@ class PPOEngine:
         folded into clip+Adam).  Reference: cat + all_reduce + 12 copy-backs after the whole backward
         (ppo_atari_multigpu.py:360-374).  Here the fc + head gradients -- 95 % of the vector, finished first by the
         hand-written backward -- start their all-reduce on a side stream as soon as the kernel that completes them has
-        run, underneath the ~2 ms of convolution backward; only the 78 k conv gradients are exchanged after the
+        run, underneath the convolution backward; only the 78 k conv gradients are exchanged after the
         backward.  Both parts are elementwise sums of disjoint slices: same result as one all-reduce."""
         flat = self.flat
         tail = self.agent.grad_tail() if (self.overlap_exchange and hasattr(self.agent, "grad_tail")) else None

@@ -4,7 +4,7 @@ Replaces the host-side numpy ``ReplayBuffer`` of cleanrl_utils/buffers.py:250-43
 (``optimize_memory_usage=True``: one uint8 frame ring, ``next_obs`` = slot ``(i+1) % size``, buffers.py:359-362,
 :402).  Differences in mechanism, not in semantics:
 
-* the ring lives in HBM (1 M x 28 224 B = 28 GB fits a 180 GB B200); ``add`` uploads the two 28 KB frames;
+* the ring lives in HBM (1 M x 28 224 B = 28 GB fits an 80 GB H100); ``add`` uploads the two 28 KB frames;
 * ``sample`` draws the SAME index stream from numpy's global RNG (buffers.py:390-399: ``randint(1, size) + pos``
   when full, ``randint(0, pos)`` otherwise, then ``randint(0, n_envs)``) but returns ROW INDICES into the ring:
   the network kernels gather the frames themselves (no 2 x 231 MB host fancy-index + H2D per batch of 8192).

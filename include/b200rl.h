@@ -1,5 +1,5 @@
 /*
- * b200rl.h -- C-ABI of libb200rl.so: the B200-native (sm_100a) PPO hot path.
+ * b200rl.h -- C-ABI of libb200rl.so: the H100-native (sm_90a) PPO hot path.
  *
  * The reference (vwxyzjn/cleanrl) is pure Python/PyTorch and has NO native
  * interface; this header is the boundary SURVEY.md section 8(b) defines for it.
@@ -42,7 +42,7 @@ typedef enum {
 int b200rl_version(void);
 /* message of the last failing call on this host thread ("" if none) */
 const char* b200rl_last_error(void);
-/* compute capability the kernels were compiled for (100 = sm_100a) */
+/* compute capability the kernels were compiled for (90 = sm_90a) */
 int b200rl_compiled_arch(void);
 
 /* Optional per-kernel timing: when enabled, every kernel launch below is bracketed by CUDA events
@@ -243,7 +243,7 @@ int b200rl_linear_bwd_weight_f32(const float* x, const int64_t* rows, const floa
 /* ------------------------------------------- NatureCNN, bf16 tensor cores ---
  * The throughput path of Agent.network/actor/critic (cleanrl/ppo_atari_envpool.py:123-149):
  * every conv / linear contraction (forward, data-gradient, weight-gradient) is an implicit GEMM
- * on tcgen05.mma with bf16 operands and fp32 accumulation in TMEM, fed by TMA; a minibatch gather
+ * on wgmma with bf16 operands and fp32 accumulation in registers, fed by TMA; a minibatch gather
  * (rows) is the image coordinate of conv1's TMA boxes, nothing is materialised; the two heads
  * (A+1 outputs, 1 <= A <= 23) run in fp32 on CUDA cores.
  *

@@ -49,7 +49,8 @@ def atari_envpool(name, argv, n_iter, script="ppo_atari_envpool.py", gymnasium_k
 def atari_envpool_full(name, argv):
     """The HEADLINE configuration (BASELINE.json configs[1]: num_envs=1024, num_steps=128, minibatch 32 768), one
     iteration of the unmodified cleanrl/ppo_atari_envpool.py on the Breakout-shaped synthetic env.  Integer-valued
-    tensors are stored narrow (actions int8, rewards int8, dones uint8) to keep the fixture at a few MB."""
+    tensors are stored narrow (actions int8, rewards int8, dones uint8), and the returns are not stored: the reference
+    computes them as advantages + values in float32, so that sum reproduces them bit for bit (fixture below 1 MB)."""
     rec, g = run_reference("ppo_atari_envpool.py", argv, atari_mode="fresh", gymnasium_kind="atari")
     assert len(rec.iterations) == 1
     it = rec.iterations[0]
@@ -58,7 +59,8 @@ def atari_envpool_full(name, argv):
     out["actions"] = it["actions"].astype(np.int8)[None]
     out["rewards"] = it["rewards"].astype(np.int8)[None]
     out["dones"] = it["dones"].astype(np.uint8)[None]
-    for k in ("logprobs", "values", "advantages", "returns", "next_value", "next_done", "param_sums", "param_abs_sums"):
+    assert np.array_equal(it["returns"], (it["advantages"] + it["values"]).astype(np.float32))
+    for k in ("logprobs", "values", "advantages", "next_value", "next_done", "param_sums", "param_abs_sums"):
         out[k] = it[k][None]
     for k in ("pg_loss", "v_loss", "entropy_loss", "old_approx_kl", "approx_kl", "loss", "clipfrac", "lr",
               "grad_norm_postclip"):
@@ -148,9 +150,89 @@ def dqn(name, argv):
     print("wrote", name, len(losses), "updates")
 
 
+# scripts whose command-line surface (Args fields: default + help text) and module-level names the drop-ins mirror
+SURFACE_SCRIPTS = ["ppo.py", "ppo_atari.py", "ppo_atari_envpool.py", "ppo_atari_multigpu.py", "ppo_continuous_action.py",
+                   "dqn_atari.py", "ppo_procgen.py", "ppo_atari_lstm.py"]
+
+
+def reference_surface(name):
+    """Per reference script: every field of its Args dataclass (default, or "<expr>" where the default is not a literal,
+    and the help string) and every top-level class / function name."""
+    import ast
+    import json
+    from oracle.ref_harness import REFERENCE_ROOT
+    out = {}
+    for script in SURFACE_SCRIPTS:
+        tree = ast.parse((REFERENCE_ROOT / "cleanrl" / script).read_text())
+        cls = next(n for n in tree.body if isinstance(n, ast.ClassDef) and n.name == "Args")
+        fields = []
+        for i, node in enumerate(cls.body):
+            if isinstance(node, ast.AnnAssign):
+                try:
+                    default = ast.literal_eval(node.value)
+                except Exception:
+                    default = "<expr>"
+                doc = None
+                if i + 1 < len(cls.body) and isinstance(cls.body[i + 1], ast.Expr) and isinstance(cls.body[i + 1].value, ast.Constant):
+                    doc = cls.body[i + 1].value.value
+                fields.append([node.target.id, default, doc])
+        names = [n.name for n in tree.body if isinstance(n, (ast.ClassDef, ast.FunctionDef))]
+        out[script] = {"args": fields, "names": names}
+    (OUT / name).write_text(json.dumps(out, indent=1, sort_keys=True) + "\n")
+
+
+def replay_buffer(name):
+    """cleanrl_utils/buffers.py ReplayBuffer (optimize_memory_usage=True, size 50) fed 137 seeded random transitions and
+    sampled (16 rows, np.random.seed(t)) at t = 20, 49, 50, 77, 136, i.e. before and after the ring wraps.  The sampled
+    observations are recorded as indices into the generated frame sequence (frame 0 = first obs, frame t + 1 = the t-th
+    next_obs); actions, rewards and dones as values."""
+    import torch
+    from oracle import stubs
+    from oracle.ref_harness import REFERENCE_ROOT
+    from cleanrl_b200.synthetic_envs import Box, Discrete
+    stubs.install()
+    sys.path.insert(0, str(REFERENCE_ROOT))
+    try:
+        from cleanrl_utils.buffers import ReplayBuffer
+        rng = np.random.default_rng(0)
+        ref = ReplayBuffer(50, Box(0, 255, (4, 84, 84), np.uint8), Discrete(4), "cpu", optimize_memory_usage=True,
+                           handle_timeout_termination=False)
+        frames = [rng.integers(0, 256, (1, 4, 84, 84), dtype=np.uint8)]
+        rec = {}
+        for t in range(137):
+            nxt = rng.integers(0, 256, (1, 4, 84, 84), dtype=np.uint8)
+            a = rng.integers(0, 4, (1,)); r = rng.standard_normal(1).astype(np.float32); d = rng.random(1) < 0.1
+            ref.add(frames[-1], nxt, a, r, d, [{}])
+            frames.append(nxt)
+            if t in (20, 49, 50, 77, 136):
+                st = np.random.get_state()
+                np.random.seed(t)
+                data = ref.sample(16)
+                np.random.set_state(st)
+                seq = torch.from_numpy(np.concatenate(frames))
+
+                def which(o):
+                    return [next(j for j in range(len(seq)) if torch.equal(seq[j], o[i])) for i in range(o.shape[0])]
+                rec[f"t{t}_obs_frame"] = np.array(which(data.observations), dtype=np.int64)
+                rec[f"t{t}_next_obs_frame"] = np.array(which(data.next_observations), dtype=np.int64)
+                rec[f"t{t}_actions"] = data.actions.view(-1).numpy()
+                rec[f"t{t}_rewards"] = data.rewards.view(-1).numpy()
+                rec[f"t{t}_dones"] = data.dones.view(-1).numpy()
+        np.savez_compressed(OUT / name, **rec)
+    finally:
+        sys.path.remove(str(REFERENCE_ROOT))
+        stubs.uninstall()
+        for m in [k for k in sys.modules if k.startswith("cleanrl_utils")]:
+            sys.modules.pop(m)
+
+
 def main():
     OUT.mkdir(parents=True, exist_ok=True)
     only = sys.argv[1:]
+    if not only or "reference_surface" in only:
+        reference_surface("reference_surface.json")
+    if not only or "replay_buffer" in only:
+        replay_buffer("replay_buffer_samples.npz")
     if not only or "ppo_atari_gym" in only:
         atari_envpool("ppo_atari_gym_n8_t32_seed2.npz",
                       ["--no-cuda", "--num-envs", "8", "--num-steps", "32", "--total-timesteps", "512", "--seed", "2"], 2,

@@ -1,4 +1,4 @@
-"""CPU tests: the C-ABI library builds for sm_100a, loads, and exports every symbol
+"""CPU tests: the C-ABI library builds for sm_90a, loads, and exports every symbol
 include/b200rl.h declares; the CLI surface matches the reference; the product has no
 CPU fallback and never imports the oracle."""
 import ctypes
@@ -27,16 +27,16 @@ def test_library_exports_every_declared_symbol(lib):
         assert hasattr(raw, s), f"{s} declared in include/b200rl.h but not exported"
     from cleanrl_b200 import _lib
     assert sorted(_lib.SIGNATURES) == syms, "python binding table out of sync with the header"
-    assert lib.b200rl_compiled_arch() == 100
+    assert lib.b200rl_compiled_arch() == 90
     assert lib.b200rl_version() >= 100
 
 
-def test_library_contains_sm100a_code_only():
+def test_library_contains_sm90a_code_only():
     out = subprocess.run(["cuobjdump", "-lelf", str(ROOT / "cleanrl_b200" / "libb200rl.so")], capture_output=True, text=True)
     if out.returncode != 0:
         pytest.skip("cuobjdump unavailable")
     archs = set(re.findall(r"sm_(\d+a?)", out.stdout))
-    assert archs == {"100a"}, archs
+    assert archs == {"90a"}, archs
 
 
 def test_argument_validation_without_gpu(lib):
@@ -82,7 +82,13 @@ def test_product_never_imports_oracle():
         assert not re.search(r"^\s*(from|import)\s+oracle\b", txt, flags=re.M), f"{p} imports the oracle"
 
 
-@pytest.mark.reference
+def _reference_surface(script):
+    """Args fields and top-level names of the reference script, as recorded from it (oracle/make_golden.py)."""
+    import json
+    from conftest import GOLDEN
+    return json.loads((GOLDEN / "reference_surface.json").read_text())[script]
+
+
 @pytest.mark.parametrize("script,factory", [
     ("ppo.py", "ppo_args"), ("ppo_atari.py", "ppo_atari_args"), ("ppo_atari_envpool.py", "ppo_atari_envpool_args"),
     ("ppo_atari_multigpu.py", "ppo_atari_multigpu_args"), ("ppo_continuous_action.py", "ppo_continuous_action_args"),
@@ -90,25 +96,9 @@ def test_product_never_imports_oracle():
     ("ppo_atari_lstm.py", "ppo_atari_args")])
 def test_cli_fields_match_reference_args(script, factory):
     """Every reference flag exists with the same default and help text (reference Args dataclasses)."""
-    import ast
     import dataclasses
     from cleanrl_b200 import cli
-    src = Path("/root/reference/cleanrl") / script
-    tree = ast.parse(src.read_text())
-    cls = next(n for n in tree.body if isinstance(n, ast.ClassDef) and n.name == "Args")
-    ref = {}
-    body = cls.body
-    for i, node in enumerate(body):
-        if isinstance(node, ast.AnnAssign):
-            name = node.target.id
-            try:
-                default = ast.literal_eval(node.value)
-            except Exception:
-                default = "<expr>"
-            doc = None
-            if i + 1 < len(body) and isinstance(body[i + 1], ast.Expr) and isinstance(body[i + 1].value, ast.Constant):
-                doc = body[i + 1].value.value
-            ref[name] = (default, doc)
+    ref = {name: (default, doc) for name, default, doc in _reference_surface(script)["args"]}
     ours = getattr(cli, factory)()
     fields = {f.name: f for f in dataclasses.fields(ours)}
     for name, (default, doc) in ref.items():
@@ -123,17 +113,14 @@ def test_cli_fields_match_reference_args(script, factory):
     assert extra <= {"precision", "gae_kernel", "synthetic_env", "huber_loss", "env_groups"}, extra
 
 
-@pytest.mark.reference
 @pytest.mark.parametrize("script", ["ppo.py", "ppo_atari.py", "ppo_atari_envpool.py", "ppo_atari_multigpu.py",
                                     "ppo_continuous_action.py", "dqn_atari.py"])
 def test_module_level_names_match_reference(script):
     """Every top-level class / function of the reference script (what tuner.py, the eval helpers and user code
     import: Args, make_env, layer_init, Agent / QNetwork, RecordEpisodeStatistics, linear_schedule) exists in the
     drop-in module under the same name."""
-    import ast
     import importlib
-    tree = ast.parse((Path("/root/reference/cleanrl") / script).read_text())
-    names = [n.name for n in tree.body if isinstance(n, (ast.ClassDef, ast.FunctionDef))]
+    names = _reference_surface(script)["names"]
     mod = importlib.import_module("cleanrl_b200." + script[:-3])
     missing = [n for n in names if not hasattr(mod, n)]
     assert names and not missing, (script, missing)

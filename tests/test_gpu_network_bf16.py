@@ -1,4 +1,4 @@
-"""-m gpu: bf16 tcgen05 NatureCNN path vs a torch fp32 reference of the same network
+"""-m gpu: bf16 wgmma NatureCNN path vs a torch fp32 reference of the same network
 (floating-point kernel => torch fp32 reference; tolerance = bf16 operand rounding, stated per check).
 
 Layer-by-layer: the activation workspace is read back and compared against torch's NCHW activations

@@ -60,4 +60,3 @@ torch.cuda.synchronize()
 out["reference_host_gather_h2d_ms"] = round((time.time() - t0) / 3 * 1e3, 2)
 out["batch"] = B
 print(json.dumps(out))
-json.dump(out, open("gpurun_out/dqn_bench.json", "w"))

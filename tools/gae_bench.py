@@ -66,4 +66,4 @@ for T, N in [(128, 1024), (128, 4), (2048, 512), (123, 7), (128, 8192)]:
     row["torch_loop_us"] = round(med, 1)
     out.append(row)
     print(json.dumps(row))
-json.dump(out, open("gpurun_out/gae_bench.json", "w"), indent=1)
+print(json.dumps(out, indent=1))

@@ -1,6 +1,6 @@
-"""Summarise an Nsight Compute report of tools/profile_update.py into the JSON files kept under profiles/.
+"""Summarise an Nsight Compute report of tools/profile_update.py into JSON files.
 
-    python tools/ncu_summary.py gpurun_out/x.ncu-rep profiles/rN_ncu_update.json [profiles/rN_traffic.json]
+    python tools/ncu_summary.py update.ncu-rep ncu_update.json [traffic.json]
 
 Kernel launches are mapped to the layer they implement by instantiation and order inside one minibatch
 (forward conv1-3, fc, heads; backward heads, fc, conv3, conv2, conv1).  The traffic file carries, per layer,
