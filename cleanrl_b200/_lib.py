@@ -62,6 +62,9 @@ SIGNATURES = {
     "b200rl_dqn_td_loss_workspace_bytes": (_sz, [_i64]),
     "b200rl_dqn_td_loss_f32": (_i, [_p, _i64, _p, _i64, _p, _p, _p, _i64, _i, _d, _i, _p, _i64, _p, _p, _sz, _p]),
     "b200rl_argmax_f32": (_i, [_p, _i64, _i64, _i, _p, _p]),
+    "b200rl_c51_act_f32": (_i, [_p, _i64, _p, _i64, _i, _i, _p, _p, _p, _p, _p]),
+    "b200rl_c51_loss_workspace_bytes": (_sz, [_i64]),
+    "b200rl_c51_loss_f32": (_i, [_p, _i64, _p, _i64, _p, _p, _p, _p, _i64, _i, _i, _d, _d, _d, _p, _i64, _p, _p, _sz, _p]),
     "b200rl_naturecnn_param_count": (_i64, [_i]),
     "b200rl_naturecnn_bf16_packed_bytes": (_sz, [_i]),
     "b200rl_naturecnn_bf16_acts_bytes": (_sz, [_i64, _i]),

@@ -705,10 +705,13 @@ class QNetworkAgent(nn.Module):
         self._tc_dirty = True
         return out
 
+    def _head_outputs(self):
+        return self.num_actions
+
     def _plan(self):
         f = self.flat
         if self._tc is None:
-            self._tc = ops.NatureCNNBf16(self.num_actions - 1, f.flat.device)   # heads = (A-1) + 1 = A outputs
+            self._tc = ops.NatureCNNBf16(self._head_outputs() - 1, f.flat.device)   # heads = (W-1) + 1 = W outputs
         if self._tc_dirty:
             self._tc.pack(f.flat)
             self._tc_dirty = False
@@ -750,6 +753,62 @@ def dqn_update(q_network, target_network, ring, batch, gamma, lr, huber=False, s
         f = q_network.flat
         f.step += 1
         ops.clip_adam(f.flat, f.grad, f.exp_avg, f.exp_avg_sq, f.step, lr, eps=1e-8, max_norm=None)
+        q_network.params_updated()
+    return stats
+
+
+class C51QNetwork(QNetworkAgent):
+    """C51 distributional Q-network (reference: cleanrl/c51_atari.py:111-138): NatureCNN trunk + Linear(512, A * n_atoms),
+    default torch initialisation, the ``atoms`` buffer (linspace(v_min, v_max, n_atoms)); state_dict keys
+    ``atoms, network.{0,2,4,7,9}.*``.  ``get_action(x, action=None)`` -> (action [n], pmf [n, n_atoms]) runs the head
+    softmax / expectation / argmax in one kernel.  The bf16 path is the tensor-core NatureCNN with an A * n_atoms-wide
+    head (wgmma); fp32 is the exact CUDA-core chain."""
+
+    def __init__(self, env, n_atoms=101, v_min=-100, v_max=100):
+        nn.Module.__init__(self)
+        self.n_atoms = n_atoms
+        self.register_buffer("atoms", torch.linspace(v_min, v_max, steps=n_atoms))
+        self.n = int(env.single_action_space.n)
+        self.network = nn.Sequential(
+            nn.Conv2d(4, 32, 8, stride=4), nn.ReLU(), nn.Conv2d(32, 64, 4, stride=2), nn.ReLU(),
+            nn.Conv2d(64, 64, 3, stride=1), nn.ReLU(), nn.Flatten(), nn.Linear(3136, 512), nn.ReLU(),
+            nn.Linear(512, self.n * n_atoms))
+        self.num_actions = self.n
+        self.precision = "fp32"
+        self._flat = None
+        self._tc = None
+        self._tc_dirty = True
+
+    def _head_outputs(self):
+        return self.n * self.n_atoms
+
+    def logits(self, frames, rows=None, keep=False):
+        """Head logits [n, A * n_atoms] for frames[rows]."""
+        return self.q_values(frames, rows=rows, keep=keep)
+
+    def forward(self, x):
+        return self.logits(x)
+
+    def get_action(self, x, action=None):
+        self.flat
+        act, _, pmf = ops.c51_act(self.logits(x), self.atoms, action)
+        return act, pmf
+
+
+def c51_update(q_network, target_network, ring, batch, gamma, lr, v_min, v_max, batch_size, stats=None):
+    """One C51 update (reference: c51_atari.py:232-265): target forward on next_rows, online forward on rows (activations
+    kept), fused projection + cross-entropy + dL/dlogits, hand-written backward, Adam with eps = 0.01 / batch_size and no
+    gradient clipping."""
+    frames = ring.frames
+    with torch.no_grad():
+        lt = target_network.logits(frames, rows=batch["next_rows"])
+        lo = q_network.logits(frames, rows=batch["rows"], keep=True)
+        stats, dl = ops.c51_loss(lo, lt, target_network.atoms, batch["actions"], batch["rewards"], batch["dones"],
+                                 gamma, v_min, v_max, stats=stats)
+        q_network.backward(dl)
+        f = q_network.flat
+        f.step += 1
+        ops.clip_adam(f.flat, f.grad, f.exp_avg, f.exp_avg_sq, f.step, lr, eps=0.01 / batch_size, max_norm=None)
         q_network.params_updated()
     return stats
 

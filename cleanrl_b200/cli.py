@@ -189,6 +189,36 @@ def dqn_atari_args(exp_name="dqn_atari"):
     return _make("Args", common + algo + extra)
 
 
+def c51_atari_args(exp_name="c51_atari"):
+    """cleanrl/c51_atari.py:25-82."""
+    common = list(_override(_COMMON, exp_name=exp_name))
+    common += [
+        ("save_model", bool, False, "whether to save model into the `runs/{run_name}` folder"),
+        ("upload_model", bool, False, "whether to upload the saved model to huggingface"),
+        ("hf_entity", str, "", "the user or org name of the model repository from the Hugging Face Hub"),
+    ]
+    algo = [
+        ("env_id", str, "BreakoutNoFrameskip-v4", "the id of the environment"),
+        ("total_timesteps", int, 10000000, "total timesteps of the experiments"),
+        ("learning_rate", float, 2.5e-4, "the learning rate of the optimizer"),
+        ("num_envs", int, 1, "the number of parallel game environments"),
+        ("n_atoms", int, 51, "the number of atoms"),
+        ("v_min", float, -10, "the return lower bound"),
+        ("v_max", float, 10, "the return upper bound"),
+        ("buffer_size", int, 1000000, "the replay memory buffer size"),
+        ("gamma", float, 0.99, "the discount factor gamma"),
+        ("target_network_frequency", int, 10000, "the timesteps it takes to update the target network"),
+        ("batch_size", int, 32, "the batch size of sample from the reply memory"),
+        ("start_e", float, 1, "the starting epsilon for exploration"),
+        ("end_e", float, 0.01, "the ending epsilon for exploration"),
+        ("exploration_fraction", float, 0.10, "the fraction of `total-timesteps` it takes from start-e to go end-e"),
+        ("learning_starts", int, 80000, "timestep to start learning"),
+        ("train_frequency", int, 4, "the frequency of training"),
+    ]
+    extra = [r for r in _EXTRA if r[0] != "gae_kernel"]
+    return _make("Args", common + algo + extra)
+
+
 def parse(cls, argv=None):
     return tyro.cli(cls, args=argv)
 

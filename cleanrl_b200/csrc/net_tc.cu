@@ -27,7 +27,10 @@
 //       gradient (column sums of dY) is accumulated by the four dY warps from the staged tiles.
 //   tc_gemm_tma<BN,STAGES>       fc forward / data-gradient: both operands are TMA boxes of row-major matrices.
 //   tc_wgrad_tma                 fc weight gradient (MN-major views of TMA-loaded dhid / act3 row boxes).
-//   tc_heads_*                   the A+1 head outputs in fp32 on CUDA cores.
+//   tc_heads_*                   the A+1 head outputs in fp32 on CUDA cores (A+1 <= kMaxHeads).
+//   wide heads (kMaxHeads < A+1 <= kMaxWideHeads, e.g. C51 logits): forward = tc_gemm_tma with an fp32 + bias epilogue
+//       over hidden; backward = a bf16 copy of dhead feeding tc_wgrad_tma (dWh, folded over row splits in order) and
+//       tc_gemm_tma (dhid, ReLU-masked, into the slot the fc kernels read); dbh = fp32 column sums of dhead.
 #include <cuda.h>            // CUtensorMap types only; the encoder is resolved at run time (no libcuda link)
 #include "tc_base.cuh"
 #include "tc_conv_win.cuh"
@@ -37,6 +40,7 @@
 #include "tc_reduce.cuh"
 #include "tc_aux.cuh"
 #include "tc_heads.cuh"
+#include "tc_heads_wide.cuh"
 
 // =====================================================================================
 // Host side: NatureCNN plan over the kernels above (C-ABI entry points, include/b200rl.h)
@@ -49,6 +53,8 @@ struct NatureLayout {
     int64_t c1w, c1b, c2w, c2b, c3w, c3b, fcw, fcb, hw, hb, total;
     // packed bf16 operand offsets (elements)
     int64_t w1f, w2f, w2dg, w3f, w3dg, wfcf, wfcdg, w1l, w1sc, packed_total;
+    // wide heads only: G = A+1 padded to kWideHeadPad; whf bf16 [G,512], whdg bf16 [512,G], hbp f32 [G]
+    bool wide; int G; int64_t whf, whdg, hbp;
     explicit NatureLayout(int A_) : A(A_) {
         int64_t o = 0;
         c1w = o; o += 32 * 4 * 8 * 8;  c1b = o; o += 32;
@@ -68,6 +74,14 @@ struct NatureLayout {
         wfcdg = q; q += 3136 * 512;
         w1l = q; q += 64 * 256 / 2;          // conv1 weight limbs: s8 [64][256] (16 KB)
         w1sc = q; q += 64 * 2;               // conv1 column scales: f32 [64]
+        wide = A + 1 > kMaxHeads;
+        G = wide ? (int)ceil_div(A + 1, kWideHeadPad) * kWideHeadPad : 0;
+        whf = whdg = hbp = 0;
+        if (wide) {
+            whf = q; q += (int64_t)G * 512;
+            whdg = q; q += (int64_t)G * 512;
+            hbp = q; q += (int64_t)G * 2;
+        }
         packed_total = q;
     }
 };
@@ -181,9 +195,22 @@ static size_t colsum_ws(int64_t M, int ncols) {
 
 using namespace b200rl;
 
+namespace b200rl {
+// head widths the bf16 NatureCNN accepts: narrow (CUDA-core heads) or wide (wgmma heads)
+static bool head_ok(int A) { return A >= 1 && A < kMaxWideHeads; }
+// wide-head backward scratch: weight-gradient partials (big part) and dhead bf16 + bias-sum partials (small part)
+static size_t wide_big_bytes(int64_t n, const NatureLayout& L) {
+    return (size_t)wgrad_plan(n, kFcSplits, 64).splits * L.G * 512 * 4;
+}
+static size_t wide_dhead_bytes(int64_t n, const NatureLayout& L) { return ((size_t)n * L.G * 2 + 255) & ~(size_t)255; }
+static size_t wide_small_bytes(int64_t n, const NatureLayout& L) {
+    return wide_dhead_bytes(n, L) + (size_t)ceil_div(n, wide_colsum_rows(n)) * (L.A + 1) * 4;
+}
+}  // namespace b200rl
+
 extern "C" int64_t b200rl_naturecnn_param_count(int A) { return A >= 1 ? NatureLayout(A).total : -1; }
 extern "C" int64_t b200rl_naturecnn_grad_tail_offset(int A) { return A >= 1 ? NatureLayout(A).fcw : -1; }
-extern "C" size_t b200rl_naturecnn_bf16_packed_bytes(int A) { return A >= 1 ? (size_t)NatureLayout(A).packed_total * 2 : 0; }
+extern "C" size_t b200rl_naturecnn_bf16_packed_bytes(int A) { return head_ok(A) ? (size_t)NatureLayout(A).packed_total * 2 : 0; }
 extern "C" size_t b200rl_naturecnn_bf16_acts_bytes(int64_t n, int obs_format) {
     return n >= 0 ? (size_t)NatureActs(n, obs_format == B200RL_OBS_U8_NCHW).total * 2 + 256 : 0;
 }
@@ -212,22 +239,25 @@ extern "C" int b200rl_frames_to_s2d_u8(const uint8_t* obs, const int64_t* rows, 
 }
 
 extern "C" size_t b200rl_naturecnn_bf16_workspace_bytes(int64_t n, int A) {
-    if (n < 1 || A < 1) return 0;
+    if (n < 1 || !head_ok(A)) return 0;
+    const NatureLayout L(A);
     size_t a = 0;
     auto mx = [&](size_t v) { if (v > a) a = v; };
     mx((size_t)wgrad_plan(n * 512, kC1Ctas, 128).splits * 256 * 64 * 4);
     mx((size_t)wgrad_plan(n * 100, kC2Ctas, 128).splits * 512 * 64 * 4);
     mx((size_t)wgrad_plan(n * 81, kC3Ctas, 128).splits * 640 * 64 * 4);
     mx((size_t)wgrad_plan(n, kFcSplits, 64).splits * 512 * (13 * 256) * 4);
+    if (L.wide) mx(wide_big_bytes(n, L));
     size_t b = 0;
     auto mb = [&](size_t v) { if (v > b) b = v; };
     mb(colsum_ws(n * 441, 32)); mb(colsum_ws(n * 100, 64)); mb(colsum_ws(n * 81, 64)); mb(colsum_ws(n, 512));
-    mb((size_t)2 * ceil_div(n, heads_rows_per_block(n)) * (A + 1) * 514 * 4);
+    if (L.wide) mb(wide_small_bytes(n, L));
+    else mb((size_t)2 * ceil_div(n, heads_rows_per_block(n)) * (A + 1) * 514 * 4);
     return a + b + 512;
 }
 
 extern "C" int b200rl_naturecnn_bf16_pack(const float* params, int A, void* packed, void* stream) {
-    B200RL_REQUIRE(params && packed && A >= 1 && A < kMaxHeads, "naturecnn_pack: bad arguments (A must be in [1,23])");
+    B200RL_REQUIRE(params && packed && head_ok(A), "naturecnn_pack: bad arguments (A must be in [1,%d])", kMaxWideHeads - 1);
     B200RL_REQUIRE(aligned(packed, 16), "naturecnn_pack: packed buffer must be 16-B aligned");
     const NatureLayout L(A);
     bf16* P = reinterpret_cast<bf16*>(packed);
@@ -239,6 +269,11 @@ extern "C" int b200rl_naturecnn_bf16_pack(const float* params, int A, void* pack
     tc_pack_conv_s2_classes<<<(unsigned)ceil_div(32768, 256), 256, 0, s>>>(params + L.c2w, 64, 32, P + L.w2dg);
     tc_pack_conv<<<(unsigned)ceil_div(36864, 256), 256, 0, s>>>(params + L.c3w, 64, 64, 3, 3, 0, P + L.w3f, P + L.w3dg);
     tc_pack_fc<<<dim3(512 / 8, 49 / 7), 256, 0, s>>>(params + L.fcw, 512, 49, P + L.wfcf, P + L.wfcdg);
+    if (L.wide) {
+        tc_pack_head_wide<<<(unsigned)ceil_div((int64_t)L.G * 512, 256), 256, 0, s>>>(params + L.hw, params + L.hb, A + 1, L.G,
+                                                                                    P + L.whf, P + L.whdg, reinterpret_cast<float*>(P + L.hbp));
+        return check_launch("naturecnn_pack", 7);
+    }
     return check_launch("naturecnn_pack", 6);
 }
 
@@ -248,7 +283,7 @@ extern "C" int b200rl_naturecnn_bf16_forward(const void* obs, int obs_format, co
     B200RL_REQUIRE(n >= 0, "naturecnn_forward: negative n");
     if (n == 0) return B200RL_OK;
     B200RL_REQUIRE(obs && params && packed && acts && head_out, "naturecnn_forward: null pointer");
-    B200RL_REQUIRE(A >= 1 && A < kMaxHeads, "naturecnn_forward: A=%d outside [1,23]", A);
+    B200RL_REQUIRE(head_ok(A), "naturecnn_forward: A=%d outside [1,%d]", A, kMaxWideHeads - 1);
     B200RL_REQUIRE(obs_format == B200RL_OBS_U8_NCHW || obs_format == B200RL_OBS_S2D_BF16 || obs_format == B200RL_OBS_S2D_U8,
                    "naturecnn_forward: bad obs_format %d", obs_format);
     B200RL_REQUIRE(aligned(obs, 16) && aligned(acts, 16) && aligned(packed, 16), "naturecnn_forward: misaligned buffer");
@@ -304,6 +339,14 @@ extern "C" int b200rl_naturecnn_bf16_forward(const void* obs, int obs_format, co
       // small batches (rollout step): narrower N tiles => 4x more CTAs for the same work
       if (n <= 8192) { if ((rc = launch_gemm_tma<64, 6>(p, s, "naturecnn/fc"))) return rc; }
       else if ((rc = launch_gemm_tma<128, 4>(p, s, "naturecnn/fc"))) return rc; }
+    if (L.wide) {
+        // wide heads on wgmma: head_out [n, A+1] (fp32) = hidden . Wh^T + bh, over the zero-padded [G, 512] weights
+        gemm_rowmajor(p, act + Q.hid, n, 8);
+        p.Bw = P + L.whf; p.N = L.G; p.bias = reinterpret_cast<const float*>(P + L.hbp);
+        p.out_f32 = head_out; p.ldo = A + 1; p.ncols_f32 = A + 1;
+        ProfScope ps(s, "heads_fwd", 2.0 * n * 512 * (A + 1), (double)n * (1024 + 4 * (A + 1)) + (double)L.G * 1024);
+        return launch_gemm_tma<128, 4>(p, s, "naturecnn/heads_wide");
+    }
     // heads (fp32 math on CUDA cores): head_out [n, A+1] = [logits | value]
     { ProfScope ps(s, "heads_fwd", 2.0 * n * 512 * (A + 1), (double)n * (1024 + 4 * (A + 1)));
       int hb = (int)ceil_div(n, 8); if (hb > num_sms() * 8) hb = num_sms() * 8;
@@ -317,7 +360,7 @@ extern "C" int b200rl_naturecnn_bf16_backward(const void* obs, const void* obs_a
                                               void* workspace, size_t workspace_bytes, void* tail_ready_event, void* stream) {
     B200RL_REQUIRE(n >= 1, "naturecnn_backward: n must be >= 1");
     B200RL_REQUIRE(obs && params && packed && acts && dhead && grads && workspace, "naturecnn_backward: null pointer");
-    B200RL_REQUIRE(A >= 1 && A < kMaxHeads, "naturecnn_backward: A=%d outside [1,23]", A);
+    B200RL_REQUIRE(head_ok(A), "naturecnn_backward: A=%d outside [1,%d]", A, kMaxWideHeads - 1);
     B200RL_REQUIRE(aligned(workspace, 16), "naturecnn_backward: workspace misaligned");
     const size_t need = b200rl_naturecnn_bf16_workspace_bytes(n, A);
     if (workspace_bytes < need) return fail(B200RL_ERR_WORKSPACE, "naturecnn_backward: workspace %zu < %zu", workspace_bytes, need);
@@ -340,12 +383,44 @@ extern "C" int b200rl_naturecnn_bf16_backward(const void* obs, const void* obs_a
         mx((size_t)wgrad_plan(n * 100, kC2Ctas, 128).splits * 512 * 64 * 4);
         mx((size_t)wgrad_plan(n * 81, kC3Ctas, 128).splits * 640 * 64 * 4);
         mx((size_t)wgrad_plan(n, kFcSplits, 64).splits * 512 * (13 * 256) * 4);
+        if (L.wide) mx(wide_big_bytes(n, L));
         big = (big + 255) & ~(size_t)255;
     }
     float* wsbig = reinterpret_cast<float*>(workspace);
     float* wssmall = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + big);
     int rc;
     const int A1 = A + 1;
+    KGemmParams p;
+    if (L.wide) {
+        // ---- wide heads: dhead -> bf16 [n, G]; dbh = fp32 column sums; dWh = dhead_bf16^T . hid on wgmma (row splits
+        //      folded in order); dhid_pre = (dhead_bf16 . Wh) * (hid > 0) on wgmma
+        bf16* dh16 = reinterpret_cast<bf16*>(wssmall);
+        float* dbpart = reinterpret_cast<float*>(reinterpret_cast<char*>(wssmall) + wide_dhead_bytes(n, L));
+        ProfScope ps(s, "heads_bwd", 4.0 * n * 512 * A1, (double)n * (2048 + 64 + 8 * A1));
+        int cb = (int)ceil_div(n * L.G, 256); if (cb > num_sms() * 8) cb = num_sms() * 8;
+        tc_head_dhead_bf16<<<cb, 256, 0, s>>>(dhead, n, A1, L.G, dh16);
+        const int64_t rpb = wide_colsum_rows(n);
+        const int nb = (int)ceil_div(n, rpb);
+        tc_colsum_f32_partial<<<dim3(nb, (unsigned)ceil_div(A1, 128)), 128, 0, s>>>(dhead, n, A1, rpb, dbpart);
+        tc_colsum_f32_final<<<(unsigned)ceil_div(A1, 128), 128, 0, s>>>(dbpart, nb, A1, grads + L.hb);
+        if ((rc = check_launch("naturecnn/heads_wide_bias", 3))) return rc;
+        const WPlan pl = wgrad_plan(n, kFcSplits, 64);
+        CUtensorMap tmX, tmY;
+        if ((rc = make_tmap_2d(&tmX, dh16, n, L.G, 64, "naturecnn/heads_wide_wgrad"))) return rc;
+        if ((rc = make_tmap_2d(&tmY, act + Q.hid, n, 512, 64, "naturecnn/heads_wide_wgrad"))) return rc;
+        const size_t smem = (size_t)4 * (kFcWgradXChunks + kFcWgradYChunks) * 64 * 128 + 1024;
+        static SmemAttrCache attr;
+        if ((rc = attr.ensure(tc_wgrad_tma, smem, "naturecnn/heads_wide_wgrad"))) return rc;
+        const dim3 grid(pl.splits, L.G / (64 * kFcWgradXChunks), 512 / (64 * kFcWgradYChunks));
+        tc_wgrad_tma<<<grid, kWgradTmaThreads, smem, s>>>(tmX, tmY, n, pl.rows_per_cta, wsbig);
+        tc_fold_head_wide<<<(unsigned)ceil_div((int64_t)A1 * 512, 256), 256, 0, s>>>(wsbig, pl.splits, A1, L.G, grads + L.hw);
+        if ((rc = check_launch("naturecnn/heads_wide_wgrad", 2))) return rc;
+        gemm_rowmajor(p, dh16, n, L.G / 64);
+        p.Bw = P + L.whdg; p.N = 512; p.out = act + Q.dhid; p.ldo = 512;
+        p.mask_bits = reinterpret_cast<const uint32_t*>(act + Q.m4);
+        if (n <= 8192) { if ((rc = launch_gemm_tma<64, 6>(p, s, "naturecnn/heads_wide_dgrad"))) return rc; }
+        else if ((rc = launch_gemm_tma<128, 4>(p, s, "naturecnn/heads_wide_dgrad"))) return rc;
+    } else
     // ---- heads: dW, db, then dhid_pre = (dhead . Wh) * (hid > 0)
     {
         const int64_t rpb = heads_rows_per_block(n);
@@ -359,7 +434,6 @@ extern "C" int b200rl_naturecnn_bf16_backward(const void* obs, const void* obs_a
         tc_heads_bwd_data<<<db_blocks, 256, (size_t)A1 * 2048, s>>>(dhead, params + L.hw, reinterpret_cast<const uint8_t*>(act + Q.m4), n, A1, 512, act + Q.dhid);
         if ((rc = check_launch("naturecnn/heads_bwd", 3))) return rc;
     }
-    KGemmParams p;
     // ---- fc: dW[o][c*49+p] = sum_m dhid[m][o] * act3[m][p*64+c]
     {
         const WPlan pl = wgrad_plan(n, kFcSplits, 64);

@@ -24,6 +24,9 @@ struct KGemmParams {
     // fc data-gradient only: write dact3 on the 9x9 linear grid (out) and zero-padded 11x11 grid (out2)
     int dual_dact3;
     bf16* out2;
+    // fp32 output instead of bf16 (wide heads): columns [0, ncols_f32) of out_f32 [M, ldo]; null = bf16 `out`
+    float* out_f32;
+    int ncols_f32;
 };
 
 // ------------------------------------------------------------------ kernel 1d: TMA-fed GEMM (fc forward / data-gradient)
@@ -145,6 +148,12 @@ __global__ void __launch_bounds__(kGemmThreads, 1) tc_gemm_tma(const __grid_cons
                 if (p.mask_bits) {
 #pragma unroll
                     for (int e = 0; e < 32; ++e) if (!((mbw >> e) & 1u)) v[e] = 0u;
+                }
+                if (p.out_f32) {
+                    float* dst = p.out_f32 + (int64_t)r * p.ldo + col;
+#pragma unroll
+                    for (int e = 0; e < 32; ++e) if (col + e < p.ncols_f32) dst[e] = __uint_as_float(v[e]);
+                    continue;
                 }
                 int4 w[4];
 #pragma unroll

@@ -1,4 +1,4 @@
-"""Post-training evaluation with the call surfaces of cleanrl_utils/evals/ppo_eval.py:7-36 and dqn_eval.py:9-44
+"""Post-training evaluation with the call surfaces of cleanrl_utils/evals/ppo_eval.py:7-36, dqn_eval.py:9-44 and c51_eval.py
 (SURVEY.md 8f rank 1).
 
 ``evaluate(model_path, make_env, env_id, eval_episodes, run_name, Model, device, capture_video, gamma)`` rebuilds
@@ -74,6 +74,43 @@ def evaluate_q(model_path, make_env, env_id, eval_episodes, run_name, Model, dev
             with torch.no_grad():
                 q = model(torch.as_tensor(np.asarray(obs)).to(device))
             actions = q.argmax(dim=1).cpu().numpy()
+        obs, _, _, _, infos = envs.step(actions)
+        for ret in _finished_returns(infos):
+            print(f"eval_episode={len(returns)}, episodic_return={ret}")
+            returns.append(ret)
+    return returns
+
+
+def evaluate_c51(model_path, make_env, env_id, eval_episodes, run_name, Model, device=torch.device("cuda"),
+                 epsilon=0.05, capture_video=True, envs=None, max_steps=1000000):
+    """Epsilon-greedy rollout of a saved C51 network (cleanrl_utils/evals/c51_eval.py): the file holds
+    ``{"model_weights": state_dict, "args": vars(args)}``; ``Model(envs, n_atoms=, v_min=, v_max=)`` is rebuilt from the
+    saved args and acts through ``Model.get_action`` (libb200rl kernels)."""
+    import random
+    from argparse import Namespace
+
+    if envs is None:
+        import gymnasium as gym  # type: ignore
+
+        envs = gym.vector.SyncVectorEnv([make_env(env_id, 0, 0, capture_video, run_name)])
+    model_data = torch.load(model_path, map_location="cpu")
+    args = Namespace(**model_data["args"])
+    model = Model(envs, n_atoms=args.n_atoms, v_min=args.v_min, v_max=args.v_max)
+    model.load_state_dict(model_data["model_weights"])
+    model = model.to(device)
+    model.eval()
+
+    returns = []
+    obs, _ = envs.reset()
+    for _ in range(max_steps):
+        if len(returns) >= eval_episodes:
+            break
+        if random.random() < epsilon:
+            actions = np.array([envs.single_action_space.sample() for _ in range(envs.num_envs)])
+        else:
+            with torch.no_grad():
+                actions, _ = model.get_action(torch.as_tensor(np.asarray(obs)).to(device))
+            actions = actions.cpu().numpy()
         obs, _, _, _, infos = envs.step(actions)
         for ret in _finished_returns(infos):
             print(f"eval_episode={len(returns)}, episodic_return={ret}")

@@ -778,3 +778,62 @@ def argmax(q):
     rc = lib.b200rl_argmax_f32(_ptr(q, torch.float32, "q"), q.stride(0), n, A, _ptr(out, torch.int64, "out"), _stream())
     _lib.check(rc, "argmax")
     return out
+
+
+# ------------------------------------------------------------------------ C51
+def c51_act(logits, atoms, action=None, want_q=False, want_pmf=True):
+    """QNetwork.get_action (reference: c51_atari.py:131-138) from the head logits [n, A * n_atoms]: per action the
+    softmax over atoms and q = sum(pmf * atoms); the first-max greedy action (or ``action``).
+    Returns (action i64 [n], q f32 [n, A] or None, pmf f32 [n, n_atoms] of the chosen action or None)."""
+    lib = _lib.load()
+    n, W = logits.shape
+    assert logits.stride(1) == 1
+    atoms = _contig(atoms, "atoms")
+    Z = atoms.numel()
+    if W % Z != 0:
+        raise ValueError(f"c51_act: {W} logits per row is not a multiple of n_atoms={Z}")
+    A = W // Z
+    f = torch.float32
+    dev = logits.device
+    if action is not None:
+        action = _contig(action.reshape(-1), "action")
+        if action.dtype != torch.int64:
+            action = action.long()
+    out_a = torch.empty(n, dtype=torch.int64, device=dev)
+    q = torch.empty(n, A, dtype=f, device=dev) if want_q else None
+    pmf = torch.empty(n, Z, dtype=f, device=dev) if want_pmf else None
+    rc = lib.b200rl_c51_act_f32(_ptr(logits, f, "logits"), logits.stride(0), _ptr(atoms, f, "atoms"), n, A, Z,
+                                _ptr(action, torch.int64, "action", True), _ptr(out_a, torch.int64, "action_out"),
+                                _ptr(q, f, "q", True), _ptr(pmf, f, "pmf", True), _stream())
+    _lib.check(rc, "c51_act")
+    return out_a, q, pmf
+
+
+def c51_loss(logits, next_logits, atoms, actions, rewards, dones, gamma, v_min, v_max, dlogits=None, stats=None):
+    """Categorical projection + clamped cross-entropy + dloss/dlogits (reference: c51_atari.py:233-253).
+    Returns (stats f32[2] = losses/loss, losses/q_values; dlogits [B, A * n_atoms])."""
+    lib = _lib.load()
+    B, W = logits.shape
+    assert logits.stride(1) == 1 and next_logits.stride(1) == 1 and next_logits.shape == (B, W)
+    atoms = _contig(atoms, "atoms")
+    Z = atoms.numel()
+    if W % Z != 0:
+        raise ValueError(f"c51_loss: {W} logits per row is not a multiple of n_atoms={Z}")
+    f = torch.float32
+    dev = logits.device
+    if dlogits is None:
+        dlogits = torch.empty(B, W, dtype=f, device=dev)
+    if stats is None:
+        stats = torch.zeros(2, dtype=f, device=dev)
+    actions = _contig(actions.reshape(-1), "actions")
+    if actions.dtype != torch.int64:
+        actions = actions.long()
+    ws = _workspace(dev, "c51", lib.b200rl_c51_loss_workspace_bytes(B))
+    rc = lib.b200rl_c51_loss_f32(_ptr(logits, f, "logits"), logits.stride(0), _ptr(next_logits, f, "next_logits"),
+                                 next_logits.stride(0), _ptr(atoms, f, "atoms"), _ptr(actions, torch.int64, "actions"),
+                                 _ptr(_contig(rewards.reshape(-1), "rewards"), f, "rewards"),
+                                 _ptr(_contig(dones.reshape(-1), "dones"), f, "dones"), B, W // Z, Z,
+                                 float(gamma), float(v_min), float(v_max), _ptr(dlogits, f, "dlogits"), dlogits.stride(0),
+                                 _ptr(stats, f, "stats"), ws.data_ptr(), ws.numel(), _stream())
+    _lib.check(rc, "c51_loss")
+    return stats, dlogits

@@ -245,7 +245,10 @@ int b200rl_linear_bwd_weight_f32(const float* x, const int64_t* rows, const floa
  * every conv / linear contraction (forward, data-gradient, weight-gradient) is an implicit GEMM
  * on wgmma with bf16 operands and fp32 accumulation in registers, fed by TMA; a minibatch gather
  * (rows) is the image coordinate of conv1's TMA boxes, nothing is materialised; the two heads
- * (A+1 outputs, 1 <= A <= 23) run in fp32 on CUDA cores.
+ * (A+1 outputs, 1 <= A <= 23) run in fp32 on CUDA cores.  Wide heads (24 <= A+1 <= 2048 outputs, e.g. the
+ * A * n_atoms logits of C51) run on wgmma instead: bf16 hidden x bf16 head weights with fp32 output + bias, and in the
+ * backward a bf16 copy of dhead feeds the dhid GEMM and the head weight gradient (fixed-order fold over row
+ * splits); the head bias gradient is an fp32 column sum of dhead.  A+1 > 2048 is B200RL_ERR_INVALID_ARGUMENT.
  *
  * params / grads: ONE flat f32 vector in libb200rl order
  *     conv1.w[32,4,8,8] conv1.b[32] conv2.w[64,32,4,4] conv2.b[64] conv3.w[64,64,3,3] conv3.b[64]
@@ -383,6 +386,32 @@ int b200rl_dqn_td_loss_f32(const float* q, int64_t ld_q, const float* q_target_n
                            float* dq, int64_t ld_dq, float* stats,
                            void* workspace, size_t workspace_bytes, void* stream);
 int b200rl_argmax_f32(const float* q, int64_t ld_q, int64_t n, int A, int64_t* out, void* stream);
+
+/* ------------------------------------------------------------- C51 heads ---
+ * Distributional Q-learning (cleanrl/c51_atari.py).  logits f32 [n, A * n_atoms] (row stride ld) are the output of
+ * Linear(512, A * n_atoms); action a owns columns [a * n_atoms, (a + 1) * n_atoms).  atoms f32 [n_atoms] is the
+ * network's registered `atoms` buffer (linspace(v_min, v_max, n_atoms)); 2 <= n_atoms <= 256.
+ *
+ * b200rl_c51_act_f32: QNetwork.get_action(x, action) (c51_atari.py:131-138).  Per row: pmf = softmax over atoms for every
+ *   action, q = sum(pmf * atoms); the action is the first maximum of q, or action_in[i] when action_in is not NULL.
+ *   action_out i64 [n]; q_out f32 [n, A] and pmf_out f32 [n, n_atoms] (the chosen action's pmf) may be NULL.
+ * b200rl_c51_loss_f32: the update's target + loss + head gradient (c51_atari.py:233-253) in one pass:
+ *   next_pmf = target pmf of the target network's greedy action (next_logits), next_atoms = r + gamma * atoms * (1 - d)
+ *   clamped to [v_min, v_max], categorical projection onto the atoms (index_add_ order: all lower, then all upper
+ *   neighbours), loss = mean_i -sum_j target_ij * log(clamp(pmf_ij, 1e-5, 1 - 1e-5)) with pmf the online network's pmf
+ *   of actions[i].  dlogits f32 [B, A * n_atoms] (row stride ld_d) = dloss/dlogits, zero outside each row's action.
+ *   stats f32 [2] = losses/loss, losses/q_values (mean of sum(pmf * atoms) over the unclamped pmf).
+ *   gamma, v_min, v_max are rounded to f32 as torch rounds Python scalars.  Fixed-order reductions: bitwise
+ *   reproducible.  workspace: b200rl_c51_loss_workspace_bytes(B), 16-byte aligned.
+ */
+int b200rl_c51_act_f32(const float* logits, int64_t ld, const float* atoms, int64_t n, int A, int n_atoms,
+                       const int64_t* action_in, int64_t* action_out, float* q_out, float* pmf_out, void* stream);
+size_t b200rl_c51_loss_workspace_bytes(int64_t B);
+int b200rl_c51_loss_f32(const float* logits, int64_t ld, const float* next_logits, int64_t ld_next,
+                        const float* atoms, const int64_t* actions, const float* rewards, const float* dones,
+                        int64_t B, int A, int n_atoms, double gamma, double v_min, double v_max,
+                        float* dlogits, int64_t ld_d, float* stats,
+                        void* workspace, size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }
