@@ -162,6 +162,8 @@ static int launch_wgrad_win(const WGradWinParams& p, int ctas, cudaStream_t s, c
     // all-TMA when dY rows are exactly 128 bytes; image-aligned steps (3-D TMA for X, cp.async for dY) otherwise
     const int use_tma = p.tpi_shift ? 0 : 1;
     if (p.rows_per_cta % 128 != 0) return fail(B200RL_ERR_INVALID_ARGUMENT, "%s: rows per CTA must be a multiple of 128", what);
+    if (ctas < 1 || (int64_t)(ctas - 1) * p.rows_per_cta >= p.M)
+        return fail(B200RL_ERR_INVALID_ARGUMENT, "%s: every row split must own at least one row", what);
     int rc;
     if (use_tma) {
         if (p.rows || p.ldy != 64 || p.ncolsY != 64)
@@ -172,7 +174,8 @@ static int launch_wgrad_win(const WGradWinParams& p, int ctas, cudaStream_t s, c
         if ((128 << p.tpi_shift) < p.G) return fail(B200RL_ERR_INVALID_ARGUMENT, "%s: steps per image too small", what);
         if ((rc = make_tmap_3d(&tmX, p.X, p.n_images, p.G, (int64_t)p.cpr * 64, p.WRX, what))) return rc;
     }
-    const dim3 grid(ctas, (unsigned)ceil_div(p.nslots / 2, kWgradWinTilesPerCta));
+    // x = the output-tile group, y = the row split: the CTAs that share a split's rows are launched next to each other
+    const dim3 grid((unsigned)ceil_div(p.nslots / 2, kWgradWinTilesPerCta), ctas);
     tc_wgrad_win<<<grid, kWgradWinThreads, smem, s>>>(tmX, tmY, p, use_tma);
     return check_launch(what);
 }

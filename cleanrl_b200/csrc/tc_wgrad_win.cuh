@@ -22,19 +22,83 @@ struct WGradWinParams {
     int WRX;                 // X window rows
     const bf16* Y; int ldy, ncolsY;
     int64_t rows_per_cta;    // multiple of 128
-    float* ws;               // [gridDim.x][nslots*64][64]
-    float* wsb;              // [gridDim.x][64] bias-gradient partials: sum_r dY[r, co]
+    float* ws;               // [gridDim.y][nslots*64][64]
+    float* wsb;              // [gridDim.y][64] bias-gradient partials: sum_r dY[r, co]
 };
 
 // 512 threads: warps 0-3 = dY warps (bias sums; in image-aligned mode they also stage dY with cp.async), warp 4 = TMA
 // producer (warps 5-7 only keep the consumers warpgroup-aligned), warpgroups 2 and 3 = wgmma: warpgroup w accumulates slot
 // 2 t + w of every output tile t this CTA owns.  A CTA owns at most kWgradWinTilesPerCta output tiles (64 accumulator
-// registers per thread); blockIdx.y selects them, so the slots of one row split are spread over gridDim.y CTAs.
+// registers per thread); blockIdx.x selects them and blockIdx.y is the row split, so the gridDim.x CTAs that stream the
+// same rows are adjacent in launch order and run in the same wave: the first one to read a step's rows pulls them into
+// L2 and the others hit there, instead of every y-slice re-reading the whole split from HBM in a wave of its own.
 constexpr int kWgradWinThreads = 512;
 constexpr int kWgradWinTilesPerCta = 2;
+
+// One wgmma warpgroup's main loop over NT (compile-time) output tiles: every step is one straight-line batch of
+// NT x 8 MMAs and one commit group.  The indices of the accumulators must be fixed at compile time: with a runtime tile
+// count ptxas moves the accumulators between the tiles' MMAs and injects warpgroup.wait / warpgroup.arrive around them.
+template <int NT>
+__device__ __forceinline__ void wgrad_win_mma(const WGradWinParams& p, uint8_t* smem, int stage_bytes, int XBYTES, int IMGX,
+                                              uint64_t* full_bar, uint64_t* empty_bar, int nsteps, int t0, int w, int tid) {
+    constexpr int R = 128, STAGES = kWgradWinStages, NY = 64;
+    const int wt = tid & 127;
+    uint32_t arel[NT];
+#pragma unroll
+    for (int tt = 0; tt < NT; ++tt) {
+        const int slot = 2 * (t0 + tt) + w;
+        arel[tt] = (uint32_t)(p.slot_cc[slot] * IMGX + p.shift[p.slot_tap[slot]] * 128);
+    }
+    float d[NT][NY / 2];
+#pragma unroll
+    for (int tt = 0; tt < NT; ++tt)
+#pragma unroll
+        for (int e = 0; e < NY / 2; ++e) d[tt][e] = 0.f;
+    auto step = [&](int it) {                            // one batch of NT x 8 MMAs on the stage of step it, one commit group
+        const int s = it % STAGES;
+        mbar_wait(&full_bar[s], (it / STAGES) & 1);
+        wgmma_fence();
+        const uint32_t xa = smem_u32(smem + (size_t)s * stage_bytes), ya = xa + XBYTES;
+        // K-step kk starts 2048 bytes further on: + 128 in the descriptor's address field (addresses stay below 2^18)
+        const uint64_t yd = desc_mnmajor(ya, 0);
+#pragma unroll
+        for (int tt = 0; tt < NT; ++tt) {
+            const uint64_t xd = desc_mnmajor(xa + arel[tt], 0);
+#pragma unroll
+            for (int kk = 0; kk < R / 16; ++kk)
+                WgmmaBf16<NY, 1, 1>::mma(d[tt], xd + kk * 128, yd + kk * 128, (it | kk) != 0 ? 1u : 0u);
+        }
+        wgmma_commit();
+    };
+    // Step it-1's stage is released once step it's batch has been issued (wgmma_wait<1>), so the tensor pipe does not
+    // drain between steps; the producer only needs step it-STAGES released to refill for step it.  The last step is
+    // peeled: its MMAs, the final wait and the accumulator stores then share one basic block, which keeps ptxas from
+    // scheduling the stores above the wait.  Every split has at least one step (launch_wgrad_win checks it).
+    for (int it = 0; it + 1 < nsteps; ++it) {
+        step(it);
+        wgmma_wait<1>();
+        if (it > 0 && (tid & 31) == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
+    }
+    step(nsteps - 1);
+    wgmma_wait<0>();
+    const int row = ((wt >> 5) << 4) + ((wt & 31) >> 2), col = (wt & 3) * 2;
+    float* wsb = p.ws + (int64_t)blockIdx.y * (p.nslots * 64) * NY;
+#pragma unroll
+    for (int tt = 0; tt < NT; ++tt) {
+        wgmma_fence_operands(d[tt]);
+        float* d0 = wsb + (int64_t)((2 * (t0 + tt) + w) * 64 + row) * NY + col;
+#pragma unroll
+        for (int j = 0; j < NY / 8; ++j) {
+            *reinterpret_cast<float2*>(d0 + 8 * j) = make_float2(d[tt][4 * j], d[tt][4 * j + 1]);
+            *reinterpret_cast<float2*>(d0 + 8 * NY + 8 * j) = make_float2(d[tt][4 * j + 2], d[tt][4 * j + 3]);
+        }
+    }
+}
+
 __global__ void __launch_bounds__(kWgradWinThreads, 1) tc_wgrad_win(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmY,
                                                        const WGradWinParams p, int use_tma) {
     constexpr int R = 128, STAGES = kWgradWinStages, LOOKAHEAD = 1, NY = 64, TT = kWgradWinTilesPerCta;
+    static_assert(TT == 2, "the wgmma warpgroups dispatch on 1 or 2 tiles per CTA");
     extern __shared__ uint8_t smem_raw[];
     __shared__ uint64_t full_bar[STAGES], empty_bar[STAGES];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -43,7 +107,7 @@ __global__ void __launch_bounds__(kWgradWinThreads, 1) tc_wgrad_win(const __grid
     const int XBYTES = IMGX * p.cpr;
     const int stage_bytes = XBYTES + R * 128;
     const int xt = p.nslots / 2;
-    const int t0 = blockIdx.y * TT;                       // first output tile of this CTA
+    const int t0 = blockIdx.x * TT;                       // first output tile of this CTA
     float* sRed = reinterpret_cast<float*>(smem + (size_t)STAGES * stage_bytes);     // [16][64] bias partials (4 KB)
     if (tid == 0) {
         // full:  one expect_tx arrival (TMA) [+ the four cp.async warps that stage dY in image-aligned mode]
@@ -54,7 +118,7 @@ __global__ void __launch_bounds__(kWgradWinThreads, 1) tc_wgrad_win(const __grid
         if (use_tma) tma_prefetch_desc(&tmY);
     }
     __syncthreads();
-    const int64_t m_begin = (int64_t)blockIdx.x * p.rows_per_cta;
+    const int64_t m_begin = (int64_t)blockIdx.y * p.rows_per_cta;
     int64_t m_end = m_begin + p.rows_per_cta;
     if (m_end > p.M) m_end = p.M;
     const int nsteps = m_end > m_begin ? (int)((m_end - m_begin + R - 1) / R) : 0;
@@ -164,53 +228,14 @@ __global__ void __launch_bounds__(kWgradWinThreads, 1) tc_wgrad_win(const __grid
             float t = 0.f;
 #pragma unroll
             for (int l = 0; l < 16; ++l) t += sRed[l * 64 + tid];
-            if (blockIdx.y == 0) p.wsb[(int64_t)blockIdx.x * NY + tid] = t;
+            if (blockIdx.x == 0) p.wsb[(int64_t)blockIdx.y * NY + tid] = t;
         }
     } else if (warp >= 8) {
         // ======================= wgmma warpgroups: X slot (MN-major, rows = reduction index, shifted by whole rows per tap)
         // x dY rows (MN-major); 8 K-steps of 16 rows per step
-        const int w = (warp - 8) >> 2, wt = tid & 127;
-        uint32_t arel[TT];
-#pragma unroll
-        for (int tt = 0; tt < TT; ++tt) {
-            const int slot = 2 * (t0 + tt) + w;
-            arel[tt] = t0 + tt < xt ? (uint32_t)(p.slot_cc[slot] * IMGX + p.shift[p.slot_tap[slot]] * 128) : 0u;
-        }
-        float d[TT][NY / 2];
-#pragma unroll
-        for (int tt = 0; tt < TT; ++tt)
-#pragma unroll
-            for (int e = 0; e < NY / 2; ++e) d[tt][e] = 0.f;
-        for (int it = 0; it < nsteps; ++it) {
-            const int s = it % STAGES;
-            mbar_wait(&full_bar[s], (it / STAGES) & 1);
-            wgmma_fence();
-            const uint32_t xa = smem_u32(smem + (size_t)s * stage_bytes), ya = xa + XBYTES;
-#pragma unroll
-            for (int tt = 0; tt < TT; ++tt) {
-                if (t0 + tt >= xt) continue;
-#pragma unroll
-                for (int kk = 0; kk < R / 16; ++kk)
-                    WgmmaBf16<NY, 1, 1>::mma(d[tt], desc_mnmajor(xa + arel[tt] + kk * 2048, 0), desc_mnmajor(ya + kk * 2048, 0),
-                                             (it | kk) != 0 ? 1u : 0u);
-            }
-            wgmma_commit();
-            wgmma_wait<0>();
-            if ((tid & 31) == 0) mbar_arrive(&empty_bar[s]);
-        }
-        const int row = ((wt >> 5) << 4) + ((wt & 31) >> 2), col = (wt & 3) * 2;
-        float* wsb = p.ws + (int64_t)blockIdx.x * (p.nslots * 64) * NY;
-#pragma unroll
-        for (int tt = 0; tt < TT; ++tt) {
-            if (t0 + tt >= xt) continue;
-            wgmma_fence_operands(d[tt]);
-            float* d0 = wsb + (int64_t)((2 * (t0 + tt) + w) * 64 + row) * NY + col;
-#pragma unroll
-            for (int j = 0; j < NY / 8; ++j) {
-                *reinterpret_cast<float2*>(d0 + 8 * j) = make_float2(d[tt][4 * j], d[tt][4 * j + 1]);
-                *reinterpret_cast<float2*>(d0 + 8 * NY + 8 * j) = make_float2(d[tt][4 * j + 2], d[tt][4 * j + 3]);
-            }
-        }
+        const int w = (warp - 8) >> 2;
+        if (xt - t0 >= TT) wgrad_win_mma<TT>(p, smem, stage_bytes, XBYTES, IMGX, full_bar, empty_bar, nsteps, t0, w, tid);
+        else wgrad_win_mma<1>(p, smem, stage_bytes, XBYTES, IMGX, full_bar, empty_bar, nsteps, t0, w, tid);
     }
 }
 
