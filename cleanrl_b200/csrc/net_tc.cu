@@ -327,13 +327,13 @@ extern "C" int b200rl_naturecnn_bf16_forward(const void* obs, int obs_format, co
     wp.Bw = P + L.w2f; wp.N = 64; wp.vH = 9; wp.vW = 9; wp.out_mode = WOUT_DENSE; wp.out = act + Q.act2;
     wp.bias = params + L.c2b; wp.relu = 1; wp.mask_out = reinterpret_cast<uint32_t*>(act + Q.m2);
     { ProfScope ps(s, "conv2_fwd", 2.0 * n * 81 * 64 * 512, (double)n * ((12800 + 5184) * 2 + 648));
-      if ((rc = launch_conv_win<64, 2, 3, 4>(wp, s, "naturecnn/conv2"))) return rc; }
+      if ((rc = launch_conv_win_t<128, 2, 2, 4>(wp, s, "naturecnn/conv2"))) return rc; }
     // conv3: 3x3 window conv -> act3 [n,7,7,64]
     win_defaults(wp); win_conv3(wp, act + Q.act2, n);
     wp.Bw = P + L.w3f; wp.N = 64; wp.vH = 7; wp.vW = 7; wp.out_mode = WOUT_DENSE; wp.out = act + Q.act3;
     wp.bias = params + L.c3b; wp.relu = 1; wp.mask_out = reinterpret_cast<uint32_t*>(act + Q.m3);
     { ProfScope ps(s, "conv3_fwd", 2.0 * n * 49 * 64 * 576, (double)n * ((5184 + 3136) * 2 + 392));
-      if ((rc = launch_conv_win<64, 1, 6, 9>(wp, s, "naturecnn/conv3"))) return rc; }
+      if ((rc = launch_conv_win_t<128, 1, 4, 9>(wp, s, "naturecnn/conv3"))) return rc; }
     // fc -> hidden [n,512]
     gemm_rowmajor(p, act + Q.act3, n, 49);
     p.Bw = P + L.wfcf; p.N = 512; p.out = act + Q.hid; p.ldo = 512; p.bias = params + L.fcb; p.relu = 1;
@@ -495,7 +495,7 @@ extern "C" int b200rl_naturecnn_bf16_backward(const void* obs, const void* obs_a
         wp.Bw = P + L.w3dg; wp.N = 64; wp.vH = 9; wp.vW = 9; wp.out_mode = WOUT_DACT2;
         wp.out = act + Q.dact2a; wp.out2 = act + Q.dact2b; wp.mask_bits = reinterpret_cast<const uint32_t*>(act + Q.m2);
         { ProfScope ps(s, "conv3_dgrad", 2.0 * n * 81 * 64 * 576, (double)n * ((7744 + 6400 + 7744) * 2 + 648));
-          if ((rc = launch_conv_win<64, 1, 6, 9>(wp, s, "naturecnn/conv3_dgrad"))) return rc; }
+          if ((rc = launch_conv_win_t<128, 1, 4, 9>(wp, s, "naturecnn/conv3_dgrad"))) return rc; }
     }
     // ---- conv2: dW from act1 cell windows x dact2 (10x10 grid); dact1 = one N=128 GEMM over the 4 stride-parity
     //      classes (the 4 channel groups of a cell)
