@@ -88,6 +88,14 @@ SIGNATURES = {
     "b200rl_mt19937_shuffle_i64": (_i, [_p, _p, _p, _i64]),
     "b200rl_stackdelta_launch": (_i64, [_p, _p, _i64, _p]),
     "b200rl_stackdelta_join": (_i64, [_p, _p, _p]),
+    "b200rl_impala_param_count": (_i64, [_i]),
+    "b200rl_impala_bf16_packed_bytes": (_sz, [_i]),
+    "b200rl_impala_bf16_acts_bytes": (_sz, [_i64]),
+    "b200rl_impala_bf16_acts_layout": (_i, [_i64, _p]),
+    "b200rl_impala_bf16_workspace_bytes": (_sz, [_i64, _i]),
+    "b200rl_impala_bf16_pack": (_i, [_p, _i, _p, _p]),
+    "b200rl_impala_bf16_forward": (_i, [_p, _p, _i64, _i, _p, _p, _p, _p, _p]),
+    "b200rl_impala_bf16_backward": (_i, [_p, _p, _i64, _i, _p, _p, _p, _p, _p, _p, _sz, _p]),
 }
 
 

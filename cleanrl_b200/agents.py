@@ -482,7 +482,8 @@ class ImpalaAgent(KernelAgent):
     ``state_dict`` files interchange.  Frames arrive NHWC uint8 ([n, 64, 64, 3]) and are permuted on the device.
 
     Execution: fp32 kernels of libb200rl (padded 3x3 convolutions, max-pool with arg-max, ReLU / add glue), explicit
-    backward in reverse order; no autograd, no cuDNN."""
+    backward in reverse order; no autograd, no cuDNN.  ``precision = "bf16"`` runs the whole network on the tensor
+    cores instead (ops.ImpalaCNNBf16, csrc/net_impala_tc.cu; uint8 frames [*, 64, 64, 3] only)."""
 
     def __init__(self, envs):
         super().__init__()
@@ -501,7 +502,37 @@ class ImpalaAgent(KernelAgent):
         self.num_actions = int(envs.single_action_space.n)
         self._feat_shape = shape
 
-    graph_capturable = False
+    # -- bf16 tensor-core plan ("--precision bf16") ------------------------------
+    precision = "fp32"
+
+    @property
+    def graph_capturable(self):
+        """Only the bf16 plan is free of host work and allocations inside forward / backward."""
+        return self.precision == "bf16"
+
+    def params_updated(self):
+        """Call after the optimiser changed the flat parameters: the packed bf16 operands are stale."""
+        self._tc_dirty = True
+
+    def _tc_plan(self):
+        f = self._flat
+        if self._tc is None:
+            self._tc = ops.ImpalaCNNBf16(self.num_actions, f.flat.device)
+            assert f.flat.numel() >= self._tc.param_count
+        if self._tc_dirty:
+            self._tc.pack(f.flat)
+            self._tc_dirty = False
+        return self._tc
+
+    def load_state_dict(self, *a, **k):
+        out = super().load_state_dict(*a, **k)
+        self._tc_dirty = True
+        return out
+
+    def pin_workspaces(self):
+        """A CUDA graph captured by the engine holds raw pointers into the workspaces: never evict them."""
+        if self._tc is not None:
+            self._tc.pin()
 
     def _param_order(self):
         net = [p for p in self.network.parameters()]
@@ -523,11 +554,20 @@ class ImpalaAgent(KernelAgent):
             self.seqs.append(dict(conv=nets.Conv(q.conv, None, in_div=255.0 if i == 0 else 1.0),
                                   blocks=[(nets.Conv(b.conv0, "relu"), nets.Conv(b.conv1, None))
                                           for b in (q.res_block0, q.res_block1)]))
+        self._tc = None
+        self._tc_dirty = True
 
     # ------------------------------------------------------------------ forward
     def _forward_heads(self, x, rows=None, keep=False):
         if x.dtype != torch.uint8:
             x = x.to(torch.uint8)          # frames are integers 0..255 (the reference passes them as fp32)
+        if self.precision == "bf16":
+            ops.ImpalaCNNBf16.check_obs(x)
+            out = self._tc_plan().forward(x.contiguous(), rows, self._flat.flat)
+            if keep:
+                self._tc_obs, self._tc_rows = x, rows
+            A = self.num_actions
+            return out[:, :A], out[:, A]
         x = ops.nhwc_to_nchw_u8(x.contiguous(), rows)          # [n, 3, 64, 64] uint8; /255 inside the first convolution
         saved = []
         h = x
@@ -565,6 +605,10 @@ class ImpalaAgent(KernelAgent):
 
     # ----------------------------------------------------------------- backward
     def backward(self, dhead):
+        if self.precision == "bf16":
+            self._tc.backward(self._tc_obs, self._tc_rows, self._flat.flat, dhead, self._flat.grad)
+            self._tc_obs = self._tc_rows = None
+            return
         q = self._saved
         self.head.bwd_weight(q["hid"], dhead)
         d_hid = self.head.bwd_data(dhead, q["hid"], "relu")                    # through the ReLU after the Linear

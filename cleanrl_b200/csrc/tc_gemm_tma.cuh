@@ -187,7 +187,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) tc_gemm_tma(const __grid_cons
 // apart); the geometry is fixed: 2 X chunks (one per consumer warpgroup) x 4 Y chunks per CTA.
 constexpr int kWgradTmaThreads = 384;
 constexpr int kFcWgradXChunks = 2, kFcWgradYChunks = 4;
-__global__ void __launch_bounds__(kWgradTmaThreads, 1) tc_wgrad_tma(const __grid_constant__ CUtensorMap tmX,
+static __global__ void __launch_bounds__(kWgradTmaThreads, 1) tc_wgrad_tma(const __grid_constant__ CUtensorMap tmX,
                                                                     const __grid_constant__ CUtensorMap tmY,
                                                                     int64_t M, int64_t rows_per_cta, float* ws) {
     constexpr int R = 64, STAGES = 4, nxc = kFcWgradXChunks, nyc = kFcWgradYChunks, NY = 64 * nyc;

@@ -18,20 +18,23 @@ static inline int64_t heads_rows_per_block(int64_t n) {
     return rpb;
 }
 
-// out[n][A1] = hidden[n][512](bf16) . Wh[A1][512]^T + bh.  One warp per row: lane l holds hidden units
-// [8l, 8l+8) and [256+8l, 256+8l+8) (two 16-byte loads), weights are read as float4 from shared memory.
+// out[n][A1] = hidden[n][HT](bf16) . Wh[A1][HT]^T + bh (HT = 512: NatureCNN, 256: IMPALA-CNN; H == HT).  One warp per
+// row: lane l holds hidden units [256q + 8l, 256q + 8l + 8) (one 16-byte load per q), weights are read as float4 from
+// shared memory.
+template <int HT = 512>
 __global__ void __launch_bounds__(256) tc_heads_fwd(const bf16* __restrict__ hid, const float* __restrict__ Wh,
                                                     const float* __restrict__ bh, int64_t n, int A1, int H,
                                                     float* __restrict__ out) {
-    extern __shared__ float sW[];                       // [A1][512]
-    for (int i = threadIdx.x; i < A1 * 512; i += blockDim.x) sW[i] = Wh[i];
+    constexpr int NQ = HT / 256;
+    extern __shared__ float sW[];                       // [A1][HT]
+    for (int i = threadIdx.x; i < A1 * HT; i += blockDim.x) sW[i] = Wh[i];
     __syncthreads();
     const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
     for (int64_t row = (int64_t)blockIdx.x * wpb + (threadIdx.x >> 5); row < n; row += (int64_t)gridDim.x * wpb) {
-        float hv[16];
-        const bf16* hp = hid + row * 512;
+        float hv[8 * NQ];
+        const bf16* hp = hid + row * HT;
 #pragma unroll
-        for (int q = 0; q < 2; ++q) {
+        for (int q = 0; q < NQ; ++q) {
             const int4 v = ldg16(hp + q * 256 + lane * 8);
             const uint32_t w[4] = {(uint32_t)v.x, (uint32_t)v.y, (uint32_t)v.z, (uint32_t)v.w};
 #pragma unroll
@@ -44,9 +47,9 @@ __global__ void __launch_bounds__(256) tc_heads_fwd(const bf16* __restrict__ hid
         for (int a = 0; a < A1; ++a) {
             float s = 0.f;
 #pragma unroll
-            for (int q = 0; q < 2; ++q) {
-                const float4 w0 = *reinterpret_cast<const float4*>(sW + a * 512 + q * 256 + lane * 8);
-                const float4 w1 = *reinterpret_cast<const float4*>(sW + a * 512 + q * 256 + lane * 8 + 4);
+            for (int q = 0; q < NQ; ++q) {
+                const float4 w0 = *reinterpret_cast<const float4*>(sW + a * HT + q * 256 + lane * 8);
+                const float4 w1 = *reinterpret_cast<const float4*>(sW + a * HT + q * 256 + lane * 8 + 4);
                 s = fmaf(hv[q * 8 + 0], w0.x, s); s = fmaf(hv[q * 8 + 1], w0.y, s);
                 s = fmaf(hv[q * 8 + 2], w0.z, s); s = fmaf(hv[q * 8 + 3], w0.w, s);
                 s = fmaf(hv[q * 8 + 4], w1.x, s); s = fmaf(hv[q * 8 + 5], w1.y, s);
@@ -58,22 +61,24 @@ __global__ void __launch_bounds__(256) tc_heads_fwd(const bf16* __restrict__ hid
         if (lane < A1) out[row * A1 + lane] = mine;     // one coalesced store per row
     }
 }
-// dhid_pre[n][512] (bf16) = (dhead[n][A1] . Wh[A1][512]) * (hid > 0).  Thread = 8 consecutive hidden units of one
+// dhid_pre[n][HT] (bf16) = (dhead[n][A1] . Wh[A1][HT]) * (hid > 0).  Thread = 8 consecutive hidden units of one
 // row (one mask byte in, one 16-byte store out).  Weights are staged transposed, sWt[a][e][group], so the 32 lanes
 // of a warp (consecutive groups) hit 32 different banks.
+template <int HT = 512>
 __global__ void __launch_bounds__(256) tc_heads_bwd_data(const float* __restrict__ dhead, const float* __restrict__ Wh,
                                                          const uint8_t* __restrict__ hid_bits, int64_t n, int A1, int H,
                                                          bf16* __restrict__ dhid) {
-    extern __shared__ float sWt[];                      // [A1][8][64]
-    for (int i = threadIdx.x; i < A1 * 512; i += blockDim.x) {
-        const int a = i >> 9, h = i & 511;
-        sWt[a * 512 + (h & 7) * 64 + (h >> 3)] = Wh[i];
+    constexpr int G = HT / 8;                           // groups of 8 per row
+    extern __shared__ float sWt[];                      // [A1][8][G]
+    for (int i = threadIdx.x; i < A1 * HT; i += blockDim.x) {
+        const int a = i / HT, h = i % HT;
+        sWt[a * HT + (h & 7) * G + (h >> 3)] = Wh[i];
     }
     __syncthreads();
-    const int64_t total = n * 64;                      // 64 groups of 8 per row
+    const int64_t total = n * G;
     for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
-        const int64_t row = idx >> 6;
-        const int g = (int)(idx & 63);
+        const int64_t row = idx / G;
+        const int g = (int)(idx % G);
         const uint32_t m = hid_bits[idx];               // bit e: hid[row][8g + e] > 0
         float o[8];
 #pragma unroll
@@ -81,25 +86,25 @@ __global__ void __launch_bounds__(256) tc_heads_bwd_data(const float* __restrict
         for (int a = 0; a < A1; ++a) {
             const float d = __ldg(dhead + row * A1 + a);
 #pragma unroll
-            for (int e = 0; e < 8; ++e) o[e] = fmaf(d, sWt[a * 512 + e * 64 + g], o[e]);
+            for (int e = 0; e < 8; ++e) o[e] = fmaf(d, sWt[a * HT + e * G + g], o[e]);
         }
 #pragma unroll
         for (int e = 0; e < 8; ++e) if (!((m >> e) & 1u)) o[e] = 0.f;
         int4 w;
         w.x = (int)pack_bf16x2(o[0], o[1]); w.y = (int)pack_bf16x2(o[2], o[3]);
         w.z = (int)pack_bf16x2(o[4], o[5]); w.w = (int)pack_bf16x2(o[6], o[7]);
-        *reinterpret_cast<int4*>(dhid + row * 512 + g * 8) = w;
+        *reinterpret_cast<int4*>(dhid + row * HT + g * 8) = w;
     }
 }
 // dWh[a][h] = sum_m dhead[m][a] * hid[m][h]; dbh[a] = sum_m dhead[m][a]  (partial slabs per (row block, row lane),
-// folded by tc_heads_fold).  Block = 512 threads = 2 row lanes x 256 hidden pairs; the block's dhead rows are staged
+// folded by tc_heads_fold).  Block = HT threads = 2 row lanes x HT/2 hidden pairs; the block's dhead rows are staged
 // in shared memory once, 8 rows of hidden values are in flight per thread.
-template <int MAXA>
+template <int MAXA, int HT = 512>
 __global__ void __launch_bounds__(512) tc_heads_bwd_weight(const float* __restrict__ dhead, const bf16* __restrict__ hid,
                                                            int64_t n, int A1, int H, int64_t rows_per_block,
                                                            float* __restrict__ part) {
     extern __shared__ float sD[];                       // [rows_per_block][A1]
-    const int hp = threadIdx.x & 255, rl = threadIdx.x >> 8;
+    const int hp = threadIdx.x % (HT / 2), rl = threadIdx.x / (HT / 2);
     const int64_t r0 = (int64_t)blockIdx.x * rows_per_block;
     int64_t r1 = r0 + rows_per_block;
     if (r1 > n) r1 = n;
@@ -114,7 +119,7 @@ __global__ void __launch_bounds__(512) tc_heads_bwd_weight(const float* __restri
     for (; r + 14 < nrows; r += 16) {                   // 8 rows (stride 2) in flight
         uint32_t hv[8];
 #pragma unroll
-        for (int u = 0; u < 8; ++u) hv[u] = __ldg(h2 + (r0 + r + 2 * u) * 256 + hp);
+        for (int u = 0; u < 8; ++u) hv[u] = __ldg(h2 + (r0 + r + 2 * u) * (HT / 2) + hp);
 #pragma unroll
         for (int u = 0; u < 8; ++u) {
             const float x0 = __uint_as_float(hv[u] << 16), x1 = __uint_as_float(hv[u] & 0xFFFF0000u);
@@ -129,7 +134,7 @@ __global__ void __launch_bounds__(512) tc_heads_bwd_weight(const float* __restri
         }
     }
     for (; r < nrows; r += 2) {
-        const uint32_t hv = __ldg(h2 + (r0 + r) * 256 + hp);
+        const uint32_t hv = __ldg(h2 + (r0 + r) * (HT / 2) + hp);
         const float x0 = __uint_as_float(hv << 16), x1 = __uint_as_float(hv & 0xFFFF0000u);
         const float* dr = sD + r * A1;
 #pragma unroll
@@ -149,7 +154,7 @@ __global__ void __launch_bounds__(512) tc_heads_bwd_weight(const float* __restri
         }
     }
 }
-__global__ void __launch_bounds__(256) tc_heads_fold(const float* __restrict__ part, int nslabs, int A1, int H,
+static __global__ void __launch_bounds__(256) tc_heads_fold(const float* __restrict__ part, int nslabs, int A1, int H,
                                                      float* __restrict__ dW, float* __restrict__ db) {
     __shared__ float red[256];
     const int idx = blockIdx.x * 32 + (threadIdx.x & 31);

@@ -38,7 +38,7 @@ __device__ __forceinline__ float zlane_sum(const float* __restrict__ part, int64
 struct FoldWin { int layer, S, nslots, Cout; int slot_tap[16], slot_cc[16], slot_skip[16]; float scale;
                  float bscale;     // scale of the bias gradient (1, or 1 / kDact1Scale when dY was stored scaled)
                  const float* wsb; float* db; };
-__global__ void __launch_bounds__(256) tc_fold_win(const float* __restrict__ ws, const FoldWin f, float* __restrict__ dst) {
+static __global__ void __launch_bounds__(256) tc_fold_win(const float* __restrict__ ws, const FoldWin f, float* __restrict__ dst) {
     __shared__ float red[256];
     const int idx = blockIdx.x * 32 + (threadIdx.x & 31);            // (slot*64 + row) * Cout + co
     const int KX = f.nslots * 64;
@@ -72,7 +72,7 @@ __global__ void __launch_bounds__(256) tc_fold_win(const float* __restrict__ ws,
 
 // fold the fc weight-gradient partials ws[S][KX rows = o][NY cols = k], k = p*64 + c, into the REFERENCE's layout
 // dst[o][c*49 + p] (torch flattens NCHW activations channel-major); partial slabs are added in ascending order.
-__global__ void tc_fold_fc(const float* __restrict__ ws, int S, int KX, int NY, int validX, int validY,
+static __global__ void tc_fold_fc(const float* __restrict__ ws, int S, int KX, int NY, int validX, int validY,
                            int C, int KK, float scale, float* __restrict__ dst) {
     const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int64_t total = (int64_t)validX * validY;
@@ -88,7 +88,7 @@ __global__ void tc_fold_fc(const float* __restrict__ ws, int S, int KX, int NY, 
 // column sums of a bf16 matrix [M, ld] (bias gradients): two-level deterministic reduction.
 // Block = 256 threads = (256 / (ncols/8)) row lanes x (ncols/8) column groups; every thread streams
 // 16-byte vectors (8 columns) down its rows, then the row lanes are folded through shared memory.
-__global__ void __launch_bounds__(256) tc_colsum_partial(const bf16* __restrict__ Y, int64_t M, int ld, int ncols,
+static __global__ void __launch_bounds__(256) tc_colsum_partial(const bf16* __restrict__ Y, int64_t M, int ld, int ncols,
                                                          int64_t rows_per_block, float* __restrict__ part) {
     __shared__ float red[256 * 8];
     const int cg = ncols >> 3;                 // column groups of 8
@@ -121,7 +121,7 @@ __global__ void __launch_bounds__(256) tc_colsum_partial(const bf16* __restrict_
         part[(int64_t)blockIdx.x * ncols + c] = s;
     }
 }
-__global__ void __launch_bounds__(256) tc_colsum_final(const float* __restrict__ part, int nblocks, int ncols,
+static __global__ void __launch_bounds__(256) tc_colsum_final(const float* __restrict__ part, int nblocks, int ncols,
                                                        float* __restrict__ db) {
     __shared__ float red[256];
     const int c = blockIdx.x * 32 + (threadIdx.x & 31);

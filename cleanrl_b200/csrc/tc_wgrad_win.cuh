@@ -95,7 +95,7 @@ __device__ __forceinline__ void wgrad_win_mma(const WGradWinParams& p, uint8_t* 
     }
 }
 
-__global__ void __launch_bounds__(kWgradWinThreads, 1) tc_wgrad_win(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmY,
+static __global__ void __launch_bounds__(kWgradWinThreads, 1) tc_wgrad_win(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmY,
                                                        const WGradWinParams p, int use_tma) {
     constexpr int R = 128, STAGES = kWgradWinStages, LOOKAHEAD = 1, NY = 64, TT = kWgradWinTilesPerCta;
     static_assert(TT == 2, "the wgmma warpgroups dispatch on 1 or 2 tiles per CTA");

@@ -537,6 +537,119 @@ class NatureCNNBf16:
         _lib.check(rc, "naturecnn_bf16_backward")
 
 
+# ------------------------------------------------------ IMPALA-CNN bf16 (tensor-core) plan
+class ImpalaCNNBf16:
+    """Owns the packed bf16 weights, the activation workspaces and the backward workspace of the tensor-core
+    IMPALA-CNN (procgen frames uint8 [*, 64, 64, 3])."""
+
+    MAX_UNPINNED = 4
+
+    def __init__(self, A, device):
+        lib = _lib.load()
+        self.A, self.device = int(A), device
+        nbytes = lib.b200rl_impala_bf16_packed_bytes(self.A)
+        if nbytes == 0:
+            raise ValueError(f"tensor-core IMPALA-CNN supports 1 <= A <= 23 actions (got {A})")
+        self.param_count = lib.b200rl_impala_param_count(self.A)
+        self.packed = torch.empty(nbytes, dtype=torch.uint8, device=device)
+        self._acts = {}          # n -> workspace, least-recently-used first
+        self._pinned = set()     # batch sizes referenced by captured CUDA graphs: never evicted
+        self._ws = None
+        self._pinned_ws = []     # backward workspaces referenced by captured CUDA graphs
+
+    def pin(self):
+        """Every workspace that exists now may be referenced by a captured CUDA graph: keep it alive."""
+        self._pinned.update(self._acts.keys())
+        if self._ws is not None and all(w is not self._ws for w in self._pinned_ws):
+            self._pinned_ws.append(self._ws)
+
+    def acts(self, n):
+        lib = _lib.load()
+        buf = self._acts.pop(n, None)
+        if buf is None:
+            unpinned = [k for k in self._acts if k not in self._pinned]
+            while len(unpinned) >= self.MAX_UNPINNED:
+                del self._acts[unpinned.pop(0)]
+            nbytes = lib.b200rl_impala_bf16_acts_bytes(n)
+            if nbytes == 0:
+                raise ValueError(f"tensor-core IMPALA-CNN: batch of {n} rows is out of range")
+            buf = torch.zeros(nbytes, dtype=torch.uint8, device=self.device)
+        self._acts[n] = buf
+        return buf
+
+    def act_tensors(self, n):
+        """Named views of the activation workspace of batch size ``n`` (layout: b200rl_impala_bf16_acts_layout)."""
+        import ctypes
+        off = (ctypes.c_int64 * 30)()
+        _lib.check(_lib.load().b200rl_impala_bf16_acts_layout(n, off), "impala_acts_layout")
+        buf = self.acts(n)
+        bf, u8, i32 = torch.bfloat16, torch.uint8, torch.int32
+
+        def view(o, dtype, shape):
+            cnt = 1
+            for d in shape:
+                cnt *= d
+            nb = cnt * torch.tensor([], dtype=dtype).element_size()
+            return buf[o:o + nb].view(dtype).view(*shape)
+        out, k = {}, 3
+        for name, shp in (("c0", (n, 64, 64, 16)), ("c1", (n, 32, 32, 32)), ("c2", (n, 16, 16, 32))):
+            out[name] = view(off[["c0", "c1", "c2"].index(name)], bf, shp)
+        for q, shp in enumerate(((n, 32, 32, 16), (n, 16, 16, 32), (n, 8, 8, 32))):
+            for name in ("s0", "s1", "s2", "y0", "y1"):
+                if off[k] >= 0:
+                    out[f"{name}_{q}"] = view(off[k], bf, shp)
+                k += 1
+            out[f"arg_{q}"] = view(off[k], u8, shp)
+            k += 1
+        for name, dtype, shp in (("h0", bf, (n, 2048)), ("mh0", i32, (n, 64)), ("hid", bf, (n, 256)), ("mhid", i32, (n, 8)),
+                                 ("dc", bf, (n, 65536)), ("ga", bf, (n, 16384)), ("gb", bf, (n, 16384)),
+                                 ("gy", bf, (n, 16384)), ("dhid", bf, (n, 256))):
+            out[name] = view(off[k], dtype, shp)
+            k += 1
+        return out
+
+    @staticmethod
+    def check_obs(obs):
+        if obs.dtype != torch.uint8 or obs.dim() < 4 or tuple(obs.shape[-3:]) != (64, 64, 3):
+            raise ValueError("tensor-core IMPALA-CNN consumes uint8 frames [*, 64, 64, 3] "
+                             f"(got {obs.dtype} {tuple(obs.shape)})")
+
+    def pack(self, flat_params):
+        rc = _lib.load().b200rl_impala_bf16_pack(_ptr(flat_params, torch.float32, "params"), self.A,
+                                                 self.packed.data_ptr(), _stream())
+        _lib.check(rc, "impala_bf16_pack")
+
+    def forward(self, obs, rows, flat_params, head_out=None):
+        self.check_obs(obs)
+        _contig(obs, "obs")
+        n = rows.numel() if rows is not None else obs.shape[0]
+        if rows is not None:
+            _contig(rows, "rows")
+        if head_out is None:
+            head_out = torch.empty(n, self.A + 1, dtype=torch.float32, device=self.device)
+        rc = _lib.load().b200rl_impala_bf16_forward(_ptr(obs, torch.uint8, "obs"), _ptr(rows, torch.int64, "rows", True), n,
+                                                    self.A, _ptr(flat_params, torch.float32, "params"), self.packed.data_ptr(),
+                                                    self.acts(n).data_ptr(), _ptr(head_out, torch.float32, "head_out"), _stream())
+        _lib.check(rc, "impala_bf16_forward")
+        return head_out
+
+    def backward(self, obs, rows, flat_params, dhead, flat_grads):
+        """Gradient of the forward that last ran on (obs, rows) with this batch size; fills ``flat_grads``."""
+        lib = _lib.load()
+        self.check_obs(obs)
+        _contig(dhead, "dhead")
+        n = dhead.shape[0]
+        nbytes = lib.b200rl_impala_bf16_workspace_bytes(n, self.A)
+        if self._ws is None or self._ws.numel() < nbytes:
+            self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        rc = lib.b200rl_impala_bf16_backward(_ptr(obs, torch.uint8, "obs"), _ptr(rows, torch.int64, "rows", True), n, self.A,
+                                             _ptr(flat_params, torch.float32, "params"), self.packed.data_ptr(),
+                                             self.acts(n).data_ptr(), _ptr(dhead, torch.float32, "dhead"),
+                                             _ptr(flat_grads, torch.float32, "grads"), self._ws.data_ptr(), self._ws.numel(),
+                                             _stream())
+        _lib.check(rc, "impala_bf16_backward")
+
+
 def frames_to_s2d(obs_u8, out=None, rows=None):
     """uint8 [n,4,84,84] frames -> bf16 [n,21,21,64] space-to-depth frames (once per env step)."""
     lib = _lib.load()

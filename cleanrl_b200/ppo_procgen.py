@@ -82,6 +82,7 @@ def main(argv=None, writer_factory=None, env_factory=None, on_iteration=None, ag
     envs = env_factory(args) if env_factory else make_envs(args, run_name)
     assert hasattr(envs.single_action_space, "n"), "only discrete action space is supported"
     agent = Agent(envs).to(device)
+    agent.precision = args.precision
     if agent_hook:
         agent_hook(agent)
     engine = PPOEngine(agent, args, envs.single_observation_space.shape, np.uint8, args.num_envs, device,

@@ -355,6 +355,40 @@ int b200rl_naturecnn_bf16_backward(const void* obs, const void* obs_aux, int obs
  * tail on another stream while the convolution gradients are still being computed. */
 int64_t b200rl_naturecnn_grad_tail_offset(int A);
 
+/* ------------------------------------------------------------ IMPALA-CNN, bf16 tensor cores ---
+ * cleanrl/ppo_procgen.py:89-150 (three ConvSequences 16/32/32, fc 2048 -> 256, heads), bf16 operands, fp32 accumulation.
+ * params : flat fp32 vector in ImpalaAgent._param_order (the trunk in module order, both head weights, both head
+ *          biases; b200rl_impala_param_count(A) elements), 16-B aligned.
+ * packed : bf16 operand copies (b200rl_impala_bf16_packed_bytes), refreshed by b200rl_impala_bf16_pack after every
+ *          optimiser step.
+ * acts   : activation + activation-gradient workspace for batch n (b200rl_impala_bf16_acts_bytes), 256-B aligned; the
+ *          backward reads what the forward of the same (obs, rows, n) left there.
+ * obs    : uint8 NHWC frames [*, 64, 64, 3]; row i of the batch is frame rows[i] (rows may be NULL: frame i).
+ * head_out [n, A+1] fp32 = [logits | value]; dhead [n, A+1] its gradient; grads = flat fp32 gradient (overwritten).
+ * 1 <= A <= 23 (A+1 <= 24 head outputs), 0 <= n <= 131072.  Bad pointers, alignment, A or n: B200RL_ERR_INVALID_ARGUMENT
+ * before any launch.  No host synchronisation or allocation: forward and backward may be captured in a CUDA graph. */
+int64_t b200rl_impala_param_count(int A);
+size_t b200rl_impala_bf16_packed_bytes(int A);
+size_t b200rl_impala_bf16_acts_bytes(int64_t n);
+/* Byte offsets of the tensors inside `acts` for batch n (all channel-last; -1 = not stored), written to
+ * offsets[B200RL_IMPALA_ACTS_TENSORS] in this order:
+ *   c0 bf16 [n,64,64,16], c1 bf16 [n,32,32,32], c2 bf16 [n,16,16,32]      conv outputs in front of each max-pool
+ *   for each sequence q (grid 32x32x16, 16x16x32, 8x8x32):
+ *     s0 (max-pool output), s1 (after block 0), s2 (after block 1; -1 for q = 2), y0, y1 (relu(conv0) of each block)
+ *     bf16 [n,H,W,C]; arg uint8 [n,H,W,C] (arg-max 0..8 in the 3x3 window)
+ *   h0 bf16 [n,2048] (relu of the last stream = fc input), mh0 uint32 [n,64] (its > 0 bits), hid bf16 [n,256] (fc
+ *   output), mhid uint32 [n,8], then the backward scratch: dc (gradient of the last max-pool input handled, bf16 up to
+ *   [n,64,64,16]), ga, gb (stream gradients, bf16 up to [n,16384]), gy (gradient of relu(conv0)), dhid bf16 [n,256]. */
+#define B200RL_IMPALA_ACTS_TENSORS 30
+int b200rl_impala_bf16_acts_layout(int64_t n, int64_t* offsets);
+size_t b200rl_impala_bf16_workspace_bytes(int64_t n, int A);
+int b200rl_impala_bf16_pack(const float* params, int A, void* packed, void* stream);
+int b200rl_impala_bf16_forward(const uint8_t* obs, const int64_t* rows, int64_t n, int A, const float* params,
+                               const void* packed, void* acts, float* head_out, void* stream);
+int b200rl_impala_bf16_backward(const uint8_t* obs, const int64_t* rows, int64_t n, int A, const float* params,
+                                const void* packed, void* acts, const float* dhead, float* grads,
+                                void* workspace, size_t workspace_bytes, void* stream);
+
 /* ------------------------------------------------------------ LSTM cell ---
  * Recurrent PPO agent (cleanrl/ppo_atari_lstm.py:117-160: nn.LSTM(512, 128), gate order i, f, g, o; the state is reset
  * by (1 - done) BEFORE the cell, :137-142).  The gate GEMMs are b200rl_linear_fwd_f32 calls (x W_ih^T + b_ih for all
