@@ -1,12 +1,14 @@
 #!/usr/bin/env python
-"""Per-launch times of the four window convolutions of the bf16 NatureCNN (conv2 / conv3 forward, conv3 / conv2 data
-gradients) at the two batch sizes of a PPO iteration: n = 1024 (a rollout step) and n = 32 768 (a minibatch).
+"""Per-launch times of the convolutions of the bf16 NatureCNN (conv1 forward and weight gradient on the uint8 rollout,
+and the four window convolutions: conv2 / conv3 forward, conv3 / conv2 data gradients) at the two batch sizes of a PPO
+iteration: n = 1024 (a rollout step) and n = 32 768 (a minibatch).
 
     python bench_conv_win.py [--reps R] [--sizes 1024,32768]
 
 Each size runs forward + backward on uint8 space-to-depth rollout rows gathered through sorted minibatch indices (the
-engine's path), with the library's per-launch CUDA-event profiler on.  Prints one JSON line: microseconds per launch,
-per size and kernel.  Nothing is written to disk."""
+engine's path), with the library's per-launch CUDA-event profiler on.  Prints one JSON line: microseconds per launch
+and the algorithmic bandwidth (the profiler's byte count of the launch over its time, GB/s), per size and kernel.
+Nothing is written to disk."""
 import argparse
 import ctypes
 import json
@@ -18,7 +20,7 @@ import torch
 sys.path.insert(0, str(Path(__file__).resolve().parent))
 from cleanrl_b200 import _lib, build, ops  # noqa: E402
 
-KERNELS = ("conv2_fwd", "conv3_fwd", "conv3_dgrad", "conv2_dgrad")
+KERNELS = ("conv1_fwd", "conv2_fwd", "conv3_fwd", "conv3_dgrad", "conv2_dgrad", "conv1_wgrad")
 
 
 def measure(lib, n, reps, dev):
@@ -52,7 +54,8 @@ def measure(lib, n, reps, dev):
     buf = ctypes.create_string_buffer(1 << 16)
     _lib.check(lib.b200rl_profile_summary(buf, 1 << 16), "profile_summary")
     prof = {r["name"]: r for r in json.loads(buf.value.decode())}
-    return {k: round(1e3 * prof[k]["ms"] / prof[k]["launches"], 2) for k in KERNELS}
+    return {k: {"us": round(1e3 * prof[k]["ms"] / prof[k]["launches"], 2),
+                "GB/s": round(prof[k]["bytes"] / (prof[k]["ms"] * 1e-3) / 1e9, 1)} for k in KERNELS}
 
 
 def main():
@@ -63,7 +66,7 @@ def main():
     build.build()
     lib = _lib.load()
     dev = torch.device("cuda:0")
-    res = {"device": torch.cuda.get_device_name(dev), "unit": "us per launch"}
+    res = {"device": torch.cuda.get_device_name(dev), "unit": "us per launch, GB/s"}
     for n in (int(s) for s in a.sizes.split(",")):
         res[f"n{n}"] = measure(lib, n, a.reps, dev)
     print(json.dumps(res))

@@ -302,14 +302,21 @@ __device__ __forceinline__ uint32_t prmt(uint32_t a, uint32_t b, uint32_t sel) {
 constexpr float kU8Bias = 1024.0f;
 
 
-// fp16 pair (1024 + x[pos], 1024 + x[pos + 1]) from the 20-byte window w[0..4] (pos in 0..15); pos is lane-dependent, so
-// the word is picked with selects rather than a (local-memory) indexed array
-__device__ __forceinline__ uint32_t pair_f16_biased(const uint32_t (&w)[5], int pos) {
-    const int wi = pos >> 2, b = pos & 3;
-    const uint32_t lo = wi == 0 ? w[0] : wi == 1 ? w[1] : wi == 2 ? w[2] : w[3];
-    const uint32_t hi = wi == 0 ? w[1] : wi == 1 ? w[2] : wi == 2 ? w[3] : w[4];
-    const uint32_t x = prmt(lo, hi, (uint32_t)(b | ((b + 1) << 4)));
-    return prmt(x, 0x64646464u, 0x5140u);
+// fp16 pair (1024 + x[pos], 1024 + x[pos + 1]) from the 20-byte window w[0..4], pos = 4 (j + up) + b: the lane-dependent
+// word choice is one select per word on a per-thread constant (an indexed array would go to local memory, and a chain of
+// comparisons compiles to branches), and `sel` = b | (b + 1) << 4 picks the two bytes
+__device__ __forceinline__ uint32_t pair_f16_biased(const uint32_t (&w)[5], int j, bool up, uint32_t sel) {
+    const uint32_t lo = up ? w[j + 1] : w[j];
+    const uint32_t hi = up ? w[j + 2] : w[j + 1];
+    return prmt(prmt(lo, hi, sel), 0x64646464u, 0x5140u);
+}
+// 16 bytes at a shared-memory address.  The staging pointers come from the 1 KB-aligned dynamic shared memory through an
+// integer cast, so plain dereferences compile to generic 64-bit loads; these are LDS.128 with 32-bit addresses.  volatile
+// + memory: the loads stay between the mbarrier wait that publishes the block and the arrive that releases it.
+__device__ __forceinline__ uint4 lds128(uint32_t addr) {
+    uint4 v;
+    asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+    return v;
 }
 
 // 512 threads: warp 0 = X producer, warp 1 = dY producer (warps 2-3 idle: warpgroup alignment), warpgroup 1 = bias sums,
@@ -421,6 +428,9 @@ __global__ void __launch_bounds__(kC1WThreads, 1) tc_conv1_wgrad_u8(const __grid
         // B = the step's dY rows at offsets 0 (b = 0) and -21 (b = 1); 8 K-steps of 16 positions per step
         const int h = (warp - 8) >> 2, wt = tid & 127, qd = lane & 3;
         const int c0 = ((wt >> 5) << 4) + (lane >> 2);     // fragment rows c0 and c0 + 8 = channels
+        // this thread's pixel pairs start at byte 2 qd + h and 8 + 2 qd + h of each 16-position chunk: words (qd >> 1) [+ 2]
+        const bool up = qd >= 2;
+        const uint32_t pb = (uint32_t)((2 * qd + h) & 3), psel = pb | ((pb + 1) << 4);
         float d[2][16];
 #pragma unroll
         for (int b = 0; b < 2; ++b)
@@ -434,18 +444,18 @@ __global__ void __launch_bounds__(kC1WThreads, 1) tc_conv1_wgrad_u8(const __grid
 #pragma unroll
             for (int r = 0; r < 2; ++r) {
                 const int c = c0 + 8 * r;
-                const uint8_t* bm = sX + (size_t)xm * kC1WBlock + c * 128;
-                const uint8_t* bh = sX + (size_t)xh * kC1WBlock + c * 128;
+                const uint32_t bm = smem_u32(sX + (size_t)xm * kC1WBlock + c * 128);
+                const uint32_t bh = smem_u32(sX + (size_t)xh * kC1WBlock + c * 128);
                 const uint32_t sw = (uint32_t)(c & 7);
-                int4 cur = *reinterpret_cast<const int4*>(bm + ((0u ^ sw) << 4));
+                uint4 cur = lds128(bm + ((0u ^ sw) << 4));
 #pragma unroll
                 for (int kk = 0; kk < 8; ++kk) {
-                    int4 nxt = make_int4(0, 0, 0, 0);
-                    if (h == 1) nxt = *reinterpret_cast<const int4*>((kk < 7 ? bm : bh) + ((((uint32_t)(kk + 1) & 7u) ^ sw) << 4));
-                    const uint32_t w[5] = {(uint32_t)cur.x, (uint32_t)cur.y, (uint32_t)cur.z, (uint32_t)cur.w, (uint32_t)nxt.x};
-                    a[kk][r] = pair_f16_biased(w, 2 * qd + h);              // K 2 qd, 2 qd + 1
-                    a[kk][2 + r] = pair_f16_biased(w, 8 + 2 * qd + h);      // K 8 + 2 qd, 9 + 2 qd
-                    if (kk < 7) cur = h == 1 ? nxt : *reinterpret_cast<const int4*>(bm + ((((uint32_t)(kk + 1)) ^ sw) << 4));
+                    uint4 nxt = make_uint4(0, 0, 0, 0);
+                    if (h == 1) nxt = lds128((kk < 7 ? bm : bh) + ((((uint32_t)(kk + 1) & 7u) ^ sw) << 4));
+                    const uint32_t w[5] = {cur.x, cur.y, cur.z, cur.w, nxt.x};
+                    a[kk][r] = pair_f16_biased(w, 0, up, psel);             // K 2 qd, 2 qd + 1
+                    a[kk][2 + r] = pair_f16_biased(w, 2, up, psel);         // K 8 + 2 qd, 9 + 2 qd
+                    if (kk < 7) cur = h == 1 ? nxt : lds128(bm + ((((uint32_t)(kk + 1)) ^ sw) << 4));
                 }
             }
             // the pixels are in registers: release the X blocks (block 0 has no halo reader, so its h = 1 readers arrive twice)
