@@ -34,9 +34,11 @@ using namespace tc;
 __device__ __forceinline__ uint64_t desc_kmajor_sw64(uint32_t smem_addr) {
     return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | (32ull << 32) | kDescSwizzle64;
 }
-// MN-major SWIZZLE_64B operand with ONE 32-element (64-byte) MN atom: rows = K index, 8-row K groups 512 B apart
-__device__ __forceinline__ uint64_t desc_mnmajor_sw64(uint32_t smem_addr) {
-    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | (32ull << 32) | kDescSwizzle64;
+// MN-major SWIZZLE_64B operand of 32-element (64-byte) MN atoms: rows = K index, 8-row K groups 512 B apart (SBO), MN atom
+// i (columns 32 i .. 32 i + 31) at smem_addr + i * lbo (LBO; any multiple of 64 B: the swizzle is applied to the absolute
+// address bits, as for start addresses shifted by whole rows)
+__device__ __forceinline__ uint64_t desc_mnmajor_sw64(uint32_t smem_addr, uint32_t lbo) {
+    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)((lbo >> 4) & 0x3FFF) << 16) | (32ull << 32) | kDescSwizzle64;
 }
 // byte offset of 16-byte chunk c (0..3) of row r in a SWIZZLE_64B image (address bits [4,6) ^= bits [7,9))
 __device__ __forceinline__ uint32_t img64_off(int r, int c) { return (uint32_t)(r * 64 + ((c ^ ((r >> 1) & 3)) << 4)); }
@@ -264,9 +266,10 @@ __global__ void __launch_bounds__(kConv1I8Threads, 1) tc_conv1_i8(const __grid_c
 //       D_b[(h, c), co] = sum_k X[k + h, c] * dY[k - s_b, co],    tap = 2 b + h.
 //   A  (registers, 64 rows x 16 K per wgmma): warpgroup h holds channel c of the pixel stream X[k + h] as fp16 fragments;
 //       one fragment per K-step serves both tap groups b.
-//   B  (shared memory, MN-major SWIZZLE_64B, N = 32): the dY rows of the step, rows [k0, k0 + 128) for b = 0 and rows
-//       [k0 - 21, k0 + 107) for b = 1.  The stages form one contiguous ring, so the b = 1 operand is the same tile with its
-//       descriptor start moved 21 rows back into the previous stage (the swizzle is a function of the address bits);
+//   B  (shared memory, MN-major SWIZZLE_64B): the dY rows of the step, rows [k0, k0 + 128) for b = 0 and rows
+//       [k0 - 21, k0 + 107) for b = 1.  The stages form one contiguous ring, so the b = 1 operand is the same tile moved
+//       21 rows back into the previous stage (the swizzle is a function of the address bits), and both are ONE N = 64
+//       operand: MN atom 0 (columns 0-31) starts at row k0 - 21 for b = 1, atom 1 (columns 32-63) 21 rows later for b = 0;
 //       stage 0 is preceded by a 24-row pad that receives the previous rows by a second small TMA box.  Negative rows and
 //       rows >= 441 are zero-filled by the TMA unit: images are independent and occupy 512-row slots, and a CTA owns whole
 //       images.
@@ -319,6 +322,15 @@ __device__ __forceinline__ uint4 lds128(uint32_t addr) {
     return v;
 }
 
+// Per-warpgroup register budgets (setmaxnreg): the kernel launches at 128 registers per thread (512 threads, 1 CTA per
+// SM); the producer and bias warpgroups give registers back to the wgmma warpgroups, whose fragment build then keeps
+// more shared-memory loads in flight (measured: about 5 % less time per launch).  128 x 40 + 128 x 56 + 256 x 208 =
+// 65 536, the SM's register file.
+template <int R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+constexpr int kC1WRegsProducer = 40, kC1WRegsBias = 56, kC1WRegsMma = 208;
+static_assert(128 * kC1WRegsProducer + 128 * kC1WRegsBias + 256 * kC1WRegsMma <= 65536, "register budgets exceed the SM");
+
 // 512 threads: warp 0 = X producer, warp 1 = dY producer (warps 2-3 idle: warpgroup alignment), warpgroup 1 = bias sums,
 // warpgroups 2 and 3 = wgmma for the pixel streams h = 0 and h = 1
 constexpr int kC1WThreads = 512;
@@ -351,9 +363,10 @@ __global__ void __launch_bounds__(kC1WThreads, 1) tc_conv1_wgrad_u8(const __grid
     const int nsteps = m_end > m_begin ? (int)((m_end - m_begin) >> 7) : 0;
     const int64_t g0 = m_begin >> 7;                       // first global step (4 steps per image)
 
-    if (warp == 0) {
-        // ======================= TMA producer 1: X block k (k = 0 .. nsteps, the last one only feeds the one-pixel halo)
-        if (lane == 0 && nsteps > 0) {
+    if (warp < 4) {
+        setmaxnreg_dec<kC1WRegsProducer>();
+        if (warp == 0 && lane == 0 && nsteps > 0) {
+            // =================== TMA producer 1: X block k (k = 0 .. nsteps, the last one only feeds the one-pixel halo)
             auto image_of = [&](int64_t g) -> int {
                 int64_t img = g >> 2;
                 if (img >= p.n) img = p.n - 1;             // the halo block after the very last step: any mapped block will do
@@ -369,11 +382,9 @@ __global__ void __launch_bounds__(kC1WThreads, 1) tc_conv1_wgrad_u8(const __grid
                 mbar_arrive_expect_tx(&xfull[xs], (uint32_t)kC1WBlock);
                 tma_load_3d(smem_u32(sX + (size_t)xs * kC1WBlock), &tmX, (int)(g & 3) * 128, 0, z, &xfull[xs]);
             }
-        }
-    } else if (warp == 1) {
-        // ======================= TMA producer 2: the dY rows of step k.  The tail of stage s is read by step k + 1 (b = 1), so
-        // stage s is reloaded (step k + YS) once steps k and k + 1 have both been consumed: the ring is YS - 1 steps deep.
-        if (lane == 0) {
+        } else if (warp == 1 && lane == 0) {
+            // =================== TMA producer 2: the dY rows of step k.  The tail of stage s is read by step k + 1 (b = 1),
+            // so stage s is reloaded (step k + YS) once steps k and k + 1 have both been consumed: the ring is YS - 1 steps deep.
             for (int k = 0; k < nsteps; ++k) {
                 const int64_t g = g0 + k;
                 const int ys = k % YS;
@@ -383,7 +394,8 @@ __global__ void __launch_bounds__(kC1WThreads, 1) tc_conv1_wgrad_u8(const __grid
                 if (ys == 0) tma_load_3d(smem_u32(sYpad), &tmYpad, 0, (int)(g & 3) * 128 - kC1WYPadRows, (int)(g >> 2), &yfull[ys]);
             }
         }
-    } else if (warp >= 4 && warp < 8) {
+    } else if (warp < 8) {
+        setmaxnreg_dec<kC1WRegsBias>();
         // ======================= bias warps: bias gradient = column sums of dY from the staged tiles (fp32, fixed order)
         const int tb = tid - 128;
         const int rq = tb >> 2, c16 = tb & 3;
@@ -423,19 +435,22 @@ __global__ void __launch_bounds__(kC1WThreads, 1) tc_conv1_wgrad_u8(const __grid
             sBias[tb] = t * kU8Bias;
         }
         named_bar(2, 384);                                  // sBias is ready for the wgmma warpgroups' drain
-    } else if (warp >= 8) {
+    } else {
+        setmaxnreg_inc<kC1WRegsMma>();
         // ======================= wgmma warpgroup h: A = fp16 fragments of the pixel stream X[k + h] built in registers,
-        // B = the step's dY rows at offsets 0 (b = 0) and -21 (b = 1); 8 K-steps of 16 positions per step
+        // B = the step's dY rows at offsets -21 (b = 1, columns 0-31) and 0 (b = 0, columns 32-63) as one N = 64 operand;
+        // 8 K-steps of 16 positions per step.  Every accumulator column sees the same MMAs in the same K order as with two
+        // N = 32 MMAs per K-step, but a wgmma with A in registers holds the issuing warp for about as long as the MMA
+        // runs, and one m64n64k16 takes far less of that time than two m64n32k16.
+        //   d[4 j + e], j < 4: b = 1, channels 8 j + 2 qd (+1);  d[16 + 4 j + e]: b = 0, the same channels
         const int h = (warp - 8) >> 2, wt = tid & 127, qd = lane & 3;
         const int c0 = ((wt >> 5) << 4) + (lane >> 2);     // fragment rows c0 and c0 + 8 = channels
         // this thread's pixel pairs start at byte 2 qd + h and 8 + 2 qd + h of each 16-position chunk: words (qd >> 1) [+ 2]
         const bool up = qd >= 2;
         const uint32_t pb = (uint32_t)((2 * qd + h) & 3), psel = pb | ((pb + 1) << 4);
-        float d[2][16];
+        float d[32];
 #pragma unroll
-        for (int b = 0; b < 2; ++b)
-#pragma unroll
-            for (int e = 0; e < 16; ++e) d[b][e] = 0.f;
+        for (int e = 0; e < 32; ++e) d[e] = 0.f;
         for (int it = 0; it < nsteps; ++it) {
             const int xm = it % XS, xh = (it + 1) % XS, ys = it % YS;
             mbar_wait(&xfull[xm], (it / XS) & 1);
@@ -466,20 +481,14 @@ __global__ void __launch_bounds__(kC1WThreads, 1) tc_conv1_wgrad_u8(const __grid
             }
             mbar_wait(&yfull[ys], (it / YS) & 1);
             wgmma_fence();                                   // the A fragments were just written by ordinary instructions
-            const uint32_t y0 = smem_u32(sYb + (size_t)ys * kC1WYBytes);
+            const uint64_t yd = desc_mnmajor_sw64(smem_u32(sYb + (size_t)ys * kC1WYBytes) - kC1WShift * 64, kC1WShift * 64);
 #pragma unroll
-            for (int kk = 0; kk < 8; ++kk) {
-#pragma unroll
-                for (int b = 0; b < 2; ++b)
-                    wgmma_f16_rs_n32_tb(d[b], a[kk], desc_mnmajor_sw64(y0 - (uint32_t)(b * kC1WShift * 64)) + 64 * kk,
-                                        (it | kk) != 0 ? 1u : 0u);
-            }
+            for (int kk = 0; kk < 8; ++kk) wgmma_f16_rs_n64_tb(d, a[kk], yd + 64 * kk, (it | kk) != 0 ? 1u : 0u);
             wgmma_commit();
             wgmma_wait<0>();
             if (lane == 0) mbar_arrive(&yempty[ys]);
         }
-        wgmma_fence_operands(d[0]);
-        wgmma_fence_operands(d[1]);
+        wgmma_fence_operands(d);
         named_bar(2, 384);
         float* wsc = p.ws + (int64_t)blockIdx.x * 256 * 64;
 #pragma unroll
@@ -489,9 +498,8 @@ __global__ void __launch_bounds__(kC1WThreads, 1) tc_conv1_wgrad_u8(const __grid
                 float* dst = wsc + (int64_t)((2 * b + h) * 64 + c0 + 8 * r) * 64;
 #pragma unroll
                 for (int j = 0; j < 4; ++j) {
-                    const int co = 8 * j + 2 * qd;
-                    *reinterpret_cast<float2*>(dst + co) =
-                        make_float2(d[b][4 * j + 2 * r] - sBias[co], d[b][4 * j + 2 * r + 1] - sBias[co + 1]);
+                    const int co = 8 * j + 2 * qd, e = (b == 0 ? 16 : 0) + 4 * j + 2 * r;
+                    *reinterpret_cast<float2*>(dst + co) = make_float2(d[e] - sBias[co], d[e + 1] - sBias[co + 1]);
                 }
             }
         }
