@@ -308,7 +308,11 @@ class LSTMAgent(KernelAgent):
     Execution: fp32 kernels of libb200rl, no autograd.  The trunk and the input-gate GEMM ``x W_ih^T + b_ih`` run once over
     ALL steps of a sequence; per step there is one small GEMM ``h' W_hh^T + b_hh`` and one fused cell kernel.  The backward
     pass is explicit back-propagation through time (one cell-backward kernel + one ``dgates W_hh`` GEMM per step), after
-    which the weight gradients of both LSTM matrices and of the trunk are single GEMMs over the whole sequence."""
+    which the weight gradients of both LSTM matrices and of the trunk are single GEMMs over the whole sequence.
+    ``precision = "bf16"`` runs the whole network on the tensor cores instead (ops.LSTMAgentBf16; uint8 frames
+    [*, 1, 84, 84] only): one launch per sequence for the recurrence in each direction."""
+
+    precision = "fp32"
 
     def __init__(self, envs):
         super().__init__()
@@ -352,13 +356,54 @@ class LSTMAgent(KernelAgent):
         L = self.lstm
         self.l_ih = nets.Linear(None, None, L.weight_ih_l0.data, L.bias_ih_l0.data, L.weight_ih_l0.grad, L.bias_ih_l0.grad)
         self.l_hh = nets.Linear(None, None, L.weight_hh_l0.data, L.bias_hh_l0.data, L.weight_hh_l0.grad, L.bias_hh_l0.grad)
+        self._tc = None
+        self._tc_dirty = True
 
     graph_capturable = False
+
+    # -- bf16 tensor-core plan ("--precision bf16") ------------------------------
+    def params_updated(self):
+        """Call after the optimiser changed the flat parameters: the packed bf16 operands are stale."""
+        self._tc_dirty = True
+
+    def _tc_plan(self):
+        f = self._flat
+        if self._tc is None:
+            self._tc = ops.LSTMAgentBf16(self.num_actions, f.flat.device)
+            assert f.flat.numel() >= self._tc.param_count
+        if self._tc_dirty:
+            self._tc.pack(f.flat)
+            self._tc_dirty = False
+        return self._tc
+
+    def load_state_dict(self, *a, **k):
+        out = super().load_state_dict(*a, **k)
+        self._tc_dirty = True
+        return out
+
+    def _tc_states(self, x, lstm_state, done, rows, keep):
+        ops.LSTMAgentBf16.check_obs(x)
+        H = self.hidden_size
+        h0 = lstm_state[0].reshape(-1, H).to(torch.float32).contiguous()
+        c0 = lstm_state[1].reshape(-1, H).to(torch.float32).contiguous()
+        n = h0.shape[0]
+        total = rows.numel() if rows is not None else x.shape[0]
+        assert total % n == 0, "the sequence batch must be steps x envs"
+        S = total // n
+        done = done.reshape(-1).to(torch.float32).contiguous()
+        x = x.contiguous()
+        tc = self._tc_plan()
+        self._tc_head, h, c = tc.forward(x, rows, S, n, self._flat.flat, h0, c0, done)
+        if keep:
+            self._tc_seq = (x, rows, S, n, done)
+        return tc.act_tensors(S, n)["hseq"], (h.view(1, n, H), c.view(1, n, H))
 
     # ------------------------------------------------------------------ forward
     def get_states(self, x, lstm_state, done, rows=None, keep=False):
         """hidden [S*n, H], (h_S, c_S): ``x`` = S*n frames (or ``rows`` gathering them from a larger buffer), time-major."""
         self.flat
+        if self.precision == "bf16":
+            return self._tc_states(x, lstm_state, done, rows, keep)
         H = self.hidden_size
         h, c = lstm_state[0].reshape(-1, H).contiguous(), lstm_state[1].reshape(-1, H).contiguous()
         n = h.shape[0]
@@ -388,7 +433,8 @@ class LSTMAgent(KernelAgent):
         return hidden.view(S * n, H), (h.reshape(1, n, H).clone(), c.reshape(1, n, H).clone())
 
     def _heads(self, hidden):
-        out = self.head.fwd(hidden)
+        # bf16: the forward that produced ``hidden`` computed the heads too
+        out = self._tc_head if self.precision == "bf16" else self.head.fwd(hidden)
         A = self.num_actions
         return out[:, :A], out[:, A]
 
@@ -400,7 +446,7 @@ class LSTMAgent(KernelAgent):
     def get_action_and_value(self, x, lstm_state, done, action=None, rows=None, keep=False):
         hidden, lstm_state = self.get_states(x, lstm_state, done, rows=rows, keep=keep)
         logits, value = self._heads(hidden)
-        if keep:
+        if keep and self.precision != "bf16":
             self._seq["logits"], self._seq["value"] = logits, value
         m, A = logits.shape
         if action is None:
@@ -425,6 +471,11 @@ class LSTMAgent(KernelAgent):
 
     # ----------------------------------------------------------------- backward
     def backward(self, dhead):
+        if self.precision == "bf16":
+            x, rows, S, n, done = self._tc_seq
+            self._tc.backward(x, rows, S, n, self._flat.flat, done, dhead, self._flat.grad)
+            self._tc_seq = None
+            return
         q = self._seq
         S, n, H = q["S"], q["n"], self.hidden_size
         hidden = q["hidden"].view(S * n, H)

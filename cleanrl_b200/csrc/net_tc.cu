@@ -41,6 +41,7 @@
 #include "tc_aux.cuh"
 #include "tc_heads.cuh"
 #include "tc_heads_wide.cuh"
+#include "tc_lstm.cuh"
 
 // =====================================================================================
 // Host side: NatureCNN plan over the kernels above (C-ABI entry points, include/b200rl.h)
@@ -55,7 +56,9 @@ struct NatureLayout {
     int64_t w1f, w2f, w2dg, w3f, w3dg, wfcf, wfcdg, w1l, w1sc, packed_total;
     // wide heads only: G = A+1 padded to kWideHeadPad; whf bf16 [G,512], whdg bf16 [512,G], hbp f32 [G]
     bool wide; int G; int64_t whf, whdg, hbp;
-    explicit NatureLayout(int A_) : A(A_) {
+    // recurrent agent only (-1 otherwise): LSTM tensors (params) and the packed bf16 W_hh [512][128]
+    int64_t wih, whh, bih, bhh, whhp;
+    explicit NatureLayout(int A_) : A(A_), wih(-1), whh(-1), bih(-1), bhh(-1), whhp(-1) {
         int64_t o = 0;
         c1w = o; o += 32 * 4 * 8 * 8;  c1b = o; o += 32;
         c2w = o; o += 64 * 32 * 4 * 4; c2b = o; o += 64;
@@ -82,6 +85,37 @@ struct NatureLayout {
             whdg = q; q += (int64_t)G * 512;
             hbp = q; q += (int64_t)G * 2;
         }
+        packed_total = q;
+    }
+    // LSTMAgent._param_order: the trunk with conv1.w [32,1,8,8], then weight_ih [512,512], weight_hh [512,128], bias_ih,
+    // bias_hh, then the heads over the 128 hidden units.  The input projection W_ih is packed as a wide head (G = 512
+    // outputs over the 512 features: whf, whdg, hbp = b_ih); conv1 is packed for the single-frame kernel (w1f [32][64]).
+    struct Lstm {};
+    NatureLayout(int A_, Lstm) : A(A_) {
+        int64_t o = 0;
+        c1w = o; o += 32 * 8 * 8;      c1b = o; o += 32;
+        c2w = o; o += 64 * 32 * 4 * 4; c2b = o; o += 64;
+        c3w = o; o += 64 * 64 * 3 * 3; c3b = o; o += 64;
+        fcw = o; o += 512 * 3136;      fcb = o; o += 512;
+        wih = o; o += 512 * 512;       whh = o; o += 512 * 128;
+        bih = o; o += 512;             bhh = o; o += 512;
+        hw = o;  o += (int64_t)(A + 1) * 128;
+        hb = o;  o += A + 1;
+        total = o;
+        int64_t q = 0;
+        w1f = q; q += 32 * 64;
+        w2f = q; q += 64 * 512;
+        w2dg = q; q += 4 * 32 * 256;
+        w3f = q; q += 64 * 576;
+        w3dg = q; q += 64 * 576;
+        wfcf = q; q += 512 * 3136;
+        wfcdg = q; q += 3136 * 512;
+        w1l = w1sc = -1;
+        wide = true; G = 512;
+        whf = q; q += 512 * 512;
+        whdg = q; q += 512 * 512;
+        hbp = q; q += 512 * 2;
+        whhp = q; q += 512 * 128;
         packed_total = q;
     }
 };
@@ -209,6 +243,178 @@ static size_t wide_dhead_bytes(int64_t n, const NatureLayout& L) { return ((size
 static size_t wide_small_bytes(int64_t n, const NatureLayout& L) {
     return wide_dhead_bytes(n, L) + (size_t)ceil_div(n, wide_colsum_rows(n)) * (L.A + 1) * 4;
 }
+
+// ---- the parts of the NatureCNN plan that the recurrent agent shares (same kernels, same launches)
+// conv2 -> conv3 -> fc: act1 (2x2 cells) -> hid [n,512] (ReLU bits in m4)
+static int trunk_fwd(const NatureLayout& L, const NatureActs& Q, const float* params, const bf16* P, bf16* act, int64_t n,
+                     cudaStream_t s) {
+    int rc;
+    KGemmParams p;
+    WinParams wp;
+    // conv2: 2x2 window conv on the 128-channel cells -> act2 [n,9,9,64]
+    win_defaults(wp); win_conv2(wp, act + Q.act1, n);
+    wp.Bw = P + L.w2f; wp.N = 64; wp.vH = 9; wp.vW = 9; wp.out_mode = WOUT_DENSE; wp.out = act + Q.act2;
+    wp.bias = params + L.c2b; wp.relu = 1; wp.mask_out = reinterpret_cast<uint32_t*>(act + Q.m2);
+    { ProfScope ps(s, "conv2_fwd", 2.0 * n * 81 * 64 * 512, (double)n * ((12800 + 5184) * 2 + 648));
+      if ((rc = launch_conv_win_t<128, 2, 2, 4>(wp, s, "naturecnn/conv2"))) return rc; }
+    // conv3: 3x3 window conv -> act3 [n,7,7,64]
+    win_defaults(wp); win_conv3(wp, act + Q.act2, n);
+    wp.Bw = P + L.w3f; wp.N = 64; wp.vH = 7; wp.vW = 7; wp.out_mode = WOUT_DENSE; wp.out = act + Q.act3;
+    wp.bias = params + L.c3b; wp.relu = 1; wp.mask_out = reinterpret_cast<uint32_t*>(act + Q.m3);
+    { ProfScope ps(s, "conv3_fwd", 2.0 * n * 49 * 64 * 576, (double)n * ((5184 + 3136) * 2 + 392));
+      if ((rc = launch_conv_win_t<128, 1, 4, 9>(wp, s, "naturecnn/conv3"))) return rc; }
+    // fc -> hidden [n,512]
+    gemm_rowmajor(p, act + Q.act3, n, 49);
+    p.Bw = P + L.wfcf; p.N = 512; p.out = act + Q.hid; p.ldo = 512; p.bias = params + L.fcb; p.relu = 1;
+    p.mask_out = reinterpret_cast<uint32_t*>(act + Q.m4);
+    { ProfScope ps(s, "fc_fwd", 2.0 * n * 512 * 3136, (double)n * (3136 + 512) * 2 + 512.0 * 3136 * 2);
+      // small batches (rollout step): narrower N tiles => 4x more CTAs for the same work
+      if (n <= 8192) { if ((rc = launch_gemm_tma<64, 6>(p, s, "naturecnn/fc"))) return rc; }
+      else if ((rc = launch_gemm_tma<128, 4>(p, s, "naturecnn/fc"))) return rc; }
+    return B200RL_OK;
+}
+
+// fc -> conv2 backward: dhid (ReLU-masked) -> fc, conv3, conv2 weight gradients and d(act1) on the 21x21 grid (fp16 x
+// kDact1Scale when `dact1_f16`, for the uint8 conv1 weight gradient; bf16 otherwise).  `tail_ready_event` is recorded
+// when grads[fcw ..) is final.
+static int trunk_bwd(const NatureLayout& L, const NatureActs& Q, const bf16* P, bf16* act, float* grads, int64_t n,
+                     float* wsbig, float* wssmall, void* tail_ready_event, bool dact1_f16, cudaStream_t s) {
+    int rc;
+    KGemmParams p;
+    // ---- fc: dW[o][c*49+p] = sum_m dhid[m][o] * act3[m][p*64+c]
+    {
+        const WPlan pl = wgrad_plan(n, kFcSplits, 64);
+        { ProfScope ps(s, "fc_wgrad", 2.0 * n * 512 * 3136, (double)n * (3136 + 512) * 2 + 512.0 * 3136 * 4);
+          CUtensorMap tmX, tmY;
+          if ((rc = make_tmap_2d(&tmX, act + Q.dhid, n, 512, 64, "naturecnn/fc_wgrad"))) return rc;
+          if ((rc = make_tmap_2d(&tmY, act + Q.act3, n, 3136, 64, "naturecnn/fc_wgrad"))) return rc;
+          const size_t smem = (size_t)4 * (kFcWgradXChunks + kFcWgradYChunks) * 64 * 128 + 1024;
+          static SmemAttrCache attr;
+          if ((rc = attr.ensure(tc_wgrad_tma, smem, "naturecnn/fc_wgrad"))) return rc;
+          // X = dhid (512 columns), Y = act3 (3136 columns, the last Y group partly past the end: zero-filled by TMA)
+          const dim3 grid(pl.splits, 512 / (64 * kFcWgradXChunks), (unsigned)ceil_div(3136, 64 * kFcWgradYChunks));
+          tc_wgrad_tma<<<grid, kWgradTmaThreads, smem, s>>>(tmX, tmY, n, pl.rows_per_cta, wsbig);
+          if ((rc = check_launch("naturecnn/fc_wgrad"))) return rc; }
+        { ProfScope ps(s, "wgrad_fold_bias", 0, 0);
+          note_launches(1); tc_fold_fc<<<(unsigned)ceil_div((int64_t)512 * 3136, 256), 256, 0, s>>>(wsbig, pl.splits, 512, 13 * 256, 512, 3136, 64, 49, 1.f, grads + L.fcw);
+          if ((rc = colsum(act + Q.dhid, n, 512, 512, wssmall, grads + L.fcb, s))) return rc; }
+        // grads[fcw .. total) (fc weight + bias, both heads) are final: the caller may start exchanging them now
+        if (tail_ready_event) {
+            cudaError_t e = cudaEventRecord(reinterpret_cast<cudaEvent_t>(tail_ready_event), s);
+            if (e != cudaSuccess) return fail(B200RL_ERR_CUDA, "naturecnn_backward: cudaEventRecord: %s", cudaGetErrorString(e));
+        }
+        // dact3_pre = (dhid . Wfc) * (act3 > 0), written on the 9x9 linear grid and the zero-padded 11x11 grid
+        gemm_rowmajor(p, act + Q.dhid, n, 8);
+        p.Bw = P + L.wfcdg; p.N = 3136; p.out = act + Q.dact3a; p.out2 = act + Q.dact3b; p.dual_dact3 = 1;
+        p.ldo = 3136; p.mask_bits = reinterpret_cast<const uint32_t*>(act + Q.m3);
+        { ProfScope ps(s, "fc_dgrad", 2.0 * n * 512 * 3136, (double)n * ((3136 + 512) * 2 + 392) + 512.0 * 3136 * 2);
+          if ((rc = launch_gemm_tma<128, 4>(p, s, "naturecnn/fc_dgrad"))) return rc; }
+    }
+    WGradWinParams gw;
+    WinParams wp;
+    FoldWin fw;
+    // ---- conv3: dW from act2 windows x dact3 (9x9 grid), then dact2 = full correlation of padded dact3 with W3
+    {
+        wgw_defaults(gw);
+        gw.X = act + Q.act2; gw.M = n * 81; gw.n = (int)n; gw.G = 81; gw.cpr = 1; gw.nslots = 10; gw.WRX = round8(128 + 20);
+        for (int t = 0; t < 9; ++t) gw.shift[t] = (t / 3) * 9 + (t % 3);
+        const int st[10] = {0, 1, 2, 3, 4, 5, 6, 7, 7, 8};      // slot 8 duplicates tap 7 so that tap 8 has a partner
+        for (int k = 0; k < 10; ++k) { gw.slot_tap[k] = st[k]; gw.slot_cc[k] = 0; }
+        gw.Y = act + Q.dact3a; gw.ldy = 64; gw.ncolsY = 64;
+        const WPlan pl = wgrad_plan(n * 81, kC3Ctas, 128);
+        gw.rows_per_cta = pl.rows_per_cta; gw.ws = wsbig; gw.wsb = wssmall;
+        { ProfScope ps(s, "conv3_wgrad", 2.0 * n * 49 * 64 * 576, (double)n * (5184 + 5184) * 2);
+          if ((rc = launch_wgrad_win(gw, pl.splits, s, "naturecnn/conv3_wgrad"))) return rc; }
+        memset(&fw, 0, sizeof(fw));
+        fw.layer = 3; fw.S = pl.splits; fw.nslots = 10; fw.Cout = 64; fw.scale = 1.f; fw.bscale = 1.f;
+        for (int k = 0; k < 10; ++k) { fw.slot_tap[k] = st[k]; fw.slot_skip[k] = (k == 8); }
+        { ProfScope ps(s, "wgrad_fold_bias", 0, 0);
+          fw.wsb = wssmall; fw.db = grads + L.c3b;
+          tc_fold_win<<<(unsigned)ceil_div(640 * 64 + 64, 32), 256, 0, s>>>(wsbig, fw, grads + L.c3w);
+          if ((rc = check_launch("naturecnn/conv3_fold"))) return rc; }
+        win_defaults(wp);
+        wp.A = act + Q.dact3b; wp.n = (int)n; wp.G = 121; wp.Wp = 11; wp.M = n * 121; wp.ntaps = 9;
+        for (int ky = 0; ky < 3; ++ky) for (int kx = 0; kx < 3; ++kx) wp.shift[ky * 3 + kx] = (2 - ky) * 11 + (2 - kx);
+        wp.WR = round8(128 + 24);
+        wp.Bw = P + L.w3dg; wp.N = 64; wp.vH = 9; wp.vW = 9; wp.out_mode = WOUT_DACT2;
+        wp.out = act + Q.dact2a; wp.out2 = act + Q.dact2b; wp.mask_bits = reinterpret_cast<const uint32_t*>(act + Q.m2);
+        { ProfScope ps(s, "conv3_dgrad", 2.0 * n * 81 * 64 * 576, (double)n * ((7744 + 6400 + 7744) * 2 + 648));
+          if ((rc = launch_conv_win_t<128, 1, 4, 9>(wp, s, "naturecnn/conv3_dgrad"))) return rc; }
+    }
+    // ---- conv2: dW from act1 cell windows x dact2 (10x10 grid); dact1 = one N=128 GEMM over the 4 stride-parity
+    //      classes (the 4 channel groups of a cell)
+    {
+        wgw_defaults(gw);
+        gw.X = act + Q.act1; gw.M = n * 100; gw.n = (int)n; gw.G = 100; gw.cpr = 2; gw.nslots = 8; gw.WRX = round8(128 + 11);
+        gw.shift[0] = 0; gw.shift[1] = 1; gw.shift[2] = 10; gw.shift[3] = 11;
+        for (int k = 0; k < 8; ++k) { gw.slot_tap[k] = k >> 1; gw.slot_cc[k] = k & 1; }
+        gw.Y = act + Q.dact2a; gw.ldy = 64; gw.ncolsY = 64;
+        const WPlan pl = wgrad_plan(n * 100, kC2Ctas, 128);
+        gw.rows_per_cta = pl.rows_per_cta; gw.ws = wsbig; gw.wsb = wssmall;
+        { ProfScope ps(s, "conv2_wgrad", 2.0 * n * 81 * 64 * 512, (double)n * (12800 + 6400) * 2);
+          if ((rc = launch_wgrad_win(gw, pl.splits, s, "naturecnn/conv2_wgrad"))) return rc; }
+        memset(&fw, 0, sizeof(fw));
+        fw.layer = 2; fw.S = pl.splits; fw.nslots = 8; fw.Cout = 64; fw.scale = 1.f; fw.bscale = 1.f;
+        for (int k = 0; k < 8; ++k) { fw.slot_tap[k] = k >> 1; fw.slot_cc[k] = k & 1; }
+        { ProfScope ps(s, "wgrad_fold_bias", 0, 0);
+          fw.wsb = wssmall; fw.db = grads + L.c2b;
+          tc_fold_win<<<(unsigned)ceil_div(512 * 64 + 64, 32), 256, 0, s>>>(wsbig, fw, grads + L.c2w);
+          if ((rc = check_launch("naturecnn/conv2_fold"))) return rc; }
+        win_defaults(wp);
+        wp.A = act + Q.dact2b; wp.n = (int)n; wp.G = 121; wp.Wp = 11; wp.M = n * 121; wp.ntaps = 4;
+        for (int a = 0; a < 2; ++a) for (int b = 0; b < 2; ++b) wp.shift[a * 2 + b] = (1 - a) * 11 + (1 - b);
+        wp.WR = round8(128 + 12);
+        wp.Bw = P + L.w2dg; wp.N = 128; wp.vH = 10; wp.vW = 10; wp.out_mode = WOUT_DACT1;
+        wp.out = act + Q.dact1; wp.mask_bits = reinterpret_cast<const uint32_t*>(act + Q.m1);
+        if (dact1_f16) { wp.out_f16 = 1; wp.scale = kDact1Scale; }     // fp16 x 2^12 for the uint8 conv1 wgrad
+        { ProfScope ps(s, "conv2_dgrad", 2.0 * n * 400 * 32 * 256, (double)n * ((7744 + 14112) * 2 + 1600));
+          if ((rc = launch_conv_win<128, 1, 4, 4>(wp, s, "naturecnn/conv2_dgrad"))) return rc; }
+    }
+    return B200RL_OK;
+}
+
+// wide head forward: out [n, A1] (fp32, row stride A1) = hid . Wh^T + bh over the zero-padded [G, 512] operands
+static int wide_head_fwd(const NatureLayout& L, const bf16* P, const bf16* hid, int64_t n, int A1, float* out, cudaStream_t s) {
+    KGemmParams p;
+    gemm_rowmajor(p, hid, n, 8);
+    p.Bw = P + L.whf; p.N = L.G; p.bias = reinterpret_cast<const float*>(P + L.hbp);
+    p.out_f32 = out; p.ldo = A1; p.ncols_f32 = A1;
+    return launch_gemm_tma<128, 4>(p, s, "wide_heads");
+}
+
+// wide head backward: dhead [n, A1] fp32 -> bf16 [n, G] (left at the start of wssmall); dW = dhead_bf16^T . hid on wgmma
+// (row splits folded in order), db = fp32 column sums of dhead; dhid = (dhead_bf16 . Wh) * (hid > 0) on wgmma
+static int wide_head_bwd(const NatureLayout& L, const bf16* P, const float* dhead, int64_t n, int A1, const bf16* hid, bf16* dhid,
+                         const uint32_t* hid_bits, float* dW, float* db, float* wsbig, float* wssmall, cudaStream_t s) {
+    int rc;
+    KGemmParams p;
+    bf16* dh16 = reinterpret_cast<bf16*>(wssmall);
+    float* dbpart = reinterpret_cast<float*>(reinterpret_cast<char*>(wssmall) + wide_dhead_bytes(n, L));
+    int cb = (int)ceil_div(n * L.G, 256); if (cb > num_sms() * 8) cb = num_sms() * 8;
+    tc_head_dhead_bf16<<<cb, 256, 0, s>>>(dhead, n, A1, L.G, dh16);
+    const int64_t rpb = wide_colsum_rows(n);
+    const int nb = (int)ceil_div(n, rpb);
+    tc_colsum_f32_partial<<<dim3(nb, (unsigned)ceil_div(A1, 128)), 128, 0, s>>>(dhead, n, A1, rpb, dbpart);
+    tc_colsum_f32_final<<<(unsigned)ceil_div(A1, 128), 128, 0, s>>>(dbpart, nb, A1, db);
+    if ((rc = check_launch("wide_heads_bias", 3))) return rc;
+    const WPlan pl = wgrad_plan(n, kFcSplits, 64);
+    CUtensorMap tmX, tmY;
+    if ((rc = make_tmap_2d(&tmX, dh16, n, L.G, 64, "wide_heads_wgrad"))) return rc;
+    if ((rc = make_tmap_2d(&tmY, hid, n, 512, 64, "wide_heads_wgrad"))) return rc;
+    const size_t smem = (size_t)4 * (kFcWgradXChunks + kFcWgradYChunks) * 64 * 128 + 1024;
+    static SmemAttrCache attr;
+    if ((rc = attr.ensure(tc_wgrad_tma, smem, "wide_heads_wgrad"))) return rc;
+    const dim3 grid(pl.splits, L.G / (64 * kFcWgradXChunks), 512 / (64 * kFcWgradYChunks));
+    tc_wgrad_tma<<<grid, kWgradTmaThreads, smem, s>>>(tmX, tmY, n, pl.rows_per_cta, wsbig);
+    tc_fold_head_wide<<<(unsigned)ceil_div((int64_t)A1 * 512, 256), 256, 0, s>>>(wsbig, pl.splits, A1, L.G, dW);
+    if ((rc = check_launch("wide_heads_wgrad", 2))) return rc;
+    gemm_rowmajor(p, dh16, n, L.G / 64);
+    p.Bw = P + L.whdg; p.N = 512; p.out = dhid; p.ldo = 512;
+    p.mask_bits = hid_bits;
+    if (n <= 8192) { if ((rc = launch_gemm_tma<64, 6>(p, s, "wide_heads_dgrad"))) return rc; }
+    else if ((rc = launch_gemm_tma<128, 4>(p, s, "wide_heads_dgrad"))) return rc;
+    return B200RL_OK;
+}
 }  // namespace b200rl
 
 extern "C" int64_t b200rl_naturecnn_param_count(int A) { return A >= 1 ? NatureLayout(A).total : -1; }
@@ -297,7 +503,6 @@ extern "C" int b200rl_naturecnn_bf16_forward(const void* obs, int obs_format, co
     bf16* act = reinterpret_cast<bf16*>(acts);
     cudaStream_t s = (cudaStream_t)stream;
     int rc;
-    KGemmParams p;
     WinParams wp;
     // conv1: 2x2 window conv on space-to-depth frames -> act1 as 2x2 cells [n,10,10,128]
     const bf16* x0 = reinterpret_cast<const bf16*>(obs);
@@ -322,33 +527,11 @@ extern "C" int b200rl_naturecnn_bf16_forward(const void* obs, int obs_format, co
     { ProfScope ps(s, "conv1_fwd", 2.0 * n * 400 * 32 * 256, (double)n * ((28224 + 12800) * 2 + 1600));
       if ((rc = launch_conv_win<32, 1, 9, 4>(wp, s, "naturecnn/conv1"))) return rc; }
     }
-    // conv2: 2x2 window conv on the 128-channel cells -> act2 [n,9,9,64]
-    win_defaults(wp); win_conv2(wp, act + Q.act1, n);
-    wp.Bw = P + L.w2f; wp.N = 64; wp.vH = 9; wp.vW = 9; wp.out_mode = WOUT_DENSE; wp.out = act + Q.act2;
-    wp.bias = params + L.c2b; wp.relu = 1; wp.mask_out = reinterpret_cast<uint32_t*>(act + Q.m2);
-    { ProfScope ps(s, "conv2_fwd", 2.0 * n * 81 * 64 * 512, (double)n * ((12800 + 5184) * 2 + 648));
-      if ((rc = launch_conv_win_t<128, 2, 2, 4>(wp, s, "naturecnn/conv2"))) return rc; }
-    // conv3: 3x3 window conv -> act3 [n,7,7,64]
-    win_defaults(wp); win_conv3(wp, act + Q.act2, n);
-    wp.Bw = P + L.w3f; wp.N = 64; wp.vH = 7; wp.vW = 7; wp.out_mode = WOUT_DENSE; wp.out = act + Q.act3;
-    wp.bias = params + L.c3b; wp.relu = 1; wp.mask_out = reinterpret_cast<uint32_t*>(act + Q.m3);
-    { ProfScope ps(s, "conv3_fwd", 2.0 * n * 49 * 64 * 576, (double)n * ((5184 + 3136) * 2 + 392));
-      if ((rc = launch_conv_win_t<128, 1, 4, 9>(wp, s, "naturecnn/conv3"))) return rc; }
-    // fc -> hidden [n,512]
-    gemm_rowmajor(p, act + Q.act3, n, 49);
-    p.Bw = P + L.wfcf; p.N = 512; p.out = act + Q.hid; p.ldo = 512; p.bias = params + L.fcb; p.relu = 1;
-    p.mask_out = reinterpret_cast<uint32_t*>(act + Q.m4);
-    { ProfScope ps(s, "fc_fwd", 2.0 * n * 512 * 3136, (double)n * (3136 + 512) * 2 + 512.0 * 3136 * 2);
-      // small batches (rollout step): narrower N tiles => 4x more CTAs for the same work
-      if (n <= 8192) { if ((rc = launch_gemm_tma<64, 6>(p, s, "naturecnn/fc"))) return rc; }
-      else if ((rc = launch_gemm_tma<128, 4>(p, s, "naturecnn/fc"))) return rc; }
+    if ((rc = trunk_fwd(L, Q, params, P, act, n, s))) return rc;
     if (L.wide) {
         // wide heads on wgmma: head_out [n, A+1] (fp32) = hidden . Wh^T + bh, over the zero-padded [G, 512] weights
-        gemm_rowmajor(p, act + Q.hid, n, 8);
-        p.Bw = P + L.whf; p.N = L.G; p.bias = reinterpret_cast<const float*>(P + L.hbp);
-        p.out_f32 = head_out; p.ldo = A + 1; p.ncols_f32 = A + 1;
         ProfScope ps(s, "heads_fwd", 2.0 * n * 512 * (A + 1), (double)n * (1024 + 4 * (A + 1)) + (double)L.G * 1024);
-        return launch_gemm_tma<128, 4>(p, s, "naturecnn/heads_wide");
+        return wide_head_fwd(L, P, act + Q.hid, n, A + 1, head_out, s);
     }
     // heads (fp32 math on CUDA cores): head_out [n, A+1] = [logits | value]
     { ProfScope ps(s, "heads_fwd", 2.0 * n * 512 * (A + 1), (double)n * (1024 + 4 * (A + 1)));
@@ -393,36 +576,12 @@ extern "C" int b200rl_naturecnn_bf16_backward(const void* obs, const void* obs_a
     float* wssmall = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + big);
     int rc;
     const int A1 = A + 1;
-    KGemmParams p;
     if (L.wide) {
         // ---- wide heads: dhead -> bf16 [n, G]; dbh = fp32 column sums; dWh = dhead_bf16^T . hid on wgmma (row splits
         //      folded in order); dhid_pre = (dhead_bf16 . Wh) * (hid > 0) on wgmma
-        bf16* dh16 = reinterpret_cast<bf16*>(wssmall);
-        float* dbpart = reinterpret_cast<float*>(reinterpret_cast<char*>(wssmall) + wide_dhead_bytes(n, L));
         ProfScope ps(s, "heads_bwd", 4.0 * n * 512 * A1, (double)n * (2048 + 64 + 8 * A1));
-        int cb = (int)ceil_div(n * L.G, 256); if (cb > num_sms() * 8) cb = num_sms() * 8;
-        tc_head_dhead_bf16<<<cb, 256, 0, s>>>(dhead, n, A1, L.G, dh16);
-        const int64_t rpb = wide_colsum_rows(n);
-        const int nb = (int)ceil_div(n, rpb);
-        tc_colsum_f32_partial<<<dim3(nb, (unsigned)ceil_div(A1, 128)), 128, 0, s>>>(dhead, n, A1, rpb, dbpart);
-        tc_colsum_f32_final<<<(unsigned)ceil_div(A1, 128), 128, 0, s>>>(dbpart, nb, A1, grads + L.hb);
-        if ((rc = check_launch("naturecnn/heads_wide_bias", 3))) return rc;
-        const WPlan pl = wgrad_plan(n, kFcSplits, 64);
-        CUtensorMap tmX, tmY;
-        if ((rc = make_tmap_2d(&tmX, dh16, n, L.G, 64, "naturecnn/heads_wide_wgrad"))) return rc;
-        if ((rc = make_tmap_2d(&tmY, act + Q.hid, n, 512, 64, "naturecnn/heads_wide_wgrad"))) return rc;
-        const size_t smem = (size_t)4 * (kFcWgradXChunks + kFcWgradYChunks) * 64 * 128 + 1024;
-        static SmemAttrCache attr;
-        if ((rc = attr.ensure(tc_wgrad_tma, smem, "naturecnn/heads_wide_wgrad"))) return rc;
-        const dim3 grid(pl.splits, L.G / (64 * kFcWgradXChunks), 512 / (64 * kFcWgradYChunks));
-        tc_wgrad_tma<<<grid, kWgradTmaThreads, smem, s>>>(tmX, tmY, n, pl.rows_per_cta, wsbig);
-        tc_fold_head_wide<<<(unsigned)ceil_div((int64_t)A1 * 512, 256), 256, 0, s>>>(wsbig, pl.splits, A1, L.G, grads + L.hw);
-        if ((rc = check_launch("naturecnn/heads_wide_wgrad", 2))) return rc;
-        gemm_rowmajor(p, dh16, n, L.G / 64);
-        p.Bw = P + L.whdg; p.N = 512; p.out = act + Q.dhid; p.ldo = 512;
-        p.mask_bits = reinterpret_cast<const uint32_t*>(act + Q.m4);
-        if (n <= 8192) { if ((rc = launch_gemm_tma<64, 6>(p, s, "naturecnn/heads_wide_dgrad"))) return rc; }
-        else if ((rc = launch_gemm_tma<128, 4>(p, s, "naturecnn/heads_wide_dgrad"))) return rc;
+        if ((rc = wide_head_bwd(L, P, dhead, n, A1, act + Q.hid, act + Q.dhid, reinterpret_cast<const uint32_t*>(act + Q.m4),
+                                grads + L.hw, grads + L.hb, wsbig, wssmall, s))) return rc;
     } else
     // ---- heads: dW, db, then dhid_pre = (dhead . Wh) * (hid > 0)
     {
@@ -437,95 +596,9 @@ extern "C" int b200rl_naturecnn_bf16_backward(const void* obs, const void* obs_a
         tc_heads_bwd_data<<<db_blocks, 256, (size_t)A1 * 2048, s>>>(dhead, params + L.hw, reinterpret_cast<const uint8_t*>(act + Q.m4), n, A1, 512, act + Q.dhid);
         if ((rc = check_launch("naturecnn/heads_bwd", 3))) return rc;
     }
-    // ---- fc: dW[o][c*49+p] = sum_m dhid[m][o] * act3[m][p*64+c]
-    {
-        const WPlan pl = wgrad_plan(n, kFcSplits, 64);
-        { ProfScope ps(s, "fc_wgrad", 2.0 * n * 512 * 3136, (double)n * (3136 + 512) * 2 + 512.0 * 3136 * 4);
-          CUtensorMap tmX, tmY;
-          if ((rc = make_tmap_2d(&tmX, act + Q.dhid, n, 512, 64, "naturecnn/fc_wgrad"))) return rc;
-          if ((rc = make_tmap_2d(&tmY, act + Q.act3, n, 3136, 64, "naturecnn/fc_wgrad"))) return rc;
-          const size_t smem = (size_t)4 * (kFcWgradXChunks + kFcWgradYChunks) * 64 * 128 + 1024;
-          static SmemAttrCache attr;
-          if ((rc = attr.ensure(tc_wgrad_tma, smem, "naturecnn/fc_wgrad"))) return rc;
-          // X = dhid (512 columns), Y = act3 (3136 columns, the last Y group partly past the end: zero-filled by TMA)
-          const dim3 grid(pl.splits, 512 / (64 * kFcWgradXChunks), (unsigned)ceil_div(3136, 64 * kFcWgradYChunks));
-          tc_wgrad_tma<<<grid, kWgradTmaThreads, smem, s>>>(tmX, tmY, n, pl.rows_per_cta, wsbig);
-          if ((rc = check_launch("naturecnn/fc_wgrad"))) return rc; }
-        { ProfScope ps(s, "wgrad_fold_bias", 0, 0);
-          note_launches(1); tc_fold_fc<<<(unsigned)ceil_div((int64_t)512 * 3136, 256), 256, 0, s>>>(wsbig, pl.splits, 512, 13 * 256, 512, 3136, 64, 49, 1.f, grads + L.fcw);
-          if ((rc = colsum(act + Q.dhid, n, 512, 512, wssmall, grads + L.fcb, s))) return rc; }
-        // grads[fcw .. total) (fc weight + bias, both heads) are final: the caller may start exchanging them now
-        if (tail_ready_event) {
-            cudaError_t e = cudaEventRecord(reinterpret_cast<cudaEvent_t>(tail_ready_event), s);
-            if (e != cudaSuccess) return fail(B200RL_ERR_CUDA, "naturecnn_backward: cudaEventRecord: %s", cudaGetErrorString(e));
-        }
-        // dact3_pre = (dhid . Wfc) * (act3 > 0), written on the 9x9 linear grid and the zero-padded 11x11 grid
-        gemm_rowmajor(p, act + Q.dhid, n, 8);
-        p.Bw = P + L.wfcdg; p.N = 3136; p.out = act + Q.dact3a; p.out2 = act + Q.dact3b; p.dual_dact3 = 1;
-        p.ldo = 3136; p.mask_bits = reinterpret_cast<const uint32_t*>(act + Q.m3);
-        { ProfScope ps(s, "fc_dgrad", 2.0 * n * 512 * 3136, (double)n * ((3136 + 512) * 2 + 392) + 512.0 * 3136 * 2);
-          if ((rc = launch_gemm_tma<128, 4>(p, s, "naturecnn/fc_dgrad"))) return rc; }
-    }
+    if ((rc = trunk_bwd(L, Q, P, act, grads, n, wsbig, wssmall, tail_ready_event, obs_format == B200RL_OBS_S2D_U8, s))) return rc;
     WGradWinParams gw;
-    WinParams wp;
     FoldWin fw;
-    // ---- conv3: dW from act2 windows x dact3 (9x9 grid), then dact2 = full correlation of padded dact3 with W3
-    {
-        wgw_defaults(gw);
-        gw.X = act + Q.act2; gw.M = n * 81; gw.n = (int)n; gw.G = 81; gw.cpr = 1; gw.nslots = 10; gw.WRX = round8(128 + 20);
-        for (int t = 0; t < 9; ++t) gw.shift[t] = (t / 3) * 9 + (t % 3);
-        const int st[10] = {0, 1, 2, 3, 4, 5, 6, 7, 7, 8};      // slot 8 duplicates tap 7 so that tap 8 has a partner
-        for (int k = 0; k < 10; ++k) { gw.slot_tap[k] = st[k]; gw.slot_cc[k] = 0; }
-        gw.Y = act + Q.dact3a; gw.ldy = 64; gw.ncolsY = 64;
-        const WPlan pl = wgrad_plan(n * 81, kC3Ctas, 128);
-        gw.rows_per_cta = pl.rows_per_cta; gw.ws = wsbig; gw.wsb = wssmall;
-        { ProfScope ps(s, "conv3_wgrad", 2.0 * n * 49 * 64 * 576, (double)n * (5184 + 5184) * 2);
-          if ((rc = launch_wgrad_win(gw, pl.splits, s, "naturecnn/conv3_wgrad"))) return rc; }
-        memset(&fw, 0, sizeof(fw));
-        fw.layer = 3; fw.S = pl.splits; fw.nslots = 10; fw.Cout = 64; fw.scale = 1.f; fw.bscale = 1.f;
-        for (int k = 0; k < 10; ++k) { fw.slot_tap[k] = st[k]; fw.slot_skip[k] = (k == 8); }
-        { ProfScope ps(s, "wgrad_fold_bias", 0, 0);
-          fw.wsb = wssmall; fw.db = grads + L.c3b;
-          tc_fold_win<<<(unsigned)ceil_div(640 * 64 + 64, 32), 256, 0, s>>>(wsbig, fw, grads + L.c3w);
-          if ((rc = check_launch("naturecnn/conv3_fold"))) return rc; }
-        win_defaults(wp);
-        wp.A = act + Q.dact3b; wp.n = (int)n; wp.G = 121; wp.Wp = 11; wp.M = n * 121; wp.ntaps = 9;
-        for (int ky = 0; ky < 3; ++ky) for (int kx = 0; kx < 3; ++kx) wp.shift[ky * 3 + kx] = (2 - ky) * 11 + (2 - kx);
-        wp.WR = round8(128 + 24);
-        wp.Bw = P + L.w3dg; wp.N = 64; wp.vH = 9; wp.vW = 9; wp.out_mode = WOUT_DACT2;
-        wp.out = act + Q.dact2a; wp.out2 = act + Q.dact2b; wp.mask_bits = reinterpret_cast<const uint32_t*>(act + Q.m2);
-        { ProfScope ps(s, "conv3_dgrad", 2.0 * n * 81 * 64 * 576, (double)n * ((7744 + 6400 + 7744) * 2 + 648));
-          if ((rc = launch_conv_win_t<128, 1, 4, 9>(wp, s, "naturecnn/conv3_dgrad"))) return rc; }
-    }
-    // ---- conv2: dW from act1 cell windows x dact2 (10x10 grid); dact1 = one N=128 GEMM over the 4 stride-parity
-    //      classes (the 4 channel groups of a cell)
-    {
-        wgw_defaults(gw);
-        gw.X = act + Q.act1; gw.M = n * 100; gw.n = (int)n; gw.G = 100; gw.cpr = 2; gw.nslots = 8; gw.WRX = round8(128 + 11);
-        gw.shift[0] = 0; gw.shift[1] = 1; gw.shift[2] = 10; gw.shift[3] = 11;
-        for (int k = 0; k < 8; ++k) { gw.slot_tap[k] = k >> 1; gw.slot_cc[k] = k & 1; }
-        gw.Y = act + Q.dact2a; gw.ldy = 64; gw.ncolsY = 64;
-        const WPlan pl = wgrad_plan(n * 100, kC2Ctas, 128);
-        gw.rows_per_cta = pl.rows_per_cta; gw.ws = wsbig; gw.wsb = wssmall;
-        { ProfScope ps(s, "conv2_wgrad", 2.0 * n * 81 * 64 * 512, (double)n * (12800 + 6400) * 2);
-          if ((rc = launch_wgrad_win(gw, pl.splits, s, "naturecnn/conv2_wgrad"))) return rc; }
-        memset(&fw, 0, sizeof(fw));
-        fw.layer = 2; fw.S = pl.splits; fw.nslots = 8; fw.Cout = 64; fw.scale = 1.f; fw.bscale = 1.f;
-        for (int k = 0; k < 8; ++k) { fw.slot_tap[k] = k >> 1; fw.slot_cc[k] = k & 1; }
-        { ProfScope ps(s, "wgrad_fold_bias", 0, 0);
-          fw.wsb = wssmall; fw.db = grads + L.c2b;
-          tc_fold_win<<<(unsigned)ceil_div(512 * 64 + 64, 32), 256, 0, s>>>(wsbig, fw, grads + L.c2w);
-          if ((rc = check_launch("naturecnn/conv2_fold"))) return rc; }
-        win_defaults(wp);
-        wp.A = act + Q.dact2b; wp.n = (int)n; wp.G = 121; wp.Wp = 11; wp.M = n * 121; wp.ntaps = 4;
-        for (int a = 0; a < 2; ++a) for (int b = 0; b < 2; ++b) wp.shift[a * 2 + b] = (1 - a) * 11 + (1 - b);
-        wp.WR = round8(128 + 12);
-        wp.Bw = P + L.w2dg; wp.N = 128; wp.vH = 10; wp.vW = 10; wp.out_mode = WOUT_DACT1;
-        wp.out = act + Q.dact1; wp.mask_bits = reinterpret_cast<const uint32_t*>(act + Q.m1);
-        if (obs_format == B200RL_OBS_S2D_U8) { wp.out_f16 = 1; wp.scale = kDact1Scale; }     // fp16 x 2^12 for the uint8 conv1 wgrad
-        { ProfScope ps(s, "conv2_dgrad", 2.0 * n * 400 * 32 * 256, (double)n * ((7744 + 14112) * 2 + 1600));
-          if ((rc = launch_conv_win<128, 1, 4, 4>(wp, s, "naturecnn/conv2_dgrad"))) return rc; }
-    }
     // ---- conv1 (no data gradient: the input is the observation)
     if (obs_format == B200RL_OBS_S2D_U8) {
         // uint8 channel-major frames -> fp16 wgmma operands in registers (tc_conv1_u8.cuh); 1 CTA per SM
@@ -561,6 +634,240 @@ extern "C" int b200rl_naturecnn_bf16_backward(const void* obs, const void* obs_a
           fw.wsb = wssmall; fw.db = grads + L.c1b;
           tc_fold_win<<<(unsigned)ceil_div(256 * 32 + 32, 32), 256, 0, s>>>(wsbig, fw, grads + L.c1w);
           if ((rc = check_launch("naturecnn/conv1_fold"))) return rc; }
+    }
+    return B200RL_OK;
+}
+
+// =====================================================================================
+// Recurrent agent (LSTMAgent, cleanrl/ppo_atari_lstm.py:117-160): single-frame conv1 (tc_lstm.cuh), the shared trunk,
+// W_ih as a 512-output wide head, the persistent recurrence kernels, CUDA-core heads over the 128 hidden units
+// =====================================================================================
+namespace b200rl {
+constexpr int64_t kLstmMaxRows = (int64_t)1 << 17;     // S * n
+
+struct LstmActs {           // the trunk (NatureActs, bf16 element offsets, at byte 0), then byte offsets of the LSTM tensors
+    NatureActs T;
+    int64_t gx, hseq, hm, save, cm, dgates, total;
+    explicit LstmActs(int64_t M) : T(M, false) {
+        int64_t o = (T.total * 2 + 255) & ~int64_t(255);
+        auto take = [&](int64_t bytes) { const int64_t r = o; o += (bytes + 255) & ~int64_t(255); return r; };
+        gx = take(M * 512 * 4);
+        hseq = take(M * 128 * 2);
+        hm = take(M * 128 * 2);
+        save = take(M * 640 * 4);
+        cm = take(M * 128 * 4);
+        dgates = take(M * 512 * 4);
+        total = o;
+    }
+};
+
+static bool lstm_heads_ok(int A) { return A >= 1 && A + 1 <= lstm::kMaxA1; }
+static bool lstm_sizes_ok(int64_t S, int64_t n) { return S >= 1 && n >= 1 && S <= kLstmMaxRows && n <= kLstmMaxRows && S * n <= kLstmMaxRows; }
+
+struct C1Plan { int64_t per_cta; int ctas; };
+static C1Plan lstm_conv1_plan(int64_t M) {           // whole frames per CTA, one or two waves
+    C1Plan c;
+    const int64_t want = M < kC1Ctas ? M : kC1Ctas;
+    c.per_cta = ceil_div(M, want);
+    c.ctas = (int)ceil_div(M, c.per_cta);
+    return c;
+}
+static size_t lstm_big_bytes(int64_t M, const NatureLayout& L) {
+    size_t a = 0;
+    auto mx = [&](size_t v) { if (v > a) a = v; };
+    mx((size_t)wgrad_plan(M * 100, kC2Ctas, 128).splits * 512 * 64 * 4);
+    mx((size_t)wgrad_plan(M * 81, kC3Ctas, 128).splits * 640 * 64 * 4);
+    mx((size_t)wgrad_plan(M, kFcSplits, 64).splits * 512 * (13 * 256) * 4);
+    mx(wide_big_bytes(M, L));                                              // dW_ih partials (dW_hh's are half as wide)
+    mx((size_t)lstm_conv1_plan(M).ctas * 32 * 64 * 4);
+    return (a + 255) & ~(size_t)255;
+}
+static size_t lstm_small_bytes(int64_t M, int A) {
+    const NatureLayout L(A, NatureLayout::Lstm{});
+    size_t b = 0;
+    auto mb = [&](size_t v) { if (v > b) b = v; };
+    mb(colsum_ws(M * 100, 64)); mb(colsum_ws(M * 81, 64)); mb(colsum_ws(M, 512));
+    mb(wide_dhead_bytes(M, L) + (size_t)ceil_div(M, wide_colsum_rows(M)) * 512 * 4);
+    mb((size_t)2 * ceil_div(M, heads_rows_per_block(M)) * (A + 1) * 130 * 4);
+    mb((size_t)lstm_conv1_plan(M).ctas * 32 * 4);
+    return b;
+}
+}  // namespace b200rl
+
+extern "C" int64_t b200rl_lstm_agent_param_count(int A) { return A >= 1 ? NatureLayout(A, NatureLayout::Lstm{}).total : -1; }
+extern "C" size_t b200rl_lstm_agent_bf16_packed_bytes(int A) {
+    return lstm_heads_ok(A) ? (size_t)NatureLayout(A, NatureLayout::Lstm{}).packed_total * 2 : 0;
+}
+extern "C" size_t b200rl_lstm_agent_bf16_acts_bytes(int64_t S, int64_t n) {
+    return lstm_sizes_ok(S, n) ? (size_t)LstmActs(S * n).total : 0;
+}
+extern "C" int b200rl_lstm_agent_bf16_acts_layout(int64_t S, int64_t n, int64_t* offsets) {
+    B200RL_REQUIRE(offsets, "lstm_acts_layout: null pointer");
+    B200RL_REQUIRE(lstm_sizes_ok(S, n), "lstm_acts_layout: S=%lld n=%lld out of range", (long long)S, (long long)n);
+    const LstmActs Q(S * n);
+    const int64_t v[B200RL_LSTM_ACTS_TENSORS] = {Q.T.act1 * 2, Q.T.m1 * 2, Q.T.act2 * 2, Q.T.act3 * 2, Q.T.hid * 2, Q.T.m4 * 2,
+                                                 Q.gx, Q.hseq, Q.hm, Q.save, Q.cm, Q.dgates, Q.T.dhid * 2};
+    for (int k = 0; k < B200RL_LSTM_ACTS_TENSORS; ++k) offsets[k] = v[k];
+    return B200RL_OK;
+}
+extern "C" size_t b200rl_lstm_agent_bf16_workspace_bytes(int64_t S, int64_t n, int A) {
+    if (!lstm_sizes_ok(S, n) || !lstm_heads_ok(A)) return 0;
+    const NatureLayout L(A, NatureLayout::Lstm{});
+    return lstm_big_bytes(S * n, L) + lstm_small_bytes(S * n, A) + 512;
+}
+
+extern "C" int b200rl_lstm_agent_bf16_pack(const float* params, int A, void* packed, void* stream) {
+    B200RL_REQUIRE(params && packed, "lstm_pack: null pointer");
+    B200RL_REQUIRE(lstm_heads_ok(A), "lstm_pack: A=%d outside [1,%d]", A, lstm::kMaxA1 - 1);
+    B200RL_REQUIRE(aligned(params, 16) && aligned(packed, 16), "lstm_pack: misaligned buffer");
+    const NatureLayout L(A, NatureLayout::Lstm{});
+    bf16* P = reinterpret_cast<bf16*>(packed);
+    cudaStream_t s = (cudaStream_t)stream;
+    ProfScope ps(s, "pack_weights", 0, (double)L.total * 4 + (double)L.packed_total * 2);
+    lstm::lstm_pack_conv1<<<8, 256, 0, s>>>(params + L.c1w, P + L.w1f);
+    tc_pack_conv2_cells<<<128, 256, 0, s>>>(params + L.c2w, P + L.w2f);
+    tc_pack_conv_s2_classes<<<(unsigned)ceil_div(32768, 256), 256, 0, s>>>(params + L.c2w, 64, 32, P + L.w2dg);
+    tc_pack_conv<<<(unsigned)ceil_div(36864, 256), 256, 0, s>>>(params + L.c3w, 64, 64, 3, 3, 0, P + L.w3f, P + L.w3dg);
+    tc_pack_fc<<<dim3(512 / 8, 49 / 7), 256, 0, s>>>(params + L.fcw, 512, 49, P + L.wfcf, P + L.wfcdg);
+    tc_pack_head_wide<<<(unsigned)ceil_div((int64_t)L.G * 512, 256), 256, 0, s>>>(params + L.wih, params + L.bih, 512, L.G,
+                                                                                P + L.whf, P + L.whdg, reinterpret_cast<float*>(P + L.hbp));
+    tc_head_dhead_bf16<<<256, 256, 0, s>>>(params + L.whh, 512, 128, 128, P + L.whhp);     // W_hh -> bf16 [512][128]
+    return check_launch("lstm_pack", 7);
+}
+
+extern "C" int b200rl_lstm_agent_bf16_forward(const uint8_t* obs, const int64_t* rows, int64_t S, int64_t n, int A,
+                                              const float* params, const void* packed, const float* h0, const float* c0,
+                                              const float* done, void* acts, float* head_out, float* h_out, float* c_out,
+                                              void* stream) {
+    B200RL_REQUIRE(obs && params && packed && h0 && c0 && done && acts && head_out && h_out && c_out, "lstm_forward: null pointer");
+    B200RL_REQUIRE(lstm_heads_ok(A), "lstm_forward: A=%d outside [1,%d]", A, lstm::kMaxA1 - 1);
+    B200RL_REQUIRE(lstm_sizes_ok(S, n), "lstm_forward: S=%lld n=%lld (S*n at most %lld)", (long long)S, (long long)n,
+                   (long long)kLstmMaxRows);
+    B200RL_REQUIRE(aligned(obs, 16) && aligned(rows, 8) && aligned(params, 16) && aligned(packed, 16) && aligned(acts, 256) &&
+                   aligned(h0, 16) && aligned(c0, 16) && aligned(done, 4) && aligned(head_out, 4) && aligned(h_out, 16) &&
+                   aligned(c_out, 16), "lstm_forward: misaligned buffer");
+    const int64_t M = S * n;
+    const NatureLayout L(A, NatureLayout::Lstm{});
+    const LstmActs Q(M);
+    const bf16* P = reinterpret_cast<const bf16*>(packed);
+    uint8_t* ab = reinterpret_cast<uint8_t*>(acts);
+    bf16* act = reinterpret_cast<bf16*>(acts);
+    cudaStream_t s = (cudaStream_t)stream;
+    int rc;
+    {   // conv1 on the uint8 frames -> act1 (2x2 cells) + ReLU bits
+        lstm::Conv1P cp;
+        cp.obs = obs; cp.rows = rows; cp.n = M; cp.w = P + L.w1f; cp.bias = params + L.c1b; cp.out = act + Q.T.act1;
+        cp.mask_out = reinterpret_cast<uint32_t*>(act + Q.T.m1);
+        ProfScope ps(s, "conv1_fwd", 2.0 * M * 400 * 32 * 64, (double)M * (7056 + 12800 * 2 + 1600));
+        const int64_t grid = M < (int64_t)num_sms() * 8 ? M : (int64_t)num_sms() * 8;
+        lstm::lstm_conv1_fwd<<<(unsigned)grid, lstm::kThreads, lstm::conv1_fwd_smem(), s>>>(cp);
+        if ((rc = check_launch("lstm/conv1"))) return rc;
+    }
+    if ((rc = trunk_fwd(L, Q.T, params, P, act, M, s))) return rc;
+    float* gx = reinterpret_cast<float*>(ab + Q.gx);
+    { ProfScope ps(s, "lstm_ih_fwd", 2.0 * M * 512 * 512, (double)M * (1024 + 2048) + 512.0 * 1024);
+      if ((rc = wide_head_fwd(L, P, act + Q.T.hid, M, 512, gx, s))) return rc; }
+    {
+        lstm::RecFwdP rp;
+        rp.S = (int)S; rp.n = n; rp.whh = P + L.whhp; rp.bhh = params + L.bhh; rp.gx = gx; rp.done = done; rp.h0 = h0; rp.c0 = c0;
+        rp.hseq = reinterpret_cast<bf16*>(ab + Q.hseq); rp.hm = reinterpret_cast<bf16*>(ab + Q.hm);
+        rp.save = reinterpret_cast<float*>(ab + Q.save); rp.cm = reinterpret_cast<float*>(ab + Q.cm);
+        rp.h_out = h_out; rp.c_out = c_out;
+        static SmemAttrCache attr;
+        if ((rc = attr.ensure(lstm::lstm_rec_fwd, lstm::rec_fwd_smem(), "lstm/recurrence"))) return rc;
+        ProfScope ps(s, "lstm_rec_fwd", 2.0 * M * 512 * 128, (double)M * (2048 + 4 + 512 + 3840) + 131072.0);
+        lstm::lstm_rec_fwd<<<(unsigned)ceil_div(n, lstm::kRows), lstm::kThreads, lstm::rec_fwd_smem(), s>>>(rp);
+        if ((rc = check_launch("lstm/recurrence"))) return rc;
+    }
+    { ProfScope ps(s, "heads_fwd", 2.0 * M * 128 * (A + 1), (double)M * (256 + 4 * (A + 1)));
+      const int hb = (int)(ceil_div(M, 8) < (int64_t)num_sms() * 8 ? ceil_div(M, 8) : (int64_t)num_sms() * 8);
+      tc_heads_fwd<128><<<hb, 256, (size_t)(A + 1) * 128 * 4, s>>>(reinterpret_cast<const bf16*>(ab + Q.hseq), params + L.hw,
+                                                                   params + L.hb, M, A + 1, 128, head_out);
+      if ((rc = check_launch("lstm/heads"))) return rc; }
+    return B200RL_OK;
+}
+
+extern "C" int b200rl_lstm_agent_bf16_backward(const uint8_t* obs, const int64_t* rows, int64_t S, int64_t n, int A,
+                                               const float* params, const void* packed, const float* done, void* acts,
+                                               const float* dhead, float* grads, void* workspace, size_t workspace_bytes,
+                                               void* stream) {
+    B200RL_REQUIRE(obs && params && packed && done && acts && dhead && grads && workspace, "lstm_backward: null pointer");
+    B200RL_REQUIRE(lstm_heads_ok(A), "lstm_backward: A=%d outside [1,%d]", A, lstm::kMaxA1 - 1);
+    B200RL_REQUIRE(lstm_sizes_ok(S, n), "lstm_backward: S=%lld n=%lld (S*n at most %lld)", (long long)S, (long long)n,
+                   (long long)kLstmMaxRows);
+    B200RL_REQUIRE(aligned(obs, 16) && aligned(rows, 8) && aligned(params, 16) && aligned(packed, 16) && aligned(acts, 256) &&
+                   aligned(done, 4) && aligned(dhead, 4) && aligned(grads, 16) && aligned(workspace, 256),
+                   "lstm_backward: misaligned buffer");
+    const size_t need = b200rl_lstm_agent_bf16_workspace_bytes(S, n, A);
+    if (workspace_bytes < need) return fail(B200RL_ERR_WORKSPACE, "lstm_backward: workspace %zu < %zu", workspace_bytes, need);
+    const int64_t M = S * n;
+    const int A1 = A + 1;
+    const NatureLayout L(A, NatureLayout::Lstm{});
+    const LstmActs Q(M);
+    const bf16* P = reinterpret_cast<const bf16*>(packed);
+    uint8_t* ab = reinterpret_cast<uint8_t*>(acts);
+    bf16* act = reinterpret_cast<bf16*>(acts);
+    cudaStream_t s = (cudaStream_t)stream;
+    float* wsbig = reinterpret_cast<float*>(workspace);
+    float* wssmall = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + lstm_big_bytes(M, L));
+    const bf16* hseq = reinterpret_cast<const bf16*>(ab + Q.hseq);
+    float* dgates = reinterpret_cast<float*>(ab + Q.dgates);
+    int rc;
+    {   // heads weight gradient (the data gradient is folded into the recurrence backward)
+        const int64_t rpb = heads_rows_per_block(M);
+        const int nb = (int)ceil_div(M, rpb);
+        ProfScope ps(s, "heads_bwd", 2.0 * M * 128 * A1, (double)M * (256 + 4 * A1));
+        const size_t sd = (size_t)rpb * A1 * sizeof(float);
+        if (A1 <= 8) tc_heads_bwd_weight<8, 128><<<nb, 128, sd, s>>>(dhead, hseq, M, A1, 128, rpb, wssmall);
+        else tc_heads_bwd_weight<kMaxHeads, 128><<<nb, 128, sd, s>>>(dhead, hseq, M, A1, 128, rpb, wssmall);
+        tc_heads_fold<<<(unsigned)ceil_div(A1 * 130, 32), 256, 0, s>>>(wssmall, 2 * nb, A1, 128, grads + L.hw, grads + L.hb);
+        if ((rc = check_launch("lstm/heads_bwd", 2))) return rc;
+    }
+    {
+        lstm::RecBwdP bp;
+        bp.S = (int)S; bp.n = n; bp.A1 = A1; bp.whh = P + L.whhp; bp.wh = params + L.hw; bp.dhead = dhead; bp.done = done;
+        bp.save = reinterpret_cast<const float*>(ab + Q.save); bp.cm = reinterpret_cast<const float*>(ab + Q.cm);
+        bp.dgates = dgates;
+        static SmemAttrCache attr;
+        if ((rc = attr.ensure(lstm::lstm_rec_bwd, lstm::rec_bwd_smem(), "lstm/recurrence_bwd"))) return rc;
+        ProfScope ps(s, "lstm_rec_bwd", 2.0 * M * 512 * 128 + 2.0 * M * 128 * A1, (double)M * (4 * A1 + 3072 + 2048));
+        lstm::lstm_rec_bwd<<<(unsigned)ceil_div(n, lstm::kRows), lstm::kThreads, lstm::rec_bwd_smem(), s>>>(bp);
+        if ((rc = check_launch("lstm/recurrence_bwd"))) return rc;
+    }
+    {   // W_ih, b_ih and d(feats) through the wide-head backward; it leaves dgates in bf16 at the start of wssmall
+        ProfScope ps(s, "lstm_ih_bwd", 4.0 * M * 512 * 512, (double)M * (2048 + 1024 * 3 + 64));
+        if ((rc = wide_head_bwd(L, P, dgates, M, 512, act + Q.T.hid, act + Q.T.dhid, reinterpret_cast<const uint32_t*>(act + Q.T.m4),
+                                grads + L.wih, grads + L.bih, wsbig, wssmall, s))) return rc;
+    }
+    {   // dW_hh = dgates^T . h' over all S*n rows (row splits folded in order); db_hh = db_ih
+        ProfScope ps(s, "lstm_hh_wgrad", 2.0 * M * 512 * 128, (double)M * (1024 + 256) + 512.0 * 128 * 4);
+        const WPlan pl = wgrad_plan(M, kFcSplits, 64);
+        CUtensorMap tmX, tmY;
+        if ((rc = make_tmap_2d(&tmX, wssmall, M, 512, 64, "lstm/hh_wgrad"))) return rc;
+        if ((rc = make_tmap_2d(&tmY, ab + Q.hm, M, 128, 64, "lstm/hh_wgrad"))) return rc;
+        const size_t smem = (size_t)4 * (kFcWgradXChunks + kFcWgradYChunks) * 64 * 128 + 1024;
+        static SmemAttrCache attr;
+        if ((rc = attr.ensure(tc_wgrad_tma, smem, "lstm/hh_wgrad"))) return rc;
+        // X = dgates (512 columns), Y = h' (128 columns: the rest of the 256-column Y group is zero-filled by TMA)
+        const dim3 grid(pl.splits, 512 / (64 * kFcWgradXChunks), 1);
+        tc_wgrad_tma<<<grid, kWgradTmaThreads, smem, s>>>(tmX, tmY, M, pl.rows_per_cta, wsbig);
+        tc_fold_fc<<<(unsigned)ceil_div((int64_t)512 * 128, 256), 256, 0, s>>>(wsbig, pl.splits, 512, 64 * kFcWgradYChunks, 512, 128,
+                                                                            128, 1, 1.f, grads + L.whh);
+        if ((rc = check_launch("lstm/hh_wgrad", 2))) return rc;
+        const cudaError_t e = cudaMemcpyAsync(grads + L.bhh, grads + L.bih, 512 * sizeof(float), cudaMemcpyDeviceToDevice, s);
+        if (e != cudaSuccess) return fail(B200RL_ERR_CUDA, "lstm_backward: bias copy: %s", cudaGetErrorString(e));
+    }
+    if ((rc = trunk_bwd(L, Q.T, P, act, grads, M, wsbig, wssmall, nullptr, false, s))) return rc;
+    {   // conv1 weight gradient from the frames and d(act1) on the 21x21 grid
+        const C1Plan pl = lstm_conv1_plan(M);
+        lstm::Conv1WgradP wp;
+        wp.obs = obs; wp.rows = rows; wp.n = M; wp.dy = act + Q.T.dact1; wp.imgs_per_cta = pl.per_cta; wp.ws = wsbig; wp.wsb = wssmall;
+        static SmemAttrCache attr;
+        if ((rc = attr.ensure(lstm::lstm_conv1_wgrad, lstm::conv1_wgrad_smem(), "lstm/conv1_wgrad"))) return rc;
+        ProfScope ps(s, "conv1_wgrad", 2.0 * M * 400 * 32 * 64, (double)M * (7056 + 14112 * 2));
+        lstm::lstm_conv1_wgrad<<<pl.ctas, lstm::kThreads, lstm::conv1_wgrad_smem(), s>>>(wp);
+        lstm::lstm_conv1_fold<<<(unsigned)ceil_div(32 * 64 + 32, 256), 256, 0, s>>>(wsbig, wssmall, pl.ctas, grads + L.c1w, grads + L.c1b);
+        if ((rc = check_launch("lstm/conv1_wgrad", 2))) return rc;
     }
     return B200RL_OK;
 }

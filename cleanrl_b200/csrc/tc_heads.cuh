@@ -18,14 +18,14 @@ static inline int64_t heads_rows_per_block(int64_t n) {
     return rpb;
 }
 
-// out[n][A1] = hidden[n][HT](bf16) . Wh[A1][HT]^T + bh (HT = 512: NatureCNN, 256: IMPALA-CNN; H == HT).  One warp per
-// row: lane l holds hidden units [256q + 8l, 256q + 8l + 8) (one 16-byte load per q), weights are read as float4 from
-// shared memory.
+// out[n][A1] = hidden[n][HT](bf16) . Wh[A1][HT]^T + bh (HT = 512: NatureCNN, 256: IMPALA-CNN, 128: the LSTM agent's
+// recurrent state; H == HT).  One warp per row: lane l holds hidden units [256q + 8l, 256q + 8l + 8) (one 16-byte load
+// per q; lanes past HT / 8 hold zeros), weights are read as float4 from shared memory.
 template <int HT = 512>
 __global__ void __launch_bounds__(256) tc_heads_fwd(const bf16* __restrict__ hid, const float* __restrict__ Wh,
                                                     const float* __restrict__ bh, int64_t n, int A1, int H,
                                                     float* __restrict__ out) {
-    constexpr int NQ = HT / 256;
+    constexpr int NQ = (HT + 255) / 256;
     extern __shared__ float sW[];                       // [A1][HT]
     for (int i = threadIdx.x; i < A1 * HT; i += blockDim.x) sW[i] = Wh[i];
     __syncthreads();
@@ -35,7 +35,8 @@ __global__ void __launch_bounds__(256) tc_heads_fwd(const bf16* __restrict__ hid
         const bf16* hp = hid + row * HT;
 #pragma unroll
         for (int q = 0; q < NQ; ++q) {
-            const int4 v = ldg16(hp + q * 256 + lane * 8);
+            const bool own = HT % 256 == 0 || lane * 8 < HT;
+            const int4 v = own ? ldg16(hp + q * 256 + lane * 8) : make_int4(0, 0, 0, 0);
             const uint32_t w[4] = {(uint32_t)v.x, (uint32_t)v.y, (uint32_t)v.z, (uint32_t)v.w};
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
@@ -48,6 +49,7 @@ __global__ void __launch_bounds__(256) tc_heads_fwd(const bf16* __restrict__ hid
             float s = 0.f;
 #pragma unroll
             for (int q = 0; q < NQ; ++q) {
+                if (HT % 256 != 0 && lane * 8 >= HT) continue;
                 const float4 w0 = *reinterpret_cast<const float4*>(sW + a * HT + q * 256 + lane * 8);
                 const float4 w1 = *reinterpret_cast<const float4*>(sW + a * HT + q * 256 + lane * 8 + 4);
                 s = fmaf(hv[q * 8 + 0], w0.x, s); s = fmaf(hv[q * 8 + 1], w0.y, s);

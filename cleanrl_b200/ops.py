@@ -650,6 +650,127 @@ class ImpalaCNNBf16:
         _lib.check(rc, "impala_bf16_backward")
 
 
+# ------------------------------------------------------ recurrent agent bf16 (tensor-core) plan
+class LSTMAgentBf16:
+    """Owns the packed bf16 weights, the activation workspaces and the backward workspace of the tensor-core recurrent
+    agent (single uint8 frames [*, 1, 84, 84], NatureCNN trunk, LSTM(512, 128), heads).  Sequences are S steps x n envs,
+    time-major."""
+
+    MAX_UNPINNED = 4
+    H = 128
+
+    def __init__(self, A, device):
+        lib = _lib.load()
+        self.A, self.device = int(A), device
+        nbytes = lib.b200rl_lstm_agent_bf16_packed_bytes(self.A)
+        if nbytes == 0:
+            raise ValueError(f"tensor-core LSTM agent supports 1 <= A <= 23 actions (got {A})")
+        self.param_count = lib.b200rl_lstm_agent_param_count(self.A)
+        self.packed = torch.empty(nbytes, dtype=torch.uint8, device=device)
+        self._acts = {}          # (S, n) -> workspace, least-recently-used first
+        self._pinned = set()     # shapes referenced by captured CUDA graphs: never evicted
+        self._ws = None
+        self._pinned_ws = []
+
+    def pin(self):
+        """Every workspace that exists now may be referenced by a captured CUDA graph: keep it alive."""
+        self._pinned.update(self._acts.keys())
+        if self._ws is not None and all(w is not self._ws for w in self._pinned_ws):
+            self._pinned_ws.append(self._ws)
+
+    def acts(self, S, n):
+        key = (int(S), int(n))
+        buf = self._acts.pop(key, None)
+        if buf is None:
+            unpinned = [k for k in self._acts if k not in self._pinned]
+            while len(unpinned) >= self.MAX_UNPINNED:
+                del self._acts[unpinned.pop(0)]
+            nbytes = _lib.load().b200rl_lstm_agent_bf16_acts_bytes(*key)
+            if nbytes == 0:
+                raise ValueError(f"tensor-core LSTM agent: {S} steps x {n} envs is out of range")
+            # zero-initialised: the padded-grid gradient buffers rely on never-written positions being 0
+            buf = torch.zeros(nbytes, dtype=torch.uint8, device=self.device)
+        self._acts[key] = buf
+        return buf
+
+    def act_tensors(self, S, n):
+        """Named views of the activation workspace of (S, n) (layout: b200rl_lstm_agent_bf16_acts_layout)."""
+        import ctypes
+        off = (ctypes.c_int64 * 13)()
+        _lib.check(_lib.load().b200rl_lstm_agent_bf16_acts_layout(S, n, off), "lstm_acts_layout")
+        buf = self.acts(S, n)
+        M = S * n
+        bf, f32, i32 = torch.bfloat16, torch.float32, torch.int32
+        out = {}
+        for k, (name, dtype, shape) in enumerate((
+                ("act1", bf, (M, 10, 10, 128)), ("m1", i32, (M, 400)), ("act2", bf, (M, 9, 9, 64)), ("act3", bf, (M, 7, 7, 64)),
+                ("feats", bf, (M, 512)), ("m4", i32, (M, 16)),
+                ("gx", f32, (M, 512)), ("hseq", bf, (M, 128)), ("hm", bf, (M, 128)), ("save", f32, (M, 5, 128)),
+                ("cm", f32, (M, 128)), ("dgates", f32, (M, 512)), ("dfeats", bf, (M, 512)))):
+            cnt = 1
+            for d in shape:
+                cnt *= d
+            nb = cnt * torch.tensor([], dtype=dtype).element_size()
+            out[name] = buf[off[k]:off[k] + nb].view(dtype).view(*shape)
+        return out
+
+    @staticmethod
+    def check_obs(obs):
+        if obs.dtype != torch.uint8 or obs.dim() != 4 or tuple(obs.shape[-3:]) != (1, 84, 84):
+            raise ValueError("tensor-core LSTM agent consumes uint8 frames [*, 1, 84, 84] "
+                             f"(got {obs.dtype} {tuple(obs.shape)})")
+
+    def pack(self, flat_params):
+        rc = _lib.load().b200rl_lstm_agent_bf16_pack(_ptr(flat_params, torch.float32, "params"), self.A,
+                                                     self.packed.data_ptr(), _stream())
+        _lib.check(rc, "lstm_agent_bf16_pack")
+
+    def forward(self, obs, rows, S, n, flat_params, h0, c0, done, head_out=None, h_out=None, c_out=None):
+        """(head_out [S*n, A+1], h_S [n, 128], c_S [n, 128]); the sequence's activations stay in the workspace."""
+        self.check_obs(obs)
+        _contig(obs, "obs")
+        f = torch.float32
+        M = S * n
+        if rows is not None:
+            _contig(rows, "rows")
+            if rows.numel() != M:
+                raise ValueError(f"rows has {rows.numel()} entries for {S} steps x {n} envs")
+        elif obs.shape[0] != M:
+            raise ValueError(f"obs has {obs.shape[0]} frames for {S} steps x {n} envs")
+        for nm, t, shape in (("h0", h0, (n, self.H)), ("c0", c0, (n, self.H)), ("done", done, (M,))):
+            _contig(t, nm)
+            if tuple(t.shape) != shape:
+                raise ValueError(f"{nm}: expected shape {shape}, got {tuple(t.shape)}")
+        if head_out is None:
+            head_out = torch.empty(M, self.A + 1, dtype=f, device=self.device)
+        if h_out is None:
+            h_out = torch.empty(n, self.H, dtype=f, device=self.device)
+        if c_out is None:
+            c_out = torch.empty(n, self.H, dtype=f, device=self.device)
+        rc = _lib.load().b200rl_lstm_agent_bf16_forward(
+            _ptr(obs, torch.uint8, "obs"), _ptr(rows, torch.int64, "rows", True), S, n, self.A,
+            _ptr(flat_params, f, "params"), self.packed.data_ptr(), _ptr(h0, f, "h0"), _ptr(c0, f, "c0"),
+            _ptr(done, f, "done"), self.acts(S, n).data_ptr(), _ptr(head_out, f, "head_out"), _ptr(h_out, f, "h_out"),
+            _ptr(c_out, f, "c_out"), _stream())
+        _lib.check(rc, "lstm_agent_bf16_forward")
+        return head_out, h_out, c_out
+
+    def backward(self, obs, rows, S, n, flat_params, done, dhead, flat_grads):
+        """Gradient of the forward that last ran on (obs, rows, S, n, done); fills ``flat_grads``."""
+        lib = _lib.load()
+        self.check_obs(obs)
+        _contig(dhead, "dhead")
+        nbytes = lib.b200rl_lstm_agent_bf16_workspace_bytes(S, n, self.A)
+        if self._ws is None or self._ws.numel() < nbytes:
+            self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        f = torch.float32
+        rc = lib.b200rl_lstm_agent_bf16_backward(
+            _ptr(obs, torch.uint8, "obs"), _ptr(rows, torch.int64, "rows", True), S, n, self.A,
+            _ptr(flat_params, f, "params"), self.packed.data_ptr(), _ptr(done, f, "done"), self.acts(S, n).data_ptr(),
+            _ptr(dhead, f, "dhead"), _ptr(flat_grads, f, "grads"), self._ws.data_ptr(), self._ws.numel(), _stream())
+        _lib.check(rc, "lstm_agent_bf16_backward")
+
+
 def frames_to_s2d(obs_u8, out=None, rows=None):
     """uint8 [n,4,84,84] frames -> bf16 [n,21,21,64] space-to-depth frames (once per env step)."""
     lib = _lib.load()

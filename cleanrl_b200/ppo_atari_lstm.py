@@ -99,6 +99,7 @@ def main(argv=None, writer_factory=None, env_factory=None, on_iteration=None, ag
     envs = env_factory(args) if env_factory else make_envs(args, run_name)
     assert hasattr(envs.single_action_space, "n"), "only discrete action space is supported"
     agent = Agent(envs).to(device)
+    agent.precision = args.precision
     if agent_hook:
         agent_hook(agent)
     flat = agent.flat
@@ -186,6 +187,7 @@ def main(argv=None, writer_factory=None, env_factory=None, on_iteration=None, ag
                     flat.step += 1
                     ops.clip_adam(flat.flat, flat.grad, flat.exp_avg, flat.exp_avg_sq, flat.step, lrnow, eps=1e-5,
                                   max_norm=args.max_grad_norm)
+                    agent.params_updated()
                     k += 1
                 if args.target_kl is not None and stats[k - 1, 4].item() > args.target_kl:
                     stop = True

@@ -389,6 +389,45 @@ int b200rl_impala_bf16_backward(const uint8_t* obs, const int64_t* rows, int64_t
                                 const void* packed, void* acts, const float* dhead, float* grads,
                                 void* workspace, size_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------- recurrent agent, bf16 tensor cores ---
+ * cleanrl/ppo_atari_lstm.py:117-160: NatureCNN trunk over ONE grayscale frame, nn.LSTM(512, 128) with the state reset by
+ * (1 - done) before every step (gate order i, f, g, o), actor / critic on the LSTM output.  bf16 operands, fp32
+ * accumulation; the cell state and the gate math stay fp32.
+ * params / grads: ONE flat fp32 vector in LSTMAgent._param_order (b200rl_lstm_agent_param_count(A) elements), 16-B aligned:
+ *     conv1.w[32,1,8,8] conv1.b[32] conv2.w[64,32,4,4] conv2.b[64] conv3.w[64,64,3,3] conv3.b[64] fc.w[512,3136] fc.b[512]
+ *     weight_ih[512,512] weight_hh[512,128] bias_ih[512] bias_hh[512] actor.w[A,128] critic.w[1,128] actor.b[A] critic.b[1]
+ * packed : bf16 operand copies (b200rl_lstm_agent_bf16_packed_bytes), refreshed by b200rl_lstm_agent_bf16_pack after every
+ *          optimiser step.
+ * A sequence is S steps of n envs, time-major: batch row t*n + e is step t of env e (S*n rows, at most 131072).
+ * obs    : uint8 frames [*, 1, 84, 84]; row i of the batch is frame rows[i] (rows i64 [S*n], may be NULL: frame i).
+ * done   : f32 [S*n]: the state of row (t, e) is multiplied by (1 - done) before step t.
+ * h0, c0 : f32 [n, 128] state before step 0; h_out, c_out f32 [n, 128] the state after step S-1 (the rollout calls the
+ *          forward with S = 1 once per env step, carrying (h, c)).
+ * acts   : activation workspace for (S, n) (b200rl_lstm_agent_bf16_acts_bytes), 256-B aligned, ZEROED once before its first
+ *          use; the backward reads what the forward of the same (obs, rows, S, n, done) left there.
+ * head_out [S*n, A+1] fp32 = [logits | value]; dhead [S*n, A+1] its gradient; grads = flat fp32 gradient (overwritten).
+ * 1 <= A <= 23.  Bad pointers, alignment (rows: 8 B), A, S, n or S*n: B200RL_ERR_INVALID_ARGUMENT before any CUDA call.  No
+ * host synchronisation or allocation: forward and backward may be captured in a CUDA graph. */
+int64_t b200rl_lstm_agent_param_count(int A);
+size_t b200rl_lstm_agent_bf16_packed_bytes(int A);
+size_t b200rl_lstm_agent_bf16_acts_bytes(int64_t S, int64_t n);
+/* Byte offsets of the tensors inside `acts` (M = S*n rows), written to offsets[B200RL_LSTM_ACTS_TENSORS] in this order:
+ *   act1 bf16 [M,10,10,128] (conv1 output as 2x2 cells), m1 uint32 [M,400] (act1 > 0 bits), act2 bf16 [M,9,9,64], act3 bf16
+ *   [M,7,7,64] (conv2 / conv3 outputs, channel-last), feats bf16 [M,512] (fc output,
+ *   post-ReLU), m4 uint32 [M,16], gx f32 [M,512] (feats W_ih^T + b_ih), hseq bf16 [M,128] (h_t), hm bf16 [M,128] (the
+ *   masked state h' entering step t), save f32 [M,5,128] (i, f, g, o, tanh c), cm f32 [M,128] (the masked cell state c'),
+ *   dgates f32 [M,512] (backward), dfeats bf16 [M,512] (backward). */
+#define B200RL_LSTM_ACTS_TENSORS 13
+int b200rl_lstm_agent_bf16_acts_layout(int64_t S, int64_t n, int64_t* offsets);
+size_t b200rl_lstm_agent_bf16_workspace_bytes(int64_t S, int64_t n, int A);
+int b200rl_lstm_agent_bf16_pack(const float* params, int A, void* packed, void* stream);
+int b200rl_lstm_agent_bf16_forward(const uint8_t* obs, const int64_t* rows, int64_t S, int64_t n, int A,
+                                   const float* params, const void* packed, const float* h0, const float* c0,
+                                   const float* done, void* acts, float* head_out, float* h_out, float* c_out, void* stream);
+int b200rl_lstm_agent_bf16_backward(const uint8_t* obs, const int64_t* rows, int64_t S, int64_t n, int A,
+                                    const float* params, const void* packed, const float* done, void* acts,
+                                    const float* dhead, float* grads, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ------------------------------------------------------------ LSTM cell ---
  * Recurrent PPO agent (cleanrl/ppo_atari_lstm.py:117-160: nn.LSTM(512, 128), gate order i, f, g, o; the state is reset
  * by (1 - done) BEFORE the cell, :137-142).  The gate GEMMs are b200rl_linear_fwd_f32 calls (x W_ih^T + b_ih for all
