@@ -80,10 +80,22 @@ class KernelAgent(nn.Module):
     # -- engine hooks (one policy step / one minibatch loss+backward) ---------------
     action_dim = 0          # 0 = discrete (int64 actions [n]); D > 0 = continuous (f32 actions [n, D])
 
-    @property
-    def graph_capturable(self):
-        """May the engine capture the per-step device work (frame conversion, network, sampler) in CUDA graphs?"""
-        return getattr(self, "precision", "bf16") == "bf16" or not hasattr(self, "network")
+    # may the engine capture the per-step device work (frame conversion, network, sampler) in CUDA graphs?
+    graph_capturable = True
+
+    def uses_tc_plan(self):
+        """Do forward and backward run on a tensor-core plan (``TensorCoreAgent`` with ``precision = "bf16"``)?"""
+        return False
+
+    def params_updated(self):
+        """Call after the optimiser changed the flat parameters."""
+
+    def pin_workspaces(self):
+        """Call after capturing a CUDA graph that runs this agent."""
+
+    def grad_tail(self):
+        """(offset, event) when ``flat.grad[offset:]`` is final before ``backward`` returns (NatureCNNAgent), else None."""
+        return None
 
     @property
     def graph_friendly(self):
@@ -119,6 +131,12 @@ class KernelAgent(nn.Module):
                      dlogits=scratch["dl"], dvalue=scratch["dv"], stats=stats_row)
         self.backward(scratch["dhead"])
 
+    def alloc_head_grad(self, M, device):
+        """(dhead [M, A+1], its dlogits view, its dvalue view): the gradient of the joint actor / critic head."""
+        A = self.num_actions
+        d = torch.empty(M, A + 1, dtype=torch.float32, device=device)
+        return d, d[:, :A], d[:, A]
+
     # -- reference API ---------------------------------------------------------
     def get_value(self, x):
         self.flat
@@ -138,8 +156,69 @@ class KernelAgent(nn.Module):
         return action, logprob, entropy, v.reshape(-1, 1)
 
 
-class NatureCNNAgent(KernelAgent):
+class TensorCoreAgent(KernelAgent):
+    """An agent whose network ``precision = "bf16"`` runs on the tensor cores through an ``ops`` plan (``plan_class``,
+    built on first use for ``_head_outputs()`` outputs); its packed bf16 weight copies are refreshed lazily after every
+    change of the flat parameters."""
+
+    precision = "fp32"
+    plan_class = None
+    _tc = None               # the plan
+    _tc_dirty = True         # the plan's packed weights are stale
+
+    def _head_outputs(self):
+        return self.num_actions + 1          # actor + critic
+
+    def bind(self):
+        self._tc, self._tc_dirty = None, True
+        return super().bind()
+
+    def uses_tc_plan(self):
+        return self.precision == "bf16"
+
+    @property
+    def graph_capturable(self):
+        """Only the bf16 plan is free of host work and allocations inside forward / backward."""
+        return self.uses_tc_plan()
+
+    def params_updated(self):
+        """Call after the optimiser changed the flat parameters: the packed bf16 operands are stale."""
+        self._tc_dirty = True
+
+    def _tc_plan(self):
+        f = self._flat
+        if self._tc is None:
+            self._tc = self.plan_class(self._head_outputs() - 1, f.flat.device)
+            assert f.flat.numel() >= self._tc.param_count
+        if self._tc_dirty:
+            self._tc.pack(f.flat)
+            self._tc_dirty = False
+        return self._tc
+
+    def load_state_dict(self, *a, **k):
+        out = super().load_state_dict(*a, **k)
+        self._tc_dirty = True
+        return out
+
+    def pin_workspaces(self):
+        """A CUDA graph captured by the engine holds raw pointers into the plan's workspaces: keep them all alive."""
+        if self._tc is not None:
+            self._tc.pin()
+
+    def _joint_head(self):
+        """``actor`` and ``critic`` as ONE layer over the flat buffer (adjacent in ``_param_order``): weight [A+1, hidden],
+        bias [A+1]."""
+        f, A1, H = self._flat, self.num_actions + 1, self.actor.in_features
+        ow = (f.view_of(self.actor.weight)[0].data_ptr() - f.flat.data_ptr()) // 4
+        ob = (f.view_of(self.actor.bias)[0].data_ptr() - f.flat.data_ptr()) // 4
+        return nets.Linear(None, None, f.flat[ow:ow + A1 * H].view(A1, H), f.flat[ob:ob + A1],
+                           f.grad[ow:ow + A1 * H].view(A1, H), f.grad[ob:ob + A1])
+
+
+class NatureCNNAgent(TensorCoreAgent):
     """NatureCNN actor-critic (reference: cleanrl/ppo_atari_envpool.py:123-149)."""
+
+    plan_class = ops.NatureCNNBf16
 
     def __init__(self, envs):
         super().__init__()
@@ -160,50 +239,11 @@ class NatureCNNAgent(KernelAgent):
         return net + [self.actor.weight, self.critic.weight, self.actor.bias, self.critic.bias]
 
     def _build_plan(self):
-        f = self._flat
-        A = self.num_actions
-        wa, ga = f.view_of(self.actor.weight)
-        ba, gba = f.view_of(self.actor.bias)
-        off_w = (wa.data_ptr() - f.flat.data_ptr()) // 4
-        off_b = (ba.data_ptr() - f.flat.data_ptr()) // 4
-        self._head_w = f.flat[off_w:off_w + (A + 1) * 512].view(A + 1, 512)
-        self._head_b = f.flat[off_b:off_b + A + 1]
-        self._head_dw = f.grad[off_w:off_w + (A + 1) * 512].view(A + 1, 512)
-        self._head_db = f.grad[off_b:off_b + A + 1]
         n = self.network
         self.trunk = nets.Chain([
             nets.Conv(n[0], "relu", in_div=255.0), nets.Conv(n[2], "relu"), nets.Conv(n[4], "relu"),
             nets.Linear(n[7], "relu")])
-        self.head = nets.Linear(None, None, self._head_w, self._head_b, self._head_dw, self._head_db)
-        self._tc = None
-        self._tc_dirty = True
-
-    # -- bf16 tensor-core plan ("--precision bf16") ------------------------------
-    precision = "fp32"
-
-    def params_updated(self):
-        """Call after the optimiser changed the flat parameters: the packed bf16 operands are stale."""
-        self._tc_dirty = True
-
-    def _tc_plan(self):
-        f = self._flat
-        if self._tc is None:
-            assert f.flat.numel() >= ops._lib.load().b200rl_naturecnn_param_count(self.num_actions)
-            self._tc = ops.NatureCNNBf16(self.num_actions, f.flat.device)
-        if self._tc_dirty:
-            self._tc.pack(f.flat)
-            self._tc_dirty = False
-        return self._tc
-
-    def load_state_dict(self, *a, **k):
-        out = super().load_state_dict(*a, **k)
-        self._tc_dirty = True
-        return out
-
-    def pin_workspaces(self):
-        """A CUDA graph captured by the engine holds raw pointers into the activation workspaces: never evict them."""
-        if self._tc is not None:
-            self._tc.pin()
+        self.head = self._joint_head()
 
     def _forward_heads(self, x, rows=None, keep=False, aux=None):
         if self.precision == "bf16":
@@ -229,11 +269,6 @@ class NatureCNNAgent(KernelAgent):
         ``aux``: channel-major copy of a uint8 space-to-depth rollout (consumed by the conv1 weight gradient)."""
         self.flat
         return self._forward_heads(b_obs, rows=mb_inds, keep=True, aux=aux)
-
-    def alloc_head_grad(self, M, device):
-        A = self.num_actions
-        d = torch.empty(M, A + 1, dtype=torch.float32, device=device)
-        return d, d[:, :A], d[:, A]
 
     def grad_tail(self):
         """(offset, event): ``flat.grad[offset:]`` (fc + heads, 95 % of the vector) is final when ``event`` fires in the
@@ -299,7 +334,7 @@ class MLPAgent(KernelAgent):
         self.c_chain.bwd(dv)
 
 
-class LSTMAgent(KernelAgent):
+class LSTMAgent(TensorCoreAgent):
     """Recurrent actor-critic (reference: cleanrl/ppo_atari_lstm.py:117-160): NatureCNN trunk over ONE grayscale frame,
     ``nn.LSTM(512, 128)`` with the state reset by ``(1 - done)`` before every step, ``actor`` / ``critic`` on the LSTM
     output.  Same module names / ``state_dict`` keys (``network.*``, ``lstm.weight_ih_l0`` ..., ``actor.*``, ``critic.*``),
@@ -312,7 +347,8 @@ class LSTMAgent(KernelAgent):
     ``precision = "bf16"`` runs the whole network on the tensor cores instead (ops.LSTMAgentBf16; uint8 frames
     [*, 1, 84, 84] only): one launch per sequence for the recurrence in each direction."""
 
-    precision = "fp32"
+    plan_class = ops.LSTMAgentBf16
+    graph_capturable = False
 
     def __init__(self, envs):
         super().__init__()
@@ -339,47 +375,13 @@ class LSTMAgent(KernelAgent):
         return net + list(self.lstm.parameters()) + [self.actor.weight, self.critic.weight, self.actor.bias, self.critic.bias]
 
     def _build_plan(self):
-        f = self._flat
-        A, H = self.num_actions, self.hidden_size
-        wa, _ = f.view_of(self.actor.weight)
-        ba, _ = f.view_of(self.actor.bias)
-        off_w = (wa.data_ptr() - f.flat.data_ptr()) // 4
-        off_b = (ba.data_ptr() - f.flat.data_ptr()) // 4
-        head_w = f.flat[off_w:off_w + (A + 1) * H].view(A + 1, H)
-        head_b = f.flat[off_b:off_b + A + 1]
-        head_dw = f.grad[off_w:off_w + (A + 1) * H].view(A + 1, H)
-        head_db = f.grad[off_b:off_b + A + 1]
         n = self.network
         self.trunk = nets.Chain([nets.Conv(n[0], "relu", in_div=255.0), nets.Conv(n[2], "relu"), nets.Conv(n[4], "relu"),
                                  nets.Linear(n[7], "relu")])
-        self.head = nets.Linear(None, None, head_w, head_b, head_dw, head_db)
+        self.head = self._joint_head()
         L = self.lstm
         self.l_ih = nets.Linear(None, None, L.weight_ih_l0.data, L.bias_ih_l0.data, L.weight_ih_l0.grad, L.bias_ih_l0.grad)
         self.l_hh = nets.Linear(None, None, L.weight_hh_l0.data, L.bias_hh_l0.data, L.weight_hh_l0.grad, L.bias_hh_l0.grad)
-        self._tc = None
-        self._tc_dirty = True
-
-    graph_capturable = False
-
-    # -- bf16 tensor-core plan ("--precision bf16") ------------------------------
-    def params_updated(self):
-        """Call after the optimiser changed the flat parameters: the packed bf16 operands are stale."""
-        self._tc_dirty = True
-
-    def _tc_plan(self):
-        f = self._flat
-        if self._tc is None:
-            self._tc = ops.LSTMAgentBf16(self.num_actions, f.flat.device)
-            assert f.flat.numel() >= self._tc.param_count
-        if self._tc_dirty:
-            self._tc.pack(f.flat)
-            self._tc_dirty = False
-        return self._tc
-
-    def load_state_dict(self, *a, **k):
-        out = super().load_state_dict(*a, **k)
-        self._tc_dirty = True
-        return out
 
     def _tc_states(self, x, lstm_state, done, rows, keep):
         ops.LSTMAgentBf16.check_obs(x)
@@ -464,11 +466,6 @@ class LSTMAgent(KernelAgent):
         hidden, _ = self.get_states(b_obs, lstm_state, done, rows=mb_inds, keep=True)
         return self._heads(hidden)
 
-    def alloc_head_grad(self, M, device):
-        A = self.num_actions
-        d = torch.empty(M, A + 1, dtype=torch.float32, device=device)
-        return d, d[:, :A], d[:, A]
-
     # ----------------------------------------------------------------- backward
     def backward(self, dhead):
         if self.precision == "bf16":
@@ -525,7 +522,7 @@ class ConvSequence(nn.Module):
         return (self._out_channels, (h + 1) // 2, (w + 1) // 2)
 
 
-class ImpalaAgent(KernelAgent):
+class ImpalaAgent(TensorCoreAgent):
     """IMPALA-CNN actor-critic (reference: cleanrl/ppo_procgen.py:89-150): three ConvSequences (16, 32, 32 channels),
     Flatten, ReLU, Linear(2048 -> 256), ReLU, ``actor`` / ``critic``.  Same module tree (``network.{0,1,2}.conv``,
     ``network.{0,1,2}.res_block{0,1}.conv{0,1}``, ``network.5``), same construction order, torch's default initialisation
@@ -535,6 +532,8 @@ class ImpalaAgent(KernelAgent):
     Execution: fp32 kernels of libb200rl (padded 3x3 convolutions, max-pool with arg-max, ReLU / add glue), explicit
     backward in reverse order; no autograd, no cuDNN.  ``precision = "bf16"`` runs the whole network on the tensor
     cores instead (ops.ImpalaCNNBf16, csrc/net_impala_tc.cu; uint8 frames [*, 64, 64, 3] only)."""
+
+    plan_class = ops.ImpalaCNNBf16
 
     def __init__(self, envs):
         super().__init__()
@@ -553,51 +552,12 @@ class ImpalaAgent(KernelAgent):
         self.num_actions = int(envs.single_action_space.n)
         self._feat_shape = shape
 
-    # -- bf16 tensor-core plan ("--precision bf16") ------------------------------
-    precision = "fp32"
-
-    @property
-    def graph_capturable(self):
-        """Only the bf16 plan is free of host work and allocations inside forward / backward."""
-        return self.precision == "bf16"
-
-    def params_updated(self):
-        """Call after the optimiser changed the flat parameters: the packed bf16 operands are stale."""
-        self._tc_dirty = True
-
-    def _tc_plan(self):
-        f = self._flat
-        if self._tc is None:
-            self._tc = ops.ImpalaCNNBf16(self.num_actions, f.flat.device)
-            assert f.flat.numel() >= self._tc.param_count
-        if self._tc_dirty:
-            self._tc.pack(f.flat)
-            self._tc_dirty = False
-        return self._tc
-
-    def load_state_dict(self, *a, **k):
-        out = super().load_state_dict(*a, **k)
-        self._tc_dirty = True
-        return out
-
-    def pin_workspaces(self):
-        """A CUDA graph captured by the engine holds raw pointers into the workspaces: never evict them."""
-        if self._tc is not None:
-            self._tc.pin()
-
     def _param_order(self):
         net = [p for p in self.network.parameters()]
         return net + [self.actor.weight, self.critic.weight, self.actor.bias, self.critic.bias]
 
     def _build_plan(self):
-        f = self._flat
-        A = self.num_actions
-        wa, _ = f.view_of(self.actor.weight)
-        ba, _ = f.view_of(self.actor.bias)
-        off_w = (wa.data_ptr() - f.flat.data_ptr()) // 4
-        off_b = (ba.data_ptr() - f.flat.data_ptr()) // 4
-        self.head = nets.Linear(None, None, f.flat[off_w:off_w + (A + 1) * 256].view(A + 1, 256), f.flat[off_b:off_b + A + 1],
-                                f.grad[off_w:off_w + (A + 1) * 256].view(A + 1, 256), f.grad[off_b:off_b + A + 1])
+        self.head = self._joint_head()
         self.fc = nets.Linear(self.network[5], "relu")
         self.seqs = []
         for i in range(3):
@@ -605,8 +565,6 @@ class ImpalaAgent(KernelAgent):
             self.seqs.append(dict(conv=nets.Conv(q.conv, None, in_div=255.0 if i == 0 else 1.0),
                                   blocks=[(nets.Conv(b.conv0, "relu"), nets.Conv(b.conv1, None))
                                           for b in (q.res_block0, q.res_block1)]))
-        self._tc = None
-        self._tc_dirty = True
 
     # ------------------------------------------------------------------ forward
     def _forward_heads(self, x, rows=None, keep=False):
@@ -648,11 +606,6 @@ class ImpalaAgent(KernelAgent):
     def forward_train(self, b_obs, mb_inds):
         self.flat
         return self._forward_heads(b_obs, rows=mb_inds, keep=True)
-
-    def alloc_head_grad(self, M, device):
-        A = self.num_actions
-        d = torch.empty(M, A + 1, dtype=torch.float32, device=device)
-        return d, d[:, :A], d[:, A]
 
     # ----------------------------------------------------------------- backward
     def backward(self, dhead):
@@ -759,9 +712,12 @@ class ContinuousMLPAgent(KernelAgent):
         return action, logprob, entropy, v.reshape(-1, 1)
 
 
-class QNetworkAgent(nn.Module):
+class QNetworkAgent(TensorCoreAgent):
     """DQN Q-network (reference: cleanrl/dqn_atari.py:108-125): NatureCNN trunk + Linear(512, A), default torch
-    initialisation, ``forward(x)`` -> Q-values [n, A]; state_dict keys ``network.{0,2,4,7,9}.*``."""
+    initialisation, ``forward(x)`` -> Q-values [n, A]; state_dict keys ``network.{0,2,4,7,9}.*``.  Its natural parameter
+    order is libb200rl's NatureCNN order; the bf16 plan's W-wide head is the NatureCNN's (W-1) + 1 heads."""
+
+    plan_class = ops.NatureCNNBf16
 
     def __init__(self, env):
         super().__init__()
@@ -770,47 +726,14 @@ class QNetworkAgent(nn.Module):
             nn.Conv2d(4, 32, 8, stride=4), nn.ReLU(), nn.Conv2d(32, 64, 4, stride=2), nn.ReLU(),
             nn.Conv2d(64, 64, 3, stride=1), nn.ReLU(), nn.Flatten(), nn.Linear(3136, 512), nn.ReLU(), nn.Linear(512, A))
         self.num_actions = A
-        self.precision = "fp32"
-        self._flat = None
-        self._tc = None
-        self._tc_dirty = True
 
-    def bind(self):
-        dev = next(self.parameters()).device
-        if dev.type != "cuda":
-            raise RuntimeError("cleanrl_b200 agents execute on CUDA only (libb200rl kernels); "
-                               f"parameters are on {dev}. There is no CPU fallback.")
-        self._flat = nets.FlatParams(list(self.parameters()), dev)   # natural order == libb200rl NatureCNN order
+    def _build_plan(self):
         n = self.network
         self.chain = nets.Chain([nets.Conv(n[0], "relu", in_div=255.0), nets.Conv(n[2], "relu"), nets.Conv(n[4], "relu"),
                                  nets.Linear(n[7], "relu"), nets.Linear(n[9], None)])
-        return self._flat
-
-    @property
-    def flat(self):
-        if self._flat is None or self._flat.flat.device != next(self.parameters()).device:
-            self.bind()
-        return self._flat
-
-    def params_updated(self):
-        self._tc_dirty = True
-
-    def load_state_dict(self, *a, **k):
-        out = super().load_state_dict(*a, **k)
-        self._tc_dirty = True
-        return out
 
     def _head_outputs(self):
         return self.num_actions
-
-    def _plan(self):
-        f = self.flat
-        if self._tc is None:
-            self._tc = ops.NatureCNNBf16(self._head_outputs() - 1, f.flat.device)   # heads = (W-1) + 1 = W outputs
-        if self._tc_dirty:
-            self._tc.pack(f.flat)
-            self._tc_dirty = False
-        return self._tc
 
     def q_values(self, frames, rows=None, keep=False):
         """Q(s, .) for frames[rows] (uint8 [*,4,84,84]; rows gathers without materialising)."""
@@ -818,7 +741,7 @@ class QNetworkAgent(nn.Module):
         if frames.dtype != torch.uint8:
             frames = frames.to(torch.uint8)
         if self.precision == "bf16":
-            out = self._plan().forward(frames.contiguous(), rows, self._flat.flat)
+            out = self._tc_plan().forward(frames.contiguous(), rows, self._flat.flat)
             if keep:
                 self._saved = (frames, rows)
             return out
@@ -860,7 +783,7 @@ class C51QNetwork(QNetworkAgent):
     head (wgmma); fp32 is the exact CUDA-core chain."""
 
     def __init__(self, env, n_atoms=101, v_min=-100, v_max=100):
-        nn.Module.__init__(self)
+        TensorCoreAgent.__init__(self)
         self.n_atoms = n_atoms
         self.register_buffer("atoms", torch.linspace(v_min, v_max, steps=n_atoms))
         self.n = int(env.single_action_space.n)
@@ -869,10 +792,6 @@ class C51QNetwork(QNetworkAgent):
             nn.Conv2d(64, 64, 3, stride=1), nn.ReLU(), nn.Flatten(), nn.Linear(3136, 512), nn.ReLU(),
             nn.Linear(512, self.n * n_atoms))
         self.num_actions = self.n
-        self.precision = "fp32"
-        self._flat = None
-        self._tc = None
-        self._tc_dirty = True
 
     def _head_outputs(self):
         return self.n * self.n_atoms

@@ -588,11 +588,14 @@ extern "C" int b200rl_impala_bf16_acts_layout(int64_t n, int64_t* offsets) {
     for (int j = 0; j < 9; ++j) offsets[k++] = tail[j];
     return B200RL_OK;
 }
+// the first part of the backward workspace: weight-gradient partials (the small partials follow it)
+static size_t impala_big_bytes() {
+    const size_t conv = wgrad_ws_floats() * 4, fc = (size_t)kFcSplits * 256 * 2048 * 4;
+    return fc > conv ? fc : conv;
+}
 extern "C" size_t b200rl_impala_bf16_workspace_bytes(int64_t n, int A) {
     if (n < 1 || n > kMaxN || !heads_ok(A)) return 0;
-    size_t big = wgrad_ws_floats() * 4;
-    const size_t fc = (size_t)kFcSplits * 256 * 2048 * 4;
-    if (fc > big) big = fc;
+    const size_t big = impala_big_bytes();
     size_t small = (size_t)kWgradCtas * 32 * 4;
     auto mx = [&](size_t v) { if (v > small) small = v; };
     mx((size_t)ceil_div(n, colsum_rows(n)) * 256 * 4);
@@ -715,10 +718,8 @@ extern "C" int b200rl_impala_bf16_backward(const uint8_t* obs, const int64_t* ro
     uint8_t* ab = reinterpret_cast<uint8_t*>(acts);
     auto T = [&](int64_t off) { return reinterpret_cast<bf16*>(ab + off); };
     cudaStream_t s = (cudaStream_t)stream;
-    size_t big = wgrad_ws_floats() * 4;
-    if ((size_t)kFcSplits * 256 * 2048 * 4 > big) big = (size_t)kFcSplits * 256 * 2048 * 4;
     float* wsbig = reinterpret_cast<float*>(workspace);
-    float* wssmall = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(workspace) + big);
+    float* wssmall = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(workspace) + impala_big_bytes());
     const int A1 = A + 1;
     int rc;
     // ---- heads

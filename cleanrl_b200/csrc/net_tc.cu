@@ -447,9 +447,8 @@ extern "C" int b200rl_frames_to_s2d_u8(const uint8_t* obs, const int64_t* rows, 
     return check_launch("frames_to_s2d_u8");
 }
 
-extern "C" size_t b200rl_naturecnn_bf16_workspace_bytes(int64_t n, int A) {
-    if (n < 1 || !head_ok(A)) return 0;
-    const NatureLayout L(A);
+// the first part of the backward workspace: weight-gradient partials (the small partials follow it, 256-B aligned)
+static size_t naturecnn_big_bytes(int64_t n, const NatureLayout& L) {
     size_t a = 0;
     auto mx = [&](size_t v) { if (v > a) a = v; };
     mx((size_t)wgrad_plan(n * 512, kC1Ctas, 128).splits * 256 * 64 * 4);
@@ -457,6 +456,13 @@ extern "C" size_t b200rl_naturecnn_bf16_workspace_bytes(int64_t n, int A) {
     mx((size_t)wgrad_plan(n * 81, kC3Ctas, 128).splits * 640 * 64 * 4);
     mx((size_t)wgrad_plan(n, kFcSplits, 64).splits * 512 * (13 * 256) * 4);
     if (L.wide) mx(wide_big_bytes(n, L));
+    return a;
+}
+
+extern "C" size_t b200rl_naturecnn_bf16_workspace_bytes(int64_t n, int A) {
+    if (n < 1 || !head_ok(A)) return 0;
+    const NatureLayout L(A);
+    const size_t a = naturecnn_big_bytes(n, L);
     size_t b = 0;
     auto mb = [&](size_t v) { if (v > b) b = v; };
     mb(colsum_ws(n * 441, 32)); mb(colsum_ws(n * 100, 64)); mb(colsum_ws(n * 81, 64)); mb(colsum_ws(n, 512));
@@ -562,16 +568,7 @@ extern "C" int b200rl_naturecnn_bf16_backward(const void* obs, const void* obs_a
     const bf16* x0 = obs_format == B200RL_OBS_U8_NCHW ? act + Q.x0 : reinterpret_cast<const bf16*>(obs);   // unused for S2D_U8
     const int64_t* x0rows = obs_format == B200RL_OBS_U8_NCHW ? nullptr : rows;
     // workspace split: [wgrad partials | small partials]
-    size_t big = 0;
-    {
-        auto mx = [&](size_t v) { if (v > big) big = v; };
-        mx((size_t)wgrad_plan(n * 512, kC1Ctas, 128).splits * 256 * 64 * 4);
-        mx((size_t)wgrad_plan(n * 100, kC2Ctas, 128).splits * 512 * 64 * 4);
-        mx((size_t)wgrad_plan(n * 81, kC3Ctas, 128).splits * 640 * 64 * 4);
-        mx((size_t)wgrad_plan(n, kFcSplits, 64).splits * 512 * (13 * 256) * 4);
-        if (L.wide) mx(wide_big_bytes(n, L));
-        big = (big + 255) & ~(size_t)255;
-    }
+    const size_t big = (naturecnn_big_bytes(n, L) + 255) & ~(size_t)255;
     float* wsbig = reinterpret_cast<float*>(workspace);
     float* wssmall = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + big);
     int rc;

@@ -7,6 +7,8 @@ no fallback path.
 """
 from __future__ import annotations
 
+import math
+
 import torch
 
 from . import _lib
@@ -445,39 +447,84 @@ def lstm_cell_bwd(dh_heads, dh_rec_raw, done_next, dc_rec, save, c_masked, done,
     _lib.check(rc, "lstm_cell_bwd")
 
 
-# ------------------------------------------------------ NatureCNN bf16 (wgmma) plan
-class NatureCNNBf16:
-    """Owns the packed bf16 weights and activation workspaces of the tensor-core NatureCNN path."""
+# ------------------------------------------------------ tensor-core (bf16) network plans
+class _TensorCorePlan:
+    """Owns the device memory of one tensor-core network: the packed bf16 weights, the activation workspaces (one per
+    batch shape) and the grow-only backward workspace.  Subclasses name their C entry points by ``NET``
+    (``b200rl_<NET>_param_count``, ``b200rl_<NET>_bf16_{packed_bytes,pack,acts_bytes,acts_layout,workspace_bytes}``)
+    and marshal the arguments of their forward / backward calls.
+
+    A captured CUDA graph (and the CUtensorMaps baked into it) holds raw device pointers into these workspaces, so
+    ``pin()`` runs after every capture: each workspace that exists at that moment then lives as long as the plan, whether
+    it is an activation workspace of a batch shape or a backward workspace superseded by a larger one."""
+
+    NET = NAME = None
+    MAX_A = 23               # widest supported action space
+    MAX_UNPINNED = 4         # activation workspaces kept for batch shapes that no captured graph references
 
     def __init__(self, A, device):
-        lib = _lib.load()
         self.A, self.device = int(A), device
-        self.param_count = lib.b200rl_naturecnn_param_count(self.A)
-        self.packed = torch.empty(lib.b200rl_naturecnn_bf16_packed_bytes(self.A), dtype=torch.uint8, device=device)
-        self._acts = {}          # (n, fmt) -> workspace, in least-recently-used order
-        self._pinned = set()     # keys referenced by captured CUDA graphs (raw pointers baked in): never evicted
-        self._ws = None
+        nbytes = self._c("packed_bytes")(self.A)
+        if nbytes == 0:
+            raise ValueError(f"{self.NAME} supports 1 <= A <= {self.MAX_A} actions (got {A})")
+        self.param_count = getattr(_lib.load(), f"b200rl_{self.NET}_param_count")(self.A)
+        self.packed = torch.empty(nbytes, dtype=torch.uint8, device=device)
+        self._acts = {}          # batch shape -> activation workspace, least-recently-used first
+        self._pinned = set()     # batch shapes referenced by captured CUDA graphs: never evicted
+        self._ws = None          # backward workspace (grow-only)
+        self._pinned_ws = []     # backward workspaces referenced by captured CUDA graphs
 
-    MAX_UNPINNED = 4
+    def _c(self, name):
+        return getattr(_lib.load(), f"b200rl_{self.NET}_bf16_{name}")
 
     def pin(self):
-        """Called by the engine after a CUDA-graph capture: every workspace that exists now may be referenced by a
-        graph (and by its baked CUtensorMaps) through its raw device pointer, so it must outlive the graph."""
-        self._pinned.update(self._acts.keys())
+        """Every workspace that exists now may be referenced by a captured CUDA graph: keep it alive."""
+        self._pinned.update(self._acts)
+        if self._ws is not None and all(w is not self._ws for w in self._pinned_ws):
+            self._pinned_ws.append(self._ws)
 
-    def acts(self, n, fmt):
-        lib = _lib.load()
-        key = (n, fmt)
+    def acts(self, *shape):
+        """The activation workspace of one batch shape, least recently used ones evicted unless pinned."""
+        key = tuple(int(d) for d in shape)
         buf = self._acts.pop(key, None)
         if buf is None:
-            # bounded cache of batch shapes: evict least-recently-used workspaces that no graph can reference
             unpinned = [k for k in self._acts if k not in self._pinned]
             while len(unpinned) >= self.MAX_UNPINNED:
                 del self._acts[unpinned.pop(0)]
+            nbytes = self._c("acts_bytes")(*key)
+            if nbytes == 0:
+                raise ValueError(f"{self.NAME}: batch shape {key} is out of range")
             # zero-initialised: the padded-grid gradient buffers rely on never-written positions being 0
-            buf = torch.zeros(lib.b200rl_naturecnn_bf16_acts_bytes(n, fmt), dtype=torch.uint8, device=self.device)
+            buf = torch.zeros(nbytes, dtype=torch.uint8, device=self.device)
         self._acts[key] = buf    # most recently used = last
         return buf
+
+    def _named_views(self, shape, specs):
+        """``{name: view}`` of the activation workspace ``acts(*shape)``; ``specs`` lists ``(name, dtype, shape)`` in the
+        order of the C layout table, whose negative offsets mark tensors the layout does not have."""
+        import ctypes
+        off = (ctypes.c_int64 * len(specs))()
+        _lib.check(self._c("acts_layout")(*shape, off), f"{self.NET}_acts_layout")
+        buf = self.acts(*shape)
+        return {name: buf[o:o + math.prod(dims) * dtype.itemsize].view(dtype).view(*dims)
+                for o, (name, dtype, dims) in zip(off, specs) if o >= 0}
+
+    def workspace(self, *shape):
+        """The backward workspace for one batch shape: grows, never shrinks."""
+        nbytes = self._c("workspace_bytes")(*shape, self.A)
+        if self._ws is None or self._ws.numel() < nbytes:
+            self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        return self._ws
+
+    def pack(self, flat_params):
+        rc = self._c("pack")(_ptr(flat_params, torch.float32, "params"), self.A, self.packed.data_ptr(), _stream())
+        _lib.check(rc, f"{self.NET}_bf16_pack")
+
+
+class NatureCNNBf16(_TensorCorePlan):
+    """The tensor-core NatureCNN; its activation workspaces are keyed by (n, obs format)."""
+
+    NET, NAME, MAX_A = "naturecnn", "tensor-core NatureCNN", 2047
 
     @staticmethod
     def obs_format(obs):
@@ -489,12 +536,6 @@ class NatureCNNBf16:
             return 2
         raise TypeError("tensor-core NatureCNN path consumes uint8 [*,4,84,84] frames, uint8 space-to-depth rollout rows "
                         f"[*,441,64] or space-to-depth bf16 [*,21,21,64] (got {obs.dtype} {tuple(obs.shape)})")
-
-    def pack(self, flat_params):
-        lib = _lib.load()
-        rc = lib.b200rl_naturecnn_bf16_pack(_ptr(flat_params, torch.float32, "params"), self.A,
-                                            self.packed.data_ptr(), _stream())
-        _lib.check(rc, "naturecnn_bf16_pack")
 
     def forward(self, obs, rows, flat_params, head_out=None):
         lib = _lib.load()
@@ -524,100 +565,37 @@ class NatureCNNBf16:
             _contig(obs_aux, "obs_aux")
         n = dhead.shape[0]
         _contig(dhead, "dhead")
-        nbytes = lib.b200rl_naturecnn_bf16_workspace_bytes(n, self.A)
-        if self._ws is None or self._ws.numel() < nbytes:
-            self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        ws = self.workspace(n)
         rc = lib.b200rl_naturecnn_bf16_backward(_ptr(obs, None, "obs"), _ptr(obs_aux, None, "obs_aux", True), fmt,
                                                 _ptr(rows, torch.int64, "rows", True), n, self.A,
                                                 _ptr(flat_params, torch.float32, "params"), self.packed.data_ptr(),
                                                 self.acts(n, fmt).data_ptr(), _ptr(dhead, torch.float32, "dhead"),
-                                                _ptr(flat_grads, torch.float32, "grads"),
-                                                self._ws.data_ptr(), self._ws.numel(),
+                                                _ptr(flat_grads, torch.float32, "grads"), ws.data_ptr(), ws.numel(),
                                                 tail_event.cuda_event if tail_event is not None else None, _stream())
         _lib.check(rc, "naturecnn_bf16_backward")
 
 
-# ------------------------------------------------------ IMPALA-CNN bf16 (tensor-core) plan
-class ImpalaCNNBf16:
-    """Owns the packed bf16 weights, the activation workspaces and the backward workspace of the tensor-core
-    IMPALA-CNN (procgen frames uint8 [*, 64, 64, 3])."""
+class ImpalaCNNBf16(_TensorCorePlan):
+    """The tensor-core IMPALA-CNN (procgen frames uint8 [*, 64, 64, 3]); its activation workspaces are keyed by n."""
 
-    MAX_UNPINNED = 4
-
-    def __init__(self, A, device):
-        lib = _lib.load()
-        self.A, self.device = int(A), device
-        nbytes = lib.b200rl_impala_bf16_packed_bytes(self.A)
-        if nbytes == 0:
-            raise ValueError(f"tensor-core IMPALA-CNN supports 1 <= A <= 23 actions (got {A})")
-        self.param_count = lib.b200rl_impala_param_count(self.A)
-        self.packed = torch.empty(nbytes, dtype=torch.uint8, device=device)
-        self._acts = {}          # n -> workspace, least-recently-used first
-        self._pinned = set()     # batch sizes referenced by captured CUDA graphs: never evicted
-        self._ws = None
-        self._pinned_ws = []     # backward workspaces referenced by captured CUDA graphs
-
-    def pin(self):
-        """Every workspace that exists now may be referenced by a captured CUDA graph: keep it alive."""
-        self._pinned.update(self._acts.keys())
-        if self._ws is not None and all(w is not self._ws for w in self._pinned_ws):
-            self._pinned_ws.append(self._ws)
-
-    def acts(self, n):
-        lib = _lib.load()
-        buf = self._acts.pop(n, None)
-        if buf is None:
-            unpinned = [k for k in self._acts if k not in self._pinned]
-            while len(unpinned) >= self.MAX_UNPINNED:
-                del self._acts[unpinned.pop(0)]
-            nbytes = lib.b200rl_impala_bf16_acts_bytes(n)
-            if nbytes == 0:
-                raise ValueError(f"tensor-core IMPALA-CNN: batch of {n} rows is out of range")
-            buf = torch.zeros(nbytes, dtype=torch.uint8, device=self.device)
-        self._acts[n] = buf
-        return buf
+    NET, NAME = "impala", "tensor-core IMPALA-CNN"
 
     def act_tensors(self, n):
         """Named views of the activation workspace of batch size ``n`` (layout: b200rl_impala_bf16_acts_layout)."""
-        import ctypes
-        off = (ctypes.c_int64 * 30)()
-        _lib.check(_lib.load().b200rl_impala_bf16_acts_layout(n, off), "impala_acts_layout")
-        buf = self.acts(n)
         bf, u8, i32 = torch.bfloat16, torch.uint8, torch.int32
-
-        def view(o, dtype, shape):
-            cnt = 1
-            for d in shape:
-                cnt *= d
-            nb = cnt * torch.tensor([], dtype=dtype).element_size()
-            return buf[o:o + nb].view(dtype).view(*shape)
-        out, k = {}, 3
-        for name, shp in (("c0", (n, 64, 64, 16)), ("c1", (n, 32, 32, 32)), ("c2", (n, 16, 16, 32))):
-            out[name] = view(off[["c0", "c1", "c2"].index(name)], bf, shp)
+        specs = [("c0", bf, (n, 64, 64, 16)), ("c1", bf, (n, 32, 32, 32)), ("c2", bf, (n, 16, 16, 32))]
         for q, shp in enumerate(((n, 32, 32, 16), (n, 16, 16, 32), (n, 8, 8, 32))):
-            for name in ("s0", "s1", "s2", "y0", "y1"):
-                if off[k] >= 0:
-                    out[f"{name}_{q}"] = view(off[k], bf, shp)
-                k += 1
-            out[f"arg_{q}"] = view(off[k], u8, shp)
-            k += 1
-        for name, dtype, shp in (("h0", bf, (n, 2048)), ("mh0", i32, (n, 64)), ("hid", bf, (n, 256)), ("mhid", i32, (n, 8)),
-                                 ("dc", bf, (n, 65536)), ("ga", bf, (n, 16384)), ("gb", bf, (n, 16384)),
-                                 ("gy", bf, (n, 16384)), ("dhid", bf, (n, 256))):
-            out[name] = view(off[k], dtype, shp)
-            k += 1
-        return out
+            specs += [(f"{name}_{q}", bf, shp) for name in ("s0", "s1", "s2", "y0", "y1")] + [(f"arg_{q}", u8, shp)]
+        specs += [("h0", bf, (n, 2048)), ("mh0", i32, (n, 64)), ("hid", bf, (n, 256)), ("mhid", i32, (n, 8)),
+                  ("dc", bf, (n, 65536)), ("ga", bf, (n, 16384)), ("gb", bf, (n, 16384)), ("gy", bf, (n, 16384)),
+                  ("dhid", bf, (n, 256))]
+        return self._named_views((n,), specs)
 
     @staticmethod
     def check_obs(obs):
         if obs.dtype != torch.uint8 or obs.dim() < 4 or tuple(obs.shape[-3:]) != (64, 64, 3):
             raise ValueError("tensor-core IMPALA-CNN consumes uint8 frames [*, 64, 64, 3] "
                              f"(got {obs.dtype} {tuple(obs.shape)})")
-
-    def pack(self, flat_params):
-        rc = _lib.load().b200rl_impala_bf16_pack(_ptr(flat_params, torch.float32, "params"), self.A,
-                                                 self.packed.data_ptr(), _stream())
-        _lib.check(rc, "impala_bf16_pack")
 
     def forward(self, obs, rows, flat_params, head_out=None):
         self.check_obs(obs)
@@ -635,95 +613,39 @@ class ImpalaCNNBf16:
 
     def backward(self, obs, rows, flat_params, dhead, flat_grads):
         """Gradient of the forward that last ran on (obs, rows) with this batch size; fills ``flat_grads``."""
-        lib = _lib.load()
         self.check_obs(obs)
         _contig(dhead, "dhead")
         n = dhead.shape[0]
-        nbytes = lib.b200rl_impala_bf16_workspace_bytes(n, self.A)
-        if self._ws is None or self._ws.numel() < nbytes:
-            self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-        rc = lib.b200rl_impala_bf16_backward(_ptr(obs, torch.uint8, "obs"), _ptr(rows, torch.int64, "rows", True), n, self.A,
-                                             _ptr(flat_params, torch.float32, "params"), self.packed.data_ptr(),
-                                             self.acts(n).data_ptr(), _ptr(dhead, torch.float32, "dhead"),
-                                             _ptr(flat_grads, torch.float32, "grads"), self._ws.data_ptr(), self._ws.numel(),
-                                             _stream())
+        ws = self.workspace(n)
+        rc = _lib.load().b200rl_impala_bf16_backward(_ptr(obs, torch.uint8, "obs"), _ptr(rows, torch.int64, "rows", True), n,
+                                                     self.A, _ptr(flat_params, torch.float32, "params"), self.packed.data_ptr(),
+                                                     self.acts(n).data_ptr(), _ptr(dhead, torch.float32, "dhead"),
+                                                     _ptr(flat_grads, torch.float32, "grads"), ws.data_ptr(), ws.numel(), _stream())
         _lib.check(rc, "impala_bf16_backward")
 
 
-# ------------------------------------------------------ recurrent agent bf16 (tensor-core) plan
-class LSTMAgentBf16:
-    """Owns the packed bf16 weights, the activation workspaces and the backward workspace of the tensor-core recurrent
-    agent (single uint8 frames [*, 1, 84, 84], NatureCNN trunk, LSTM(512, 128), heads).  Sequences are S steps x n envs,
-    time-major."""
+class LSTMAgentBf16(_TensorCorePlan):
+    """The tensor-core recurrent agent (single uint8 frames [*, 1, 84, 84], NatureCNN trunk, LSTM(512, 128), heads).
+    Sequences are S steps x n envs, time-major; the activation workspaces are keyed by (S, n)."""
 
-    MAX_UNPINNED = 4
+    NET, NAME = "lstm_agent", "tensor-core LSTM agent"
     H = 128
-
-    def __init__(self, A, device):
-        lib = _lib.load()
-        self.A, self.device = int(A), device
-        nbytes = lib.b200rl_lstm_agent_bf16_packed_bytes(self.A)
-        if nbytes == 0:
-            raise ValueError(f"tensor-core LSTM agent supports 1 <= A <= 23 actions (got {A})")
-        self.param_count = lib.b200rl_lstm_agent_param_count(self.A)
-        self.packed = torch.empty(nbytes, dtype=torch.uint8, device=device)
-        self._acts = {}          # (S, n) -> workspace, least-recently-used first
-        self._pinned = set()     # shapes referenced by captured CUDA graphs: never evicted
-        self._ws = None
-        self._pinned_ws = []
-
-    def pin(self):
-        """Every workspace that exists now may be referenced by a captured CUDA graph: keep it alive."""
-        self._pinned.update(self._acts.keys())
-        if self._ws is not None and all(w is not self._ws for w in self._pinned_ws):
-            self._pinned_ws.append(self._ws)
-
-    def acts(self, S, n):
-        key = (int(S), int(n))
-        buf = self._acts.pop(key, None)
-        if buf is None:
-            unpinned = [k for k in self._acts if k not in self._pinned]
-            while len(unpinned) >= self.MAX_UNPINNED:
-                del self._acts[unpinned.pop(0)]
-            nbytes = _lib.load().b200rl_lstm_agent_bf16_acts_bytes(*key)
-            if nbytes == 0:
-                raise ValueError(f"tensor-core LSTM agent: {S} steps x {n} envs is out of range")
-            # zero-initialised: the padded-grid gradient buffers rely on never-written positions being 0
-            buf = torch.zeros(nbytes, dtype=torch.uint8, device=self.device)
-        self._acts[key] = buf
-        return buf
 
     def act_tensors(self, S, n):
         """Named views of the activation workspace of (S, n) (layout: b200rl_lstm_agent_bf16_acts_layout)."""
-        import ctypes
-        off = (ctypes.c_int64 * 13)()
-        _lib.check(_lib.load().b200rl_lstm_agent_bf16_acts_layout(S, n, off), "lstm_acts_layout")
-        buf = self.acts(S, n)
         M = S * n
         bf, f32, i32 = torch.bfloat16, torch.float32, torch.int32
-        out = {}
-        for k, (name, dtype, shape) in enumerate((
-                ("act1", bf, (M, 10, 10, 128)), ("m1", i32, (M, 400)), ("act2", bf, (M, 9, 9, 64)), ("act3", bf, (M, 7, 7, 64)),
-                ("feats", bf, (M, 512)), ("m4", i32, (M, 16)),
-                ("gx", f32, (M, 512)), ("hseq", bf, (M, 128)), ("hm", bf, (M, 128)), ("save", f32, (M, 5, 128)),
-                ("cm", f32, (M, 128)), ("dgates", f32, (M, 512)), ("dfeats", bf, (M, 512)))):
-            cnt = 1
-            for d in shape:
-                cnt *= d
-            nb = cnt * torch.tensor([], dtype=dtype).element_size()
-            out[name] = buf[off[k]:off[k] + nb].view(dtype).view(*shape)
-        return out
+        return self._named_views((S, n), [
+            ("act1", bf, (M, 10, 10, 128)), ("m1", i32, (M, 400)), ("act2", bf, (M, 9, 9, 64)), ("act3", bf, (M, 7, 7, 64)),
+            ("feats", bf, (M, 512)), ("m4", i32, (M, 16)),
+            ("gx", f32, (M, 512)), ("hseq", bf, (M, 128)), ("hm", bf, (M, 128)), ("save", f32, (M, 5, 128)),
+            ("cm", f32, (M, 128)), ("dgates", f32, (M, 512)), ("dfeats", bf, (M, 512))])
 
     @staticmethod
     def check_obs(obs):
         if obs.dtype != torch.uint8 or obs.dim() != 4 or tuple(obs.shape[-3:]) != (1, 84, 84):
             raise ValueError("tensor-core LSTM agent consumes uint8 frames [*, 1, 84, 84] "
                              f"(got {obs.dtype} {tuple(obs.shape)})")
-
-    def pack(self, flat_params):
-        rc = _lib.load().b200rl_lstm_agent_bf16_pack(_ptr(flat_params, torch.float32, "params"), self.A,
-                                                     self.packed.data_ptr(), _stream())
-        _lib.check(rc, "lstm_agent_bf16_pack")
 
     def forward(self, obs, rows, S, n, flat_params, h0, c0, done, head_out=None, h_out=None, c_out=None):
         """(head_out [S*n, A+1], h_S [n, 128], c_S [n, 128]); the sequence's activations stay in the workspace."""
@@ -757,17 +679,14 @@ class LSTMAgentBf16:
 
     def backward(self, obs, rows, S, n, flat_params, done, dhead, flat_grads):
         """Gradient of the forward that last ran on (obs, rows, S, n, done); fills ``flat_grads``."""
-        lib = _lib.load()
         self.check_obs(obs)
         _contig(dhead, "dhead")
-        nbytes = lib.b200rl_lstm_agent_bf16_workspace_bytes(S, n, self.A)
-        if self._ws is None or self._ws.numel() < nbytes:
-            self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        ws = self.workspace(S, n)
         f = torch.float32
-        rc = lib.b200rl_lstm_agent_bf16_backward(
+        rc = _lib.load().b200rl_lstm_agent_bf16_backward(
             _ptr(obs, torch.uint8, "obs"), _ptr(rows, torch.int64, "rows", True), S, n, self.A,
             _ptr(flat_params, f, "params"), self.packed.data_ptr(), _ptr(done, f, "done"), self.acts(S, n).data_ptr(),
-            _ptr(dhead, f, "dhead"), _ptr(flat_grads, f, "grads"), self._ws.data_ptr(), self._ws.numel(), _stream())
+            _ptr(dhead, f, "dhead"), _ptr(flat_grads, f, "grads"), ws.data_ptr(), ws.numel(), _stream())
         _lib.check(rc, "lstm_agent_bf16_backward")
 
 

@@ -76,7 +76,7 @@ class PPOEngine:
         # [T,N,21,21,64] (converted per env step from the uint8 staging batch); every minibatch pass
         # then gathers 128-byte pixels directly -- no per-minibatch uint8 decode, no fp32 obs.
         self.sort_minibatch = os.environ.get("CLEANRL_B200_SORT_MINIBATCH", "1") != "0"
-        self.s2d = (getattr(agent, "precision", "fp32") == "bf16" and self.obs_dtype == torch.uint8
+        self.s2d = (agent.uses_tc_plan() and self.obs_dtype == torch.uint8
                     and tuple(obs_shape) == (4, 84, 84) and device.type == "cuda")
         # uint8 rollout (default): every frame is kept ONCE per orientation as 1-byte space-to-depth pixels --
         # row-major [T,N,441,64] for conv1's forward on the integer tensor cores, channel-major [T,N,64,448] for its weight
@@ -93,7 +93,7 @@ class PPOEngine:
             self.obs_u8 = torch.zeros((N,) + tuple(obs_shape), dtype=torch.uint8, device=device)
         else:
             self.obs = torch.zeros((T, N) + tuple(obs_shape), dtype=self.obs_dtype, device=device)
-        self.act_dim = int(getattr(agent, "action_dim", 0))
+        self.act_dim = int(agent.action_dim)
         if self.act_dim:     # continuous actions (ppo_continuous_action.py:213): f32 [T, N, D]
             self.actions = torch.zeros((T, N, self.act_dim), dtype=f32, device=device)
         else:                # discrete: stored as int64 (the reference stores fp32 and re-casts .long() per minibatch)
@@ -132,7 +132,7 @@ class PPOEngine:
         self.hyper = torch.zeros(max(n_upd, 1), 2, dtype=f32, device=device)
         self.hyper_h = _pin(torch.zeros(max(n_upd, 1), 2, dtype=f32))
         self.flat = agent.flat
-        if self.overlap_exchange and hasattr(agent, "grad_tail"):
+        if self.overlap_exchange:
             agent.grad_tail()          # create the tail event BEFORE the first backward records it
         # One CUDA graph per rollout slot: the per-step device work (frame conversion, 5 network launches, noise
         # draw, sampler) becomes a single graph launch that writes straight into obs[t]/actions[t]/...; the
@@ -236,12 +236,12 @@ class PPOEngine:
         return self._run_graphed(lambda: self._step_device_work(step), step, warm_key=("f", 0))
 
     def _graphable(self):
-        return self.cuda_graphs and getattr(self.agent, "graph_capturable", getattr(self.agent, "graph_friendly", False))
+        return self.cuda_graphs and self.agent.graph_capturable
 
     def _run_graphed(self, work, key, warm_key):
         if not self._graphable():
             return work()
-        if hasattr(self.agent, "_tc_plan") and getattr(self.agent, "precision", "fp32") == "bf16":
+        if self.agent.uses_tc_plan():
             self.agent._tc_plan()                      # (re)pack weights outside the graph
         g = self._graphs.get(key)
         if g is None:
@@ -259,8 +259,7 @@ class PPOEngine:
             with torch.cuda.graph(g, pool=self._graph_pool):
                 work()
             self._graphs[key] = g
-            if hasattr(self.agent, "pin_workspaces"):
-                self.agent.pin_workspaces()     # captured graphs hold raw pointers into the activation workspaces
+            self.agent.pin_workspaces()     # captured graphs hold raw pointers into the plan's workspaces
             self._graph_kernels[key] = _lib.load().b200rl_launch_count() - l0
         g.replay()
         self.graph_launches += self._graph_kernels[key]
@@ -326,7 +325,7 @@ class PPOEngine:
                     self.obs[step].copy_(src)
                 self.agent.sample_into(self.obs[step], self.actions[step], self.logprobs[step], self.values[step])
 
-        if not getattr(self.agent, "graph_friendly", False):
+        if not self.agent.graph_friendly:
             return work()          # the noise draw cannot be captured: plain launches
         self._run_graphed(work, ("rollout", obs_pool.data_ptr(), P), warm_key="r")
 
@@ -642,7 +641,7 @@ class PPOEngine:
         P = len(env_parts)
         self._part_setup(P)
         obs_parts, done_parts = list(obs_parts), list(done_parts)
-        if hasattr(self.agent, "_tc_plan") and getattr(self.agent, "precision", "fp32") == "bf16":
+        if self.agent.uses_tc_plan():
             self.agent._tc_plan()          # (re)pack the weights once: they do not change during a rollout
         self._noise_step = -1
         if self._delta is not None:
@@ -727,7 +726,7 @@ class PPOEngine:
         E = int(a.update_epochs)
         nmb = self.num_minibatches
         graphed = (self.update_graphs and a.target_kl is None and self._graphable() and self._upd_iters >= 1
-                   and getattr(self.agent, "precision", "fp32") == "bf16" and hasattr(self.agent, "_tc_plan")
+                   and self.agent.uses_tc_plan()
                    and (self.world_size == 1 or os.environ.get("CLEANRL_B200_UPDATE_GRAPHS_DP", "0") == "1"))
         self._upd_iters += 1
         if graphed:
@@ -760,8 +759,7 @@ class PPOEngine:
                     break
         if graphed:
             self.flat.step += E * nmb
-            if hasattr(self.agent, "params_updated"):
-                self.agent.params_updated()      # no python ran inside the replays: the packed operand copies are stale
+            self.agent.params_updated()      # no python ran inside the replays: the packed operand copies are stale
         self.stats_h[:k].copy_(self.stats[:k], non_blocking=True)
         t_sy = time.perf_counter()
         self.host_seconds["update_enqueue"] += t_sy - t_up
@@ -788,7 +786,7 @@ class PPOEngine:
 
     def _capture_epoch(self, epoch):
         from . import _lib
-        if epoch == 0 and hasattr(self.agent, "params_updated"):
+        if epoch == 0:
             self.agent.params_updated()     # the graph of epoch 0 always starts by packing the weights it was given
         l0 = _lib.load().b200rl_launch_count()
         g = torch.cuda.CUDAGraph()
@@ -798,8 +796,7 @@ class PPOEngine:
             self._epoch_work(epoch, None, epoch * self.num_minibatches, True)
         self._upd_graphs[epoch] = g
         self._upd_kernels[epoch] = _lib.load().b200rl_launch_count() - l0
-        if hasattr(self.agent, "pin_workspaces"):
-            self.agent.pin_workspaces()
+        self.agent.pin_workspaces()
         return g
 
     @torch.no_grad()
@@ -828,8 +825,7 @@ class PPOEngine:
             ops.clip_adam(flat.flat, flat.grad, flat.exp_avg, flat.exp_avg_sq, flat.step, lr,
                           eps=1e-5, max_norm=a.max_grad_norm, world_size=self.world_size,
                           norm_out=self.grad_norm)
-        if hasattr(agent, "params_updated"):
-            agent.params_updated()
+        agent.params_updated()
 
     def _exchange_gradients(self):
         """The ONE data-parallel exchange per update: SUM of the flat gradient over ranks (the mean's 1/world_size is
@@ -839,7 +835,7 @@ class PPOEngine:
         run, underneath the convolution backward; only the 78 k conv gradients are exchanged after the
         backward.  Both parts are elementwise sums of disjoint slices: same result as one all-reduce."""
         flat = self.flat
-        tail = self.agent.grad_tail() if (self.overlap_exchange and hasattr(self.agent, "grad_tail")) else None
+        tail = self.agent.grad_tail() if self.overlap_exchange else None
         if tail is None:
             self.all_reduce(flat.grad)
             return

@@ -121,7 +121,7 @@ def install():
         _saved[(cls, "bind")] = agents.KernelAgent.bind
         for attr, fn in (("_forward_heads", _torch_heads), ("forward_train", _forward_train),
                          ("alloc_head_grad", _alloc_head_grad), ("backward", _backward)):
-            _saved[(cls, attr)] = getattr(cls, attr)
+            _saved[(cls, attr)] = cls.__dict__.get(attr)        # None: inherited from a base class
             setattr(cls, attr, fn)
     agents.KernelAgent.bind = _bind_cpu
     _saved[(agents.KernelAgent, "_build_plan")] = agents.KernelAgent._build_plan
@@ -137,6 +137,8 @@ def uninstall():
             setattr(ops, k, v)
         elif k[1] == "bind":
             agents.KernelAgent.bind = v
+        elif v is None:
+            delattr(k[0], k[1])
         else:
             setattr(k[0], k[1], v)
     _saved.clear()

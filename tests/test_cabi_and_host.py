@@ -63,6 +63,32 @@ def test_ops_reject_cpu_tensors(lib):
         ops.clip_adam(x.view(-1), x.view(-1), x.view(-1), x.view(-1), 1, 1e-3)
 
 
+def test_tensor_core_plan_workspace_rules(lib):
+    """The workspace bookkeeping every tensor-core plan shares, on host memory (the sizes are host functions): zeroed
+    activation workspaces, at most MAX_UNPINNED of them for unpinned batch shapes (least recently used evicted first),
+    shapes pinned after a graph capture never evicted, and a pinned backward workspace kept alive after a larger batch
+    supersedes it."""
+    import torch
+    from cleanrl_b200 import ops
+    cpu = torch.device("cpu")
+    with pytest.raises(ValueError, match="actions"):
+        ops.NatureCNNBf16(2048, cpu)
+    for plan, shape in ((ops.NatureCNNBf16(6, cpu), lambda n: (n, 2)), (ops.ImpalaCNNBf16(15, cpu), lambda n: (n,)),
+                        (ops.LSTMAgentBf16(6, cpu), lambda n: (4, n))):
+        first = plan.acts(*shape(1))
+        assert first.numel() > 0 and not first.any()
+        ws = plan.workspace(*shape(1))
+        plan.pin()
+        plan.pin()
+        for n in (2, 3, 4, 5, 2, 9):         # 5 unpinned shapes, 2 used again before 9 arrives: 3 is evicted
+            plan.acts(*shape(n))
+        assert list(plan._acts) == [shape(n) for n in (1, 4, 5, 2, 9)]
+        assert plan.acts(*shape(1)) is first
+        big = plan.workspace(*shape(128))
+        assert big.numel() > ws.numel() and plan.workspace(*shape(1)) is big
+        assert [w is ws for w in plan._pinned_ws] == [True]
+
+
 def test_script_refuses_to_run_without_cuda():
     import torch
     if torch.cuda.is_available():
