@@ -38,7 +38,6 @@ namespace imp {
 
 constexpr int kThreads = 256;
 constexpr int kWgradCtas = 264;           // row splits of the conv weight gradients: two waves on 132 SMs
-constexpr int kFcSplits = 8;
 
 __device__ __forceinline__ float bf_lo(uint32_t w) { return __uint_as_float(w << 16); }
 __device__ __forceinline__ float bf_hi(uint32_t w) { return __uint_as_float(w & 0xFFFF0000u); }
@@ -562,7 +561,6 @@ static int run_wgrad(WgradP p, int64_t n, float scale, float* dw, float* db, cud
 }
 
 static size_t wgrad_ws_floats() { return (size_t)kWgradCtas * 32 * 288; }
-static int64_t colsum_rows(int64_t n) { const int64_t r = ceil_div(n, 132 * 3); return r < 64 ? 64 : r; }
 
 }  // namespace imp
 }  // namespace b200rl
@@ -588,19 +586,13 @@ extern "C" int b200rl_impala_bf16_acts_layout(int64_t n, int64_t* offsets) {
     for (int j = 0; j < 9; ++j) offsets[k++] = tail[j];
     return B200RL_OK;
 }
-// the first part of the backward workspace: weight-gradient partials (the small partials follow it)
-static size_t impala_big_bytes() {
-    const size_t conv = wgrad_ws_floats() * 4, fc = (size_t)kFcSplits * 256 * 2048 * 4;
-    return fc > conv ? fc : conv;
-}
+// the backward workspace = [big part: weight-gradient partials, sized for the largest n | small part], each the largest
+// its launches need: heads, fc, convolutions
+static size_t impala_big_bytes() { return std::max(wgrad_tma_bytes(kMaxN, 256, 2048), wgrad_ws_floats() * 4); }
 extern "C" size_t b200rl_impala_bf16_workspace_bytes(int64_t n, int A) {
     if (n < 1 || n > kMaxN || !heads_ok(A)) return 0;
-    const size_t big = impala_big_bytes();
-    size_t small = (size_t)kWgradCtas * 32 * 4;
-    auto mx = [&](size_t v) { if (v > small) small = v; };
-    mx((size_t)ceil_div(n, colsum_rows(n)) * 256 * 4);
-    mx((size_t)2 * ceil_div(n, heads_rows_per_block(n)) * (A + 1) * 258 * 4);
-    return big + small + 512;
+    const size_t small = std::max({heads_partial_bytes(n, A + 1, 256), colsum_ws(n, 256), (size_t)kWgradCtas * 32 * 4});
+    return impala_big_bytes() + small + 512;
 }
 
 extern "C" int b200rl_impala_bf16_pack(const float* params, int A, void* packed, void* stream) {
@@ -694,11 +686,8 @@ extern "C" int b200rl_impala_bf16_forward(const uint8_t* obs, const int64_t* row
     g.mask_out = reinterpret_cast<uint32_t*>(ab + Q.mhid);
     { ProfScope ps(s, "fc_fwd", 2.0 * n * 256 * 2048, (double)n * (2048 + 256) * 2 + 256.0 * 2048 * 2);
       if ((rc = launch_gemm_tma<64, 6>(g, s, "impala/fc"))) return rc; }
-    { ProfScope ps(s, "heads_fwd", 2.0 * n * 256 * (A + 1), (double)n * (512 + 4 * (A + 1)));
-      const int hb = (int)std::min<int64_t>(ceil_div(n, 8), (int64_t)num_sms() * 8);
-      tc_heads_fwd<256><<<hb, 256, (size_t)(A + 1) * 1024, s>>>(T(Q.hid), params + L.hw, params + L.hb, n, A + 1, 256, head_out);
-      if ((rc = check_launch("impala/heads"))) return rc; }
-    return B200RL_OK;
+    ProfScope ps(s, "heads_fwd", 2.0 * n * 256 * (A + 1), (double)n * (512 + 4 * (A + 1)));
+    return heads_fwd<256>(T(Q.hid), params + L.hw, params + L.hb, n, A + 1, head_out, s, "impala/heads");
 }
 
 extern "C" int b200rl_impala_bf16_backward(const uint8_t* obs, const int64_t* rows, int64_t n, int A, const float* params,
@@ -725,35 +714,17 @@ extern "C" int b200rl_impala_bf16_backward(const uint8_t* obs, const int64_t* ro
     // ---- heads
     {
         ProfScope ps(s, "heads_bwd", 4.0 * n * 256 * A1, (double)n * (1024 + 8 * A1));
-        const int64_t rpb = heads_rows_per_block(n);
-        const int nb = (int)ceil_div(n, rpb);
-        const size_t sd = (size_t)rpb * A1 * sizeof(float);
-        if (A1 <= 8) tc_heads_bwd_weight<8, 256><<<nb, 256, sd, s>>>(dhead, T(Q.hid), n, A1, 256, rpb, wssmall);
-        else tc_heads_bwd_weight<kMaxHeads, 256><<<nb, 256, sd, s>>>(dhead, T(Q.hid), n, A1, 256, rpb, wssmall);
-        tc_heads_fold<<<(unsigned)ceil_div(A1 * 258, 32), 256, 0, s>>>(wssmall, 2 * nb, A1, 256, grads + L.hw, grads + L.hb);
-        const int db = (int)std::min<int64_t>(ceil_div(n * 32, 256), (int64_t)num_sms() * 8);
-        tc_heads_bwd_data<256><<<db, 256, (size_t)A1 * 1024, s>>>(dhead, params + L.hw, ab + Q.mhid, n, A1, 256, T(Q.dhid));
-        if ((rc = check_launch("impala/heads_bwd", 3))) return rc;
+        if ((rc = heads_bwd_weight<256>(dhead, T(Q.hid), n, A1, wssmall, grads + L.hw, grads + L.hb, s, "impala/heads_bwd"))) return rc;
+        if ((rc = heads_bwd_data<256>(dhead, params + L.hw, ab + Q.mhid, n, A1, T(Q.dhid), s, "impala/heads_bwd"))) return rc;
     }
     // ---- fc: dW = dhid^T . h0 (row splits folded in order), db = column sums, dh0 = (dhid . Wfc) * (h0 > 0)
     {
         ProfScope ps(s, "fc_wgrad", 2.0 * n * 256 * 2048, (double)n * (2048 + 256) * 2 + 256.0 * 2048 * 4);
-        int64_t rpc = ceil_div(ceil_div(n, kFcSplits), 64) * 64;
-        const int splits = (int)ceil_div(n, rpc);
-        CUtensorMap tmX, tmY;
-        if ((rc = make_tmap_2d(&tmX, T(Q.dhid), n, 256, 64, "impala/fc_wgrad"))) return rc;
-        if ((rc = make_tmap_2d(&tmY, T(Q.h0), n, 2048, 64, "impala/fc_wgrad"))) return rc;
-        const size_t smem = (size_t)4 * (kFcWgradXChunks + kFcWgradYChunks) * 64 * 128 + 1024;
-        static SmemAttrCache attr;
-        if ((rc = attr.ensure(tc_wgrad_tma, smem, "impala/fc_wgrad"))) return rc;
-        const dim3 grid(splits, 256 / (64 * kFcWgradXChunks), 2048 / (64 * kFcWgradYChunks));
-        tc_wgrad_tma<<<grid, kWgradTmaThreads, smem, s>>>(tmX, tmY, n, rpc, wsbig);
+        const int splits = launch_wgrad_tma(T(Q.dhid), 256, T(Q.h0), 2048, n, wsbig, s, "impala/fc_wgrad");
+        if (splits < 0) return splits;
         tc_fold_fc<<<2048, 256, 0, s>>>(wsbig, splits, 256, 2048, 256, 2048, 32, 64, 1.f, grads + L.fcw);
-        const int64_t rpb = colsum_rows(n);
-        const int nb = (int)ceil_div(n, rpb);
-        tc_colsum_partial<<<nb, 256, 0, s>>>(T(Q.dhid), n, 256, 256, rpb, wssmall);
-        tc_colsum_final<<<256 / 32, 256, 0, s>>>(wssmall, nb, 256, grads + L.fcb);
-        if ((rc = check_launch("impala/fc_wgrad", 4))) return rc;
+        if ((rc = check_launch("impala/fc_fold"))) return rc;
+        if ((rc = colsum(T(Q.dhid), n, 256, 256, wssmall, grads + L.fcb, s))) return rc;
     }
     {
         KGemmParams g;

@@ -32,6 +32,7 @@
 //       over hidden; backward = a bf16 copy of dhead feeding tc_wgrad_tma (dWh, folded over row splits in order) and
 //       tc_gemm_tma (dhid, ReLU-masked, into the slot the fc kernels read); dbh = fp32 column sums of dhead.
 #include <cuda.h>            // CUtensorMap types only; the encoder is resolved at run time (no libcuda link)
+#include <algorithm>
 #include "tc_base.cuh"
 #include "tc_conv_win.cuh"
 #include "tc_conv1_u8.cuh"
@@ -172,20 +173,18 @@ static void win_conv3(WinParams& p, const bf16* act2, int64_t n) {              
 }
 static void wgw_defaults(WGradWinParams& w) { memset(&w, 0, sizeof(w)); }
 
-static int64_t round_up(int64_t a, int64_t b) { return ceil_div(a, b) * b; }
-
-struct WPlan { int64_t rows_per_cta; int splits; };
-static WPlan wgrad_plan(int64_t M, int target_ctas, int quantum = 32) {
-    WPlan w;
-    w.rows_per_cta = round_up(ceil_div(M, target_ctas), quantum);
-    if (w.rows_per_cta < quantum) w.rows_per_cta = quantum;
-    w.splits = (int)ceil_div(M, w.rows_per_cta);
-    if (w.splits < 1) w.splits = 1;
-    return w;
+// row splits of the window weight gradients: one or two waves of CTAs on the 132 SMs of an H100
+static const int kC1Ctas = 264, kC2Ctas = 132, kC3Ctas = 132;
+static WPlan conv1_wgrad_plan(int64_t n, bool u8) {          // the uint8 kernel takes whole images (512 rows) per CTA
+    return u8 ? wgrad_plan(n * 512, kC2Ctas, 512) : wgrad_plan(n * 512, kC1Ctas, 128);
 }
-// row splits of the weight gradients: one or two waves of CTAs on the 132 SMs of an H100
-static const int kC1Ctas = 264, kC2Ctas = 132, kC3Ctas = 132, kFcSplits = 8;
+static WPlan conv2_wgrad_plan(int64_t n) { return wgrad_plan(n * 100, kC2Ctas, 128); }
+static WPlan conv3_wgrad_plan(int64_t n) { return wgrad_plan(n * 81, kC3Ctas, 128); }
 
+// scratch of launch_wgrad_win (and of the uint8 conv1 weight gradient, nslots = 4): dW partials ws[splits][nslots*64][64]
+// in the big region, bias partials wsb[splits][64] in the small one
+static size_t wgrad_win_bytes(int splits, int nslots) { return (size_t)splits * nslots * 64 * 64 * sizeof(float); }
+static size_t wgrad_win_bias_bytes(int splits) { return (size_t)splits * 64 * sizeof(float); }
 static int launch_wgrad_win(const WGradWinParams& p, int ctas, cudaStream_t s, const char* what) {
     const size_t smem = (size_t)kWgradWinStages * ((size_t)p.WRX * 128 * p.cpr + 128 * 128) + 4096 + 1024;
     static SmemAttrCache attr;
@@ -214,20 +213,6 @@ static int launch_wgrad_win(const WGradWinParams& p, int ctas, cudaStream_t s, c
     return check_launch(what);
 }
 
-static int colsum(const bf16* Y, int64_t M, int ld, int ncols, float* part, float* db, cudaStream_t s) {
-    int64_t rpb = ceil_div(M, 132 * 3);
-    if (rpb < 64) rpb = 64;
-    const int nb = (int)ceil_div(M, rpb);
-    tc_colsum_partial<<<nb, 256, 0, s>>>(Y, M, ld, ncols, rpb, part);
-    tc_colsum_final<<<(unsigned)ceil_div(ncols, 32), 256, 0, s>>>(part, nb, ncols, db);
-    return check_launch("colsum", 2);
-}
-static size_t colsum_ws(int64_t M, int ncols) {
-    int64_t rpb = ceil_div(M, 132 * 3);
-    if (rpb < 64) rpb = 64;
-    return (size_t)ceil_div(M, rpb) * ncols * sizeof(float);
-}
-
 }  // namespace b200rl
 
 using namespace b200rl;
@@ -235,13 +220,11 @@ using namespace b200rl;
 namespace b200rl {
 // head widths the bf16 NatureCNN accepts: narrow (CUDA-core heads) or wide (wgmma heads)
 static bool head_ok(int A) { return A >= 1 && A < kMaxWideHeads; }
-// wide-head backward scratch: weight-gradient partials (big part) and dhead bf16 + bias-sum partials (small part)
-static size_t wide_big_bytes(int64_t n, const NatureLayout& L) {
-    return (size_t)wgrad_plan(n, kFcSplits, 64).splits * L.G * 512 * 4;
-}
+// wide-head backward scratch over A1 outputs: dWh partials wgrad_tma_bytes(n, G, 512) (big part) and dhead bf16 +
+// bias-sum partials (small part)
 static size_t wide_dhead_bytes(int64_t n, const NatureLayout& L) { return ((size_t)n * L.G * 2 + 255) & ~(size_t)255; }
-static size_t wide_small_bytes(int64_t n, const NatureLayout& L) {
-    return wide_dhead_bytes(n, L) + (size_t)ceil_div(n, wide_colsum_rows(n)) * (L.A + 1) * 4;
+static size_t wide_small_bytes(int64_t n, const NatureLayout& L, int A1) {
+    return wide_dhead_bytes(n, L) + colsum_f32_ws(n, A1);
 }
 
 // ---- the parts of the NatureCNN plan that the recurrent agent shares (same kernels, same launches)
@@ -283,20 +266,12 @@ static int trunk_bwd(const NatureLayout& L, const NatureActs& Q, const bf16* P, 
     KGemmParams p;
     // ---- fc: dW[o][c*49+p] = sum_m dhid[m][o] * act3[m][p*64+c]
     {
-        const WPlan pl = wgrad_plan(n, kFcSplits, 64);
+        int splits;
+        // X = dhid (512 columns), Y = act3 (3136 columns, the last Y group partly past the end: zero-filled by TMA)
         { ProfScope ps(s, "fc_wgrad", 2.0 * n * 512 * 3136, (double)n * (3136 + 512) * 2 + 512.0 * 3136 * 4);
-          CUtensorMap tmX, tmY;
-          if ((rc = make_tmap_2d(&tmX, act + Q.dhid, n, 512, 64, "naturecnn/fc_wgrad"))) return rc;
-          if ((rc = make_tmap_2d(&tmY, act + Q.act3, n, 3136, 64, "naturecnn/fc_wgrad"))) return rc;
-          const size_t smem = (size_t)4 * (kFcWgradXChunks + kFcWgradYChunks) * 64 * 128 + 1024;
-          static SmemAttrCache attr;
-          if ((rc = attr.ensure(tc_wgrad_tma, smem, "naturecnn/fc_wgrad"))) return rc;
-          // X = dhid (512 columns), Y = act3 (3136 columns, the last Y group partly past the end: zero-filled by TMA)
-          const dim3 grid(pl.splits, 512 / (64 * kFcWgradXChunks), (unsigned)ceil_div(3136, 64 * kFcWgradYChunks));
-          tc_wgrad_tma<<<grid, kWgradTmaThreads, smem, s>>>(tmX, tmY, n, pl.rows_per_cta, wsbig);
-          if ((rc = check_launch("naturecnn/fc_wgrad"))) return rc; }
+          if ((splits = launch_wgrad_tma(act + Q.dhid, 512, act + Q.act3, 3136, n, wsbig, s, "naturecnn/fc_wgrad")) < 0) return splits; }
         { ProfScope ps(s, "wgrad_fold_bias", 0, 0);
-          note_launches(1); tc_fold_fc<<<(unsigned)ceil_div((int64_t)512 * 3136, 256), 256, 0, s>>>(wsbig, pl.splits, 512, 13 * 256, 512, 3136, 64, 49, 1.f, grads + L.fcw);
+          note_launches(1); tc_fold_fc<<<(unsigned)ceil_div((int64_t)512 * 3136, 256), 256, 0, s>>>(wsbig, splits, 512, 13 * 256, 512, 3136, 64, 49, 1.f, grads + L.fcw);
           if ((rc = colsum(act + Q.dhid, n, 512, 512, wssmall, grads + L.fcb, s))) return rc; }
         // grads[fcw .. total) (fc weight + bias, both heads) are final: the caller may start exchanging them now
         if (tail_ready_event) {
@@ -321,7 +296,7 @@ static int trunk_bwd(const NatureLayout& L, const NatureActs& Q, const bf16* P, 
         const int st[10] = {0, 1, 2, 3, 4, 5, 6, 7, 7, 8};      // slot 8 duplicates tap 7 so that tap 8 has a partner
         for (int k = 0; k < 10; ++k) { gw.slot_tap[k] = st[k]; gw.slot_cc[k] = 0; }
         gw.Y = act + Q.dact3a; gw.ldy = 64; gw.ncolsY = 64;
-        const WPlan pl = wgrad_plan(n * 81, kC3Ctas, 128);
+        const WPlan pl = conv3_wgrad_plan(n);
         gw.rows_per_cta = pl.rows_per_cta; gw.ws = wsbig; gw.wsb = wssmall;
         { ProfScope ps(s, "conv3_wgrad", 2.0 * n * 49 * 64 * 576, (double)n * (5184 + 5184) * 2);
           if ((rc = launch_wgrad_win(gw, pl.splits, s, "naturecnn/conv3_wgrad"))) return rc; }
@@ -349,7 +324,7 @@ static int trunk_bwd(const NatureLayout& L, const NatureActs& Q, const bf16* P, 
         gw.shift[0] = 0; gw.shift[1] = 1; gw.shift[2] = 10; gw.shift[3] = 11;
         for (int k = 0; k < 8; ++k) { gw.slot_tap[k] = k >> 1; gw.slot_cc[k] = k & 1; }
         gw.Y = act + Q.dact2a; gw.ldy = 64; gw.ncolsY = 64;
-        const WPlan pl = wgrad_plan(n * 100, kC2Ctas, 128);
+        const WPlan pl = conv2_wgrad_plan(n);
         gw.rows_per_cta = pl.rows_per_cta; gw.ws = wsbig; gw.wsb = wssmall;
         { ProfScope ps(s, "conv2_wgrad", 2.0 * n * 81 * 64 * 512, (double)n * (12800 + 6400) * 2);
           if ((rc = launch_wgrad_win(gw, pl.splits, s, "naturecnn/conv2_wgrad"))) return rc; }
@@ -372,6 +347,16 @@ static int trunk_bwd(const NatureLayout& L, const NatureActs& Q, const bf16* P, 
     }
     return B200RL_OK;
 }
+// scratch of trunk_bwd: the fc, conv3 and conv2 weight-gradient partials (big part); the fc bias column sums and the
+// conv bias partials (small part)
+static size_t trunk_big_bytes(int64_t n) {
+    return std::max({wgrad_tma_bytes(n, 512, 3136), wgrad_win_bytes(conv3_wgrad_plan(n).splits, 10),
+                     wgrad_win_bytes(conv2_wgrad_plan(n).splits, 8)});
+}
+static size_t trunk_small_bytes(int64_t n) {
+    return std::max({colsum_ws(n, 512), wgrad_win_bias_bytes(conv3_wgrad_plan(n).splits),
+                     wgrad_win_bias_bytes(conv2_wgrad_plan(n).splits)});
+}
 
 // wide head forward: out [n, A1] (fp32, row stride A1) = hid . Wh^T + bh over the zero-padded [G, 512] operands
 static int wide_head_fwd(const NatureLayout& L, const bf16* P, const bf16* hid, int64_t n, int A1, float* out, cudaStream_t s) {
@@ -392,22 +377,12 @@ static int wide_head_bwd(const NatureLayout& L, const bf16* P, const float* dhea
     float* dbpart = reinterpret_cast<float*>(reinterpret_cast<char*>(wssmall) + wide_dhead_bytes(n, L));
     int cb = (int)ceil_div(n * L.G, 256); if (cb > num_sms() * 8) cb = num_sms() * 8;
     tc_head_dhead_bf16<<<cb, 256, 0, s>>>(dhead, n, A1, L.G, dh16);
-    const int64_t rpb = wide_colsum_rows(n);
-    const int nb = (int)ceil_div(n, rpb);
-    tc_colsum_f32_partial<<<dim3(nb, (unsigned)ceil_div(A1, 128)), 128, 0, s>>>(dhead, n, A1, rpb, dbpart);
-    tc_colsum_f32_final<<<(unsigned)ceil_div(A1, 128), 128, 0, s>>>(dbpart, nb, A1, db);
-    if ((rc = check_launch("wide_heads_bias", 3))) return rc;
-    const WPlan pl = wgrad_plan(n, kFcSplits, 64);
-    CUtensorMap tmX, tmY;
-    if ((rc = make_tmap_2d(&tmX, dh16, n, L.G, 64, "wide_heads_wgrad"))) return rc;
-    if ((rc = make_tmap_2d(&tmY, hid, n, 512, 64, "wide_heads_wgrad"))) return rc;
-    const size_t smem = (size_t)4 * (kFcWgradXChunks + kFcWgradYChunks) * 64 * 128 + 1024;
-    static SmemAttrCache attr;
-    if ((rc = attr.ensure(tc_wgrad_tma, smem, "wide_heads_wgrad"))) return rc;
-    const dim3 grid(pl.splits, L.G / (64 * kFcWgradXChunks), 512 / (64 * kFcWgradYChunks));
-    tc_wgrad_tma<<<grid, kWgradTmaThreads, smem, s>>>(tmX, tmY, n, pl.rows_per_cta, wsbig);
-    tc_fold_head_wide<<<(unsigned)ceil_div((int64_t)A1 * 512, 256), 256, 0, s>>>(wsbig, pl.splits, A1, L.G, dW);
-    if ((rc = check_launch("wide_heads_wgrad", 2))) return rc;
+    if ((rc = check_launch("wide_heads_dhead"))) return rc;
+    if ((rc = colsum_f32(dhead, n, A1, dbpart, db, s))) return rc;
+    const int splits = launch_wgrad_tma(dh16, L.G, hid, 512, n, wsbig, s, "wide_heads_wgrad");
+    if (splits < 0) return splits;
+    tc_fold_fc<<<(unsigned)ceil_div((int64_t)A1 * 512, 256), 256, 0, s>>>(wsbig, splits, L.G, 512, A1, 512, 512, 1, 1.f, dW);
+    if ((rc = check_launch("wide_heads_wgrad"))) return rc;
     gemm_rowmajor(p, dh16, n, L.G / 64);
     p.Bw = P + L.whdg; p.N = 512; p.out = dhid; p.ldo = 512;
     p.mask_bits = hid_bits;
@@ -447,28 +422,20 @@ extern "C" int b200rl_frames_to_s2d_u8(const uint8_t* obs, const int64_t* rows, 
     return check_launch("frames_to_s2d_u8");
 }
 
-// the first part of the backward workspace: weight-gradient partials (the small partials follow it, 256-B aligned)
+// the backward workspace = [big part: weight-gradient partials | small part, 256-B aligned], each the largest its launches
+// need: heads, trunk, and conv1 on either kind of input (bf16 window kernel or uint8 kernel)
 static size_t naturecnn_big_bytes(int64_t n, const NatureLayout& L) {
-    size_t a = 0;
-    auto mx = [&](size_t v) { if (v > a) a = v; };
-    mx((size_t)wgrad_plan(n * 512, kC1Ctas, 128).splits * 256 * 64 * 4);
-    mx((size_t)wgrad_plan(n * 100, kC2Ctas, 128).splits * 512 * 64 * 4);
-    mx((size_t)wgrad_plan(n * 81, kC3Ctas, 128).splits * 640 * 64 * 4);
-    mx((size_t)wgrad_plan(n, kFcSplits, 64).splits * 512 * (13 * 256) * 4);
-    if (L.wide) mx(wide_big_bytes(n, L));
-    return a;
+    return std::max({trunk_big_bytes(n), L.wide ? wgrad_tma_bytes(n, L.G, 512) : 0,
+                     wgrad_win_bytes(conv1_wgrad_plan(n, false).splits, 4), wgrad_win_bytes(conv1_wgrad_plan(n, true).splits, 4)});
 }
 
 extern "C" size_t b200rl_naturecnn_bf16_workspace_bytes(int64_t n, int A) {
     if (n < 1 || !head_ok(A)) return 0;
     const NatureLayout L(A);
-    const size_t a = naturecnn_big_bytes(n, L);
-    size_t b = 0;
-    auto mb = [&](size_t v) { if (v > b) b = v; };
-    mb(colsum_ws(n * 441, 32)); mb(colsum_ws(n * 100, 64)); mb(colsum_ws(n * 81, 64)); mb(colsum_ws(n, 512));
-    if (L.wide) mb(wide_small_bytes(n, L));
-    else mb((size_t)2 * ceil_div(n, heads_rows_per_block(n)) * (A + 1) * 514 * 4);
-    return a + b + 512;
+    const size_t small = std::max({trunk_small_bytes(n), L.wide ? wide_small_bytes(n, L, A + 1) : heads_partial_bytes(n, A + 1, 512),
+                                   wgrad_win_bias_bytes(conv1_wgrad_plan(n, false).splits),
+                                   wgrad_win_bias_bytes(conv1_wgrad_plan(n, true).splits)});
+    return naturecnn_big_bytes(n, L) + small + 512;
 }
 
 extern "C" int b200rl_naturecnn_bf16_pack(const float* params, int A, void* packed, void* stream) {
@@ -540,10 +507,8 @@ extern "C" int b200rl_naturecnn_bf16_forward(const void* obs, int obs_format, co
         return wide_head_fwd(L, P, act + Q.hid, n, A + 1, head_out, s);
     }
     // heads (fp32 math on CUDA cores): head_out [n, A+1] = [logits | value]
-    { ProfScope ps(s, "heads_fwd", 2.0 * n * 512 * (A + 1), (double)n * (1024 + 4 * (A + 1)));
-      int hb = (int)ceil_div(n, 8); if (hb > num_sms() * 8) hb = num_sms() * 8;
-      tc_heads_fwd<<<hb, 256, (size_t)(A + 1) * 2048, s>>>(act + Q.hid, params + L.hw, params + L.hb, n, A + 1, 512, head_out); }
-    return check_launch("naturecnn/heads");
+    ProfScope ps(s, "heads_fwd", 2.0 * n * 512 * (A + 1), (double)n * (1024 + 4 * (A + 1)));
+    return heads_fwd<512>(act + Q.hid, params + L.hw, params + L.hb, n, A + 1, head_out, s, "naturecnn/heads");
 }
 
 extern "C" int b200rl_naturecnn_bf16_backward(const void* obs, const void* obs_aux, int obs_format, const int64_t* rows, int64_t n, int A,
@@ -582,56 +547,46 @@ extern "C" int b200rl_naturecnn_bf16_backward(const void* obs, const void* obs_a
     } else
     // ---- heads: dW, db, then dhid_pre = (dhead . Wh) * (hid > 0)
     {
-        const int64_t rpb = heads_rows_per_block(n);
-        const int nb = (int)ceil_div(n, rpb);
         ProfScope ps(s, "heads_bwd", 4.0 * n * 512 * A1, (double)n * (2048 + 64 + 8 * A1));
-        const size_t sd = (size_t)rpb * A1 * sizeof(float);
-        if (A1 <= 8) tc_heads_bwd_weight<8><<<nb, 512, sd, s>>>(dhead, act + Q.hid, n, A1, 512, rpb, wssmall);
-        else tc_heads_bwd_weight<kMaxHeads><<<nb, 512, sd, s>>>(dhead, act + Q.hid, n, A1, 512, rpb, wssmall);
-        tc_heads_fold<<<(unsigned)ceil_div(A1 * 514, 32), 256, 0, s>>>(wssmall, 2 * nb, A1, 512, grads + L.hw, grads + L.hb);
-        int db_blocks = (int)ceil_div(n * 64, 256); if (db_blocks > num_sms() * 8) db_blocks = num_sms() * 8;
-        tc_heads_bwd_data<<<db_blocks, 256, (size_t)A1 * 2048, s>>>(dhead, params + L.hw, reinterpret_cast<const uint8_t*>(act + Q.m4), n, A1, 512, act + Q.dhid);
-        if ((rc = check_launch("naturecnn/heads_bwd", 3))) return rc;
+        if ((rc = heads_bwd_weight<512>(dhead, act + Q.hid, n, A1, wssmall, grads + L.hw, grads + L.hb, s, "naturecnn/heads_bwd"))) return rc;
+        if ((rc = heads_bwd_data<512>(dhead, params + L.hw, reinterpret_cast<const uint8_t*>(act + Q.m4), n, A1, act + Q.dhid, s,
+                                      "naturecnn/heads_bwd"))) return rc;
     }
     if ((rc = trunk_bwd(L, Q, P, act, grads, n, wsbig, wssmall, tail_ready_event, obs_format == B200RL_OBS_S2D_U8, s))) return rc;
-    WGradWinParams gw;
-    FoldWin fw;
     // ---- conv1 (no data gradient: the input is the observation)
-    if (obs_format == B200RL_OBS_S2D_U8) {
+    const bool u8 = obs_format == B200RL_OBS_S2D_U8;
+    const WPlan pl = conv1_wgrad_plan(n, u8);
+    if (u8) {
         // uint8 channel-major frames -> fp16 wgmma operands in registers (tc_conv1_u8.cuh); 1 CTA per SM
         Conv1WgradU8Params cw;
         memset(&cw, 0, sizeof(cw));
-        const WPlan pl = wgrad_plan(n * 512, kC2Ctas, 512);          // whole images per CTA
         cw.rows = rows; cw.n = (int)n; cw.rows_per_cta = pl.rows_per_cta; cw.ws = wsbig; cw.wsb = wssmall;
         { ProfScope ps(s, "conv1_wgrad", 2.0 * n * 400 * 32 * 256, (double)n * (28672 + 14112 * 2));
           if ((rc = launch_conv1_wgrad_u8(cw, obs_aux, rows ? (int64_t)1 << 24 : n, act + Q.dact1, pl.splits, s, "naturecnn/conv1_wgrad_u8"))) return rc; }
-        memset(&fw, 0, sizeof(fw));
-        fw.layer = 1; fw.S = pl.splits; fw.nslots = 4; fw.Cout = 32; fw.scale = 1.0f / 255.0f / kDact1Scale; fw.bscale = 1.0f / kDact1Scale;
-        const int st1[4] = {0, 1, 2, 3};               // ws rows: tile b, lane m -> tap 2 b + (m >> 6)
-        for (int k = 0; k < 4; ++k) fw.slot_tap[k] = st1[k];
-        { ProfScope ps(s, "wgrad_fold_bias", 0, 0);
-          fw.wsb = wssmall; fw.db = grads + L.c1b;
-          tc_fold_win<<<(unsigned)ceil_div(256 * 32 + 32, 32), 256, 0, s>>>(wsbig, fw, grads + L.c1w);
-          if ((rc = check_launch("naturecnn/conv1_fold"))) return rc; }
     } else {
+        WGradWinParams gw;
         wgw_defaults(gw);
         gw.X = x0; gw.rows = x0rows; gw.M = n * 512; gw.n = (int)n; gw.G = 441; gw.cpr = 1; gw.nslots = 4; gw.WRX = round8(128 + 22);
         gw.tpi_shift = 2; gw.n_images = x0rows ? (int64_t)1 << 24 : n;       // 4 steps of 128 grid rows per image
         gw.shift[0] = 0; gw.shift[1] = 1; gw.shift[2] = 21; gw.shift[3] = 22;
         for (int k = 0; k < 4; ++k) { gw.slot_tap[k] = k; gw.slot_cc[k] = 0; }
         gw.Y = act + Q.dact1; gw.ldy = 32; gw.ncolsY = 32;
-        const WPlan pl = wgrad_plan(n * 512, kC1Ctas, 128);
         gw.rows_per_cta = pl.rows_per_cta; gw.ws = wsbig; gw.wsb = wssmall;
         { ProfScope ps(s, "conv1_wgrad", 2.0 * n * 400 * 32 * 256, (double)n * (28224 + 14112) * 2);
           if ((rc = launch_wgrad_win(gw, pl.splits, s, "naturecnn/conv1_wgrad"))) return rc; }
-        memset(&fw, 0, sizeof(fw));
-        fw.layer = 1; fw.S = pl.splits; fw.nslots = 4; fw.Cout = 32; fw.scale = 1.0f / 255.0f; fw.bscale = 1.f;
-        for (int k = 0; k < 4; ++k) fw.slot_tap[k] = k;
-        { ProfScope ps(s, "wgrad_fold_bias", 0, 0);
-          fw.wsb = wssmall; fw.db = grads + L.c1b;
-          tc_fold_win<<<(unsigned)ceil_div(256 * 32 + 32, 32), 256, 0, s>>>(wsbig, fw, grads + L.c1w);
-          if ((rc = check_launch("naturecnn/conv1_fold"))) return rc; }
     }
+    // both kernels leave ws rows in tap order (uint8: tile b, lane m -> tap 2 b + (m >> 6)); the uint8 one scaled dY by
+    // kDact1Scale
+    FoldWin fw;
+    memset(&fw, 0, sizeof(fw));
+    fw.layer = 1; fw.S = pl.splits; fw.nslots = 4; fw.Cout = 32;
+    fw.scale = u8 ? 1.0f / 255.0f / kDact1Scale : 1.0f / 255.0f;
+    fw.bscale = u8 ? 1.0f / kDact1Scale : 1.f;
+    for (int k = 0; k < 4; ++k) fw.slot_tap[k] = k;
+    { ProfScope ps(s, "wgrad_fold_bias", 0, 0);
+      fw.wsb = wssmall; fw.db = grads + L.c1b;
+      tc_fold_win<<<(unsigned)ceil_div(256 * 32 + 32, 32), 256, 0, s>>>(wsbig, fw, grads + L.c1w);
+      if ((rc = check_launch("naturecnn/conv1_fold"))) return rc; }
     return B200RL_OK;
 }
 
@@ -669,25 +624,16 @@ static C1Plan lstm_conv1_plan(int64_t M) {           // whole frames per CTA, on
     c.ctas = (int)ceil_div(M, c.per_cta);
     return c;
 }
+// backward workspace = [big part (256-B aligned) | small part], each the largest its launches need: heads, W_ih as a wide
+// head, W_hh, trunk, conv1
 static size_t lstm_big_bytes(int64_t M, const NatureLayout& L) {
-    size_t a = 0;
-    auto mx = [&](size_t v) { if (v > a) a = v; };
-    mx((size_t)wgrad_plan(M * 100, kC2Ctas, 128).splits * 512 * 64 * 4);
-    mx((size_t)wgrad_plan(M * 81, kC3Ctas, 128).splits * 640 * 64 * 4);
-    mx((size_t)wgrad_plan(M, kFcSplits, 64).splits * 512 * (13 * 256) * 4);
-    mx(wide_big_bytes(M, L));                                              // dW_ih partials (dW_hh's are half as wide)
-    mx((size_t)lstm_conv1_plan(M).ctas * 32 * 64 * 4);
+    const size_t a = std::max({wgrad_tma_bytes(M, L.G, 512), wgrad_tma_bytes(M, 512, 128), trunk_big_bytes(M),
+                               (size_t)lstm_conv1_plan(M).ctas * 32 * 64 * 4});
     return (a + 255) & ~(size_t)255;
 }
-static size_t lstm_small_bytes(int64_t M, int A) {
-    const NatureLayout L(A, NatureLayout::Lstm{});
-    size_t b = 0;
-    auto mb = [&](size_t v) { if (v > b) b = v; };
-    mb(colsum_ws(M * 100, 64)); mb(colsum_ws(M * 81, 64)); mb(colsum_ws(M, 512));
-    mb(wide_dhead_bytes(M, L) + (size_t)ceil_div(M, wide_colsum_rows(M)) * 512 * 4);
-    mb((size_t)2 * ceil_div(M, heads_rows_per_block(M)) * (A + 1) * 130 * 4);
-    mb((size_t)lstm_conv1_plan(M).ctas * 32 * 4);
-    return b;
+static size_t lstm_small_bytes(int64_t M, const NatureLayout& L) {
+    return std::max({heads_partial_bytes(M, L.A + 1, 128), wide_small_bytes(M, L, 512), trunk_small_bytes(M),
+                     (size_t)lstm_conv1_plan(M).ctas * 32 * 4});
 }
 }  // namespace b200rl
 
@@ -710,7 +656,7 @@ extern "C" int b200rl_lstm_agent_bf16_acts_layout(int64_t S, int64_t n, int64_t*
 extern "C" size_t b200rl_lstm_agent_bf16_workspace_bytes(int64_t S, int64_t n, int A) {
     if (!lstm_sizes_ok(S, n) || !lstm_heads_ok(A)) return 0;
     const NatureLayout L(A, NatureLayout::Lstm{});
-    return lstm_big_bytes(S * n, L) + lstm_small_bytes(S * n, A) + 512;
+    return lstm_big_bytes(S * n, L) + lstm_small_bytes(S * n, L) + 512;
 }
 
 extern "C" int b200rl_lstm_agent_bf16_pack(const float* params, int A, void* packed, void* stream) {
@@ -776,12 +722,8 @@ extern "C" int b200rl_lstm_agent_bf16_forward(const uint8_t* obs, const int64_t*
         lstm::lstm_rec_fwd<<<(unsigned)ceil_div(n, lstm::kRows), lstm::kThreads, lstm::rec_fwd_smem(), s>>>(rp);
         if ((rc = check_launch("lstm/recurrence"))) return rc;
     }
-    { ProfScope ps(s, "heads_fwd", 2.0 * M * 128 * (A + 1), (double)M * (256 + 4 * (A + 1)));
-      const int hb = (int)(ceil_div(M, 8) < (int64_t)num_sms() * 8 ? ceil_div(M, 8) : (int64_t)num_sms() * 8);
-      tc_heads_fwd<128><<<hb, 256, (size_t)(A + 1) * 128 * 4, s>>>(reinterpret_cast<const bf16*>(ab + Q.hseq), params + L.hw,
-                                                                   params + L.hb, M, A + 1, 128, head_out);
-      if ((rc = check_launch("lstm/heads"))) return rc; }
-    return B200RL_OK;
+    ProfScope ps(s, "heads_fwd", 2.0 * M * 128 * (A + 1), (double)M * (256 + 4 * (A + 1)));
+    return heads_fwd<128>(reinterpret_cast<const bf16*>(ab + Q.hseq), params + L.hw, params + L.hb, M, A + 1, head_out, s, "lstm/heads");
 }
 
 extern "C" int b200rl_lstm_agent_bf16_backward(const uint8_t* obs, const int64_t* rows, int64_t S, int64_t n, int A,
@@ -811,14 +753,8 @@ extern "C" int b200rl_lstm_agent_bf16_backward(const uint8_t* obs, const int64_t
     float* dgates = reinterpret_cast<float*>(ab + Q.dgates);
     int rc;
     {   // heads weight gradient (the data gradient is folded into the recurrence backward)
-        const int64_t rpb = heads_rows_per_block(M);
-        const int nb = (int)ceil_div(M, rpb);
         ProfScope ps(s, "heads_bwd", 2.0 * M * 128 * A1, (double)M * (256 + 4 * A1));
-        const size_t sd = (size_t)rpb * A1 * sizeof(float);
-        if (A1 <= 8) tc_heads_bwd_weight<8, 128><<<nb, 128, sd, s>>>(dhead, hseq, M, A1, 128, rpb, wssmall);
-        else tc_heads_bwd_weight<kMaxHeads, 128><<<nb, 128, sd, s>>>(dhead, hseq, M, A1, 128, rpb, wssmall);
-        tc_heads_fold<<<(unsigned)ceil_div(A1 * 130, 32), 256, 0, s>>>(wssmall, 2 * nb, A1, 128, grads + L.hw, grads + L.hb);
-        if ((rc = check_launch("lstm/heads_bwd", 2))) return rc;
+        if ((rc = heads_bwd_weight<128>(dhead, hseq, M, A1, wssmall, grads + L.hw, grads + L.hb, s, "lstm/heads_bwd"))) return rc;
     }
     {
         lstm::RecBwdP bp;
@@ -838,19 +774,12 @@ extern "C" int b200rl_lstm_agent_bf16_backward(const uint8_t* obs, const int64_t
     }
     {   // dW_hh = dgates^T . h' over all S*n rows (row splits folded in order); db_hh = db_ih
         ProfScope ps(s, "lstm_hh_wgrad", 2.0 * M * 512 * 128, (double)M * (1024 + 256) + 512.0 * 128 * 4);
-        const WPlan pl = wgrad_plan(M, kFcSplits, 64);
-        CUtensorMap tmX, tmY;
-        if ((rc = make_tmap_2d(&tmX, wssmall, M, 512, 64, "lstm/hh_wgrad"))) return rc;
-        if ((rc = make_tmap_2d(&tmY, ab + Q.hm, M, 128, 64, "lstm/hh_wgrad"))) return rc;
-        const size_t smem = (size_t)4 * (kFcWgradXChunks + kFcWgradYChunks) * 64 * 128 + 1024;
-        static SmemAttrCache attr;
-        if ((rc = attr.ensure(tc_wgrad_tma, smem, "lstm/hh_wgrad"))) return rc;
         // X = dgates (512 columns), Y = h' (128 columns: the rest of the 256-column Y group is zero-filled by TMA)
-        const dim3 grid(pl.splits, 512 / (64 * kFcWgradXChunks), 1);
-        tc_wgrad_tma<<<grid, kWgradTmaThreads, smem, s>>>(tmX, tmY, M, pl.rows_per_cta, wsbig);
-        tc_fold_fc<<<(unsigned)ceil_div((int64_t)512 * 128, 256), 256, 0, s>>>(wsbig, pl.splits, 512, 64 * kFcWgradYChunks, 512, 128,
+        const int splits = launch_wgrad_tma(wssmall, 512, ab + Q.hm, 128, M, wsbig, s, "lstm/hh_wgrad");
+        if (splits < 0) return splits;
+        tc_fold_fc<<<(unsigned)ceil_div((int64_t)512 * 128, 256), 256, 0, s>>>(wsbig, splits, 512, 64 * kFcWgradYChunks, 512, 128,
                                                                             128, 1, 1.f, grads + L.whh);
-        if ((rc = check_launch("lstm/hh_wgrad", 2))) return rc;
+        if ((rc = check_launch("lstm/hh_wgrad"))) return rc;
         const cudaError_t e = cudaMemcpyAsync(grads + L.bhh, grads + L.bih, 512 * sizeof(float), cudaMemcpyDeviceToDevice, s);
         if (e != cudaSuccess) return fail(B200RL_ERR_CUDA, "lstm_backward: bias copy: %s", cudaGetErrorString(e));
     }

@@ -275,4 +275,40 @@ static int launch_gemm_tma(const KGemmParams& p, cudaStream_t s, const char* wha
     return check_launch(what);
 }
 
+// ---- row splits of the weight gradients: every CTA owns rows_per_cta rows (a multiple of `quantum`)
+static int64_t round_up(int64_t a, int64_t b) { return ceil_div(a, b) * b; }
+struct WPlan { int64_t rows_per_cta; int splits; };
+static WPlan wgrad_plan(int64_t M, int target_ctas, int quantum = 32) {
+    WPlan w;
+    w.rows_per_cta = round_up(ceil_div(M, target_ctas), quantum);
+    if (w.rows_per_cta < quantum) w.rows_per_cta = quantum;
+    w.splits = (int)ceil_div(M, w.rows_per_cta);
+    if (w.splits < 1) w.splits = 1;
+    return w;
+}
+constexpr int kFcSplits = 8;                 // row splits of tc_wgrad_tma
+
+// partials ws[splits][xcols][ycols rounded up to 256] (fp32) written by launch_wgrad_tma
+static size_t wgrad_tma_bytes(int64_t M, int xcols, int ycols) {
+    return (size_t)wgrad_plan(M, kFcSplits, 64).splits * xcols * round_up(ycols, 64 * kFcWgradYChunks) * sizeof(float);
+}
+// ws[split] = X[rows of the split]^T . Y[rows of the split] for row-major bf16 X [M, xcols] and Y [M, ycols] (Y columns
+// past ycols are zero-filled by TMA); returns the number of row splits (fold them with tc_fold_fc), or an error (< 0)
+static int launch_wgrad_tma(const void* X, int xcols, const void* Y, int ycols, int64_t M, float* ws, cudaStream_t s,
+                            const char* what) {
+    if (xcols % (64 * kFcWgradXChunks) != 0) return fail(B200RL_ERR_INVALID_ARGUMENT, "%s: X columns must be a multiple of 128", what);
+    const WPlan pl = wgrad_plan(M, kFcSplits, 64);
+    CUtensorMap tmX, tmY;
+    int rc;
+    if ((rc = make_tmap_2d(&tmX, X, M, xcols, 64, what))) return rc;
+    if ((rc = make_tmap_2d(&tmY, Y, M, ycols, 64, what))) return rc;
+    const size_t smem = (size_t)4 * (kFcWgradXChunks + kFcWgradYChunks) * 64 * 128 + 1024;
+    static SmemAttrCache attr;
+    if ((rc = attr.ensure(tc_wgrad_tma, smem, what))) return rc;
+    const dim3 grid(pl.splits, xcols / (64 * kFcWgradXChunks), (unsigned)ceil_div(ycols, 64 * kFcWgradYChunks));
+    tc_wgrad_tma<<<grid, kWgradTmaThreads, smem, s>>>(tmX, tmY, M, pl.rows_per_cta, ws);
+    if ((rc = check_launch(what))) return rc;
+    return pl.splits;
+}
+
 }  // namespace b200rl

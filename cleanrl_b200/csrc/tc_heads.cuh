@@ -167,4 +167,40 @@ static __global__ void __launch_bounds__(256) tc_heads_fold(const float* __restr
     if (h == H) db[a] = s; else dW[(int64_t)a * H + h] = s;
 }
 
+// ---- launchers over H hidden units (128: the LSTM agent, 256: IMPALA-CNN, 512: NatureCNN); Wh, bh, dW, db fp32 [A1][H]
+template <int H>
+static int heads_fwd(const bf16* hid, const float* Wh, const float* bh, int64_t n, int A1, float* out, cudaStream_t s,
+                     const char* what) {
+    static_assert(H == 128 || H == 256 || H == 512, "head input width");
+    const int grid = (int)(ceil_div(n, 8) < (int64_t)num_sms() * 8 ? ceil_div(n, 8) : (int64_t)num_sms() * 8);
+    tc_heads_fwd<H><<<grid, 256, (size_t)A1 * H * sizeof(float), s>>>(hid, Wh, bh, n, A1, H, out);
+    return check_launch(what);
+}
+// scratch of heads_bwd_weight: 2 partial slabs of A1 x (H + 2) floats per row block
+static size_t heads_partial_bytes(int64_t n, int A1, int H) {
+    return (size_t)2 * ceil_div(n, heads_rows_per_block(n)) * A1 * (H + 2) * sizeof(float);
+}
+// dW = dhead^T . hid, db = column sums of dhead, through the partial slabs `part` (heads_partial_bytes)
+template <int H>
+static int heads_bwd_weight(const float* dhead, const bf16* hid, int64_t n, int A1, float* part, float* dW, float* db,
+                            cudaStream_t s, const char* what) {
+    static_assert(H == 128 || H == 256 || H == 512, "head input width");
+    const int64_t rpb = heads_rows_per_block(n);
+    const int nb = (int)ceil_div(n, rpb);
+    const size_t sd = (size_t)rpb * A1 * sizeof(float);
+    if (A1 <= 8) tc_heads_bwd_weight<8, H><<<nb, H, sd, s>>>(dhead, hid, n, A1, H, rpb, part);
+    else tc_heads_bwd_weight<kMaxHeads, H><<<nb, H, sd, s>>>(dhead, hid, n, A1, H, rpb, part);
+    tc_heads_fold<<<(unsigned)ceil_div(A1 * (H + 2), 32), 256, 0, s>>>(part, 2 * nb, A1, H, dW, db);
+    return check_launch(what, 2);
+}
+// dhid = (dhead . Wh) * (hid > 0), hid_bits = one mask byte per 8 hidden units
+template <int H>
+static int heads_bwd_data(const float* dhead, const float* Wh, const uint8_t* hid_bits, int64_t n, int A1, bf16* dhid,
+                          cudaStream_t s, const char* what) {
+    static_assert(H == 128 || H == 256 || H == 512, "head input width");
+    const int grid = (int)(ceil_div(n * H, 2048) < (int64_t)num_sms() * 8 ? ceil_div(n * H, 2048) : (int64_t)num_sms() * 8);
+    tc_heads_bwd_data<H><<<grid, 256, (size_t)A1 * H * sizeof(float), s>>>(dhead, Wh, hid_bits, n, A1, H, dhid);
+    return check_launch(what);
+}
+
 }  // namespace b200rl

@@ -56,14 +56,13 @@ __global__ void __launch_bounds__(128) tc_colsum_f32_final(const float* __restri
     for (int b = 0; b < nb; ++b) s += part[(int64_t)b * cols + c];
     out[c] = s;
 }
-
-// dWh[a][h] = sum over row splits (in order) of ws[split][a][h], ws = tc_wgrad_tma output [S][G][512]
-__global__ void __launch_bounds__(256) tc_fold_head_wide(const float* __restrict__ ws, int S, int A1, int G, float* __restrict__ dW) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= (int64_t)A1 * 512) return;
-    float s = 0.f;
-    for (int k = 0; k < S; ++k) s += ws[(int64_t)k * G * 512 + i];
-    dW[i] = s;
+static int colsum_f32(const float* x, int64_t n, int cols, float* part, float* out, cudaStream_t s) {
+    const int64_t rpb = wide_colsum_rows(n);
+    const int nb = (int)ceil_div(n, rpb);
+    tc_colsum_f32_partial<<<dim3(nb, (unsigned)ceil_div(cols, 128)), 128, 0, s>>>(x, n, cols, rpb, part);
+    tc_colsum_f32_final<<<(unsigned)ceil_div(cols, 128), 128, 0, s>>>(part, nb, cols, out);
+    return check_launch("colsum_f32", 2);
 }
+static size_t colsum_f32_ws(int64_t n, int cols) { return (size_t)ceil_div(n, wide_colsum_rows(n)) * cols * sizeof(float); }
 
 }  // namespace b200rl

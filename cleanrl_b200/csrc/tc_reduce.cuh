@@ -129,4 +129,18 @@ static __global__ void __launch_bounds__(256) tc_colsum_final(const float* __res
     if (c < ncols && threadIdx.x < 32) db[c] = s;
 }
 
+// db = column sums of bf16 Y [M, ld] (first ncols columns), through per-block partials `part` (colsum_ws bytes)
+static int64_t colsum_rows(int64_t M) {
+    const int64_t rpb = ceil_div(M, 132 * 3);
+    return rpb < 64 ? 64 : rpb;
+}
+static int colsum(const bf16* Y, int64_t M, int ld, int ncols, float* part, float* db, cudaStream_t s) {
+    const int64_t rpb = colsum_rows(M);
+    const int nb = (int)ceil_div(M, rpb);
+    tc_colsum_partial<<<nb, 256, 0, s>>>(Y, M, ld, ncols, rpb, part);
+    tc_colsum_final<<<(unsigned)ceil_div(ncols, 32), 256, 0, s>>>(part, nb, ncols, db);
+    return check_launch("colsum", 2);
+}
+static size_t colsum_ws(int64_t M, int ncols) { return (size_t)ceil_div(M, colsum_rows(M)) * ncols * sizeof(float); }
+
 }  // namespace b200rl
