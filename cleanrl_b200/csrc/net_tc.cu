@@ -257,11 +257,11 @@ static int trunk_fwd(const NatureLayout& L, const NatureActs& Q, const float* pa
     return B200RL_OK;
 }
 
-// fc -> conv2 backward: dhid (ReLU-masked) -> fc, conv3, conv2 weight gradients and d(act1) on the 21x21 grid (fp16 x
-// kDact1Scale when `dact1_f16`, for the uint8 conv1 weight gradient; bf16 otherwise).  `tail_ready_event` is recorded
-// when grads[fcw ..) is final.
+// fc -> conv2 backward: dhid (ReLU-masked) -> fc, conv3, conv2 weight gradients and, unless `dact1_fused` (the uint8
+// rollout: tc_conv21_bwd_u8 computes it inside the conv1 weight gradient), d(act1) on the 21x21 grid in bf16.
+// `tail_ready_event` is recorded when grads[fcw ..) is final.
 static int trunk_bwd(const NatureLayout& L, const NatureActs& Q, const bf16* P, bf16* act, float* grads, int64_t n,
-                     float* wsbig, float* wssmall, void* tail_ready_event, bool dact1_f16, cudaStream_t s) {
+                     float* wsbig, float* wssmall, void* tail_ready_event, bool dact1_fused, cudaStream_t s) {
     int rc;
     KGemmParams p;
     // ---- fc: dW[o][c*49+p] = sum_m dhid[m][o] * act3[m][p*64+c]
@@ -335,13 +335,13 @@ static int trunk_bwd(const NatureLayout& L, const NatureActs& Q, const bf16* P, 
           fw.wsb = wssmall; fw.db = grads + L.c2b;
           tc_fold_win<<<(unsigned)ceil_div(512 * 64 + 64, 32), 256, 0, s>>>(wsbig, fw, grads + L.c2w);
           if ((rc = check_launch("naturecnn/conv2_fold"))) return rc; }
+        if (dact1_fused) return B200RL_OK;
         win_defaults(wp);
         wp.A = act + Q.dact2b; wp.n = (int)n; wp.G = 121; wp.Wp = 11; wp.M = n * 121; wp.ntaps = 4;
         for (int a = 0; a < 2; ++a) for (int b = 0; b < 2; ++b) wp.shift[a * 2 + b] = (1 - a) * 11 + (1 - b);
         wp.WR = round8(128 + 12);
         wp.Bw = P + L.w2dg; wp.N = 128; wp.vH = 10; wp.vW = 10; wp.out_mode = WOUT_DACT1;
         wp.out = act + Q.dact1; wp.mask_bits = reinterpret_cast<const uint32_t*>(act + Q.m1);
-        if (dact1_f16) { wp.out_f16 = 1; wp.scale = kDact1Scale; }     // fp16 x 2^12 for the uint8 conv1 wgrad
         { ProfScope ps(s, "conv2_dgrad", 2.0 * n * 400 * 32 * 256, (double)n * ((7744 + 14112) * 2 + 1600));
           if ((rc = launch_conv_win<128, 1, 4, 4>(wp, s, "naturecnn/conv2_dgrad"))) return rc; }
     }
@@ -557,12 +557,15 @@ extern "C" int b200rl_naturecnn_bf16_backward(const void* obs, const void* obs_a
     const bool u8 = obs_format == B200RL_OBS_S2D_U8;
     const WPlan pl = conv1_wgrad_plan(n, u8);
     if (u8) {
-        // uint8 channel-major frames -> fp16 wgmma operands in registers (tc_conv1_u8.cuh); 1 CTA per SM
-        Conv1WgradU8Params cw;
+        // conv2 data gradient (fp16 x kDact1Scale) + uint8 channel-major frames -> fp16 wgmma operands in registers
+        // (tc_conv1_u8.cuh); 1 CTA per SM
+        Conv21BwdU8Params cw;
         memset(&cw, 0, sizeof(cw));
         cw.rows = rows; cw.n = (int)n; cw.rows_per_cta = pl.rows_per_cta; cw.ws = wsbig; cw.wsb = wssmall;
-        { ProfScope ps(s, "conv1_wgrad", 2.0 * n * 400 * 32 * 256, (double)n * (28672 + 14112 * 2));
-          if ((rc = launch_conv1_wgrad_u8(cw, obs_aux, rows ? (int64_t)1 << 24 : n, act + Q.dact1, pl.splits, s, "naturecnn/conv1_wgrad_u8"))) return rc; }
+        cw.w2dg = P + L.w2dg; cw.m1 = reinterpret_cast<const uint32_t*>(act + Q.m1);
+        { ProfScope ps(s, "conv21_bwd", 2.0 * 2.0 * n * 400 * 32 * 256, (double)n * (7744 * 2 + 1600 + 28672 + 14112 * 2));
+          if ((rc = launch_conv21_bwd_u8(cw, obs_aux, rows ? (int64_t)1 << 24 : n, act + Q.dact2b, act + Q.dact1, pl.splits, s,
+                                         "naturecnn/conv21_bwd_u8"))) return rc; }
     } else {
         WGradWinParams gw;
         wgw_defaults(gw);

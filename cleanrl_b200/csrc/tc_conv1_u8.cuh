@@ -15,11 +15,12 @@
 //   Same window scheme as tc_conv_win: one TMA box of 128 + 22 rows per tile, the four 2x2 taps are descriptors
 //   shifted by whole 64-byte rows of a SWIZZLE_64B image.
 //
-// Weight gradient  tc_conv1_wgrad_u8: dW[tap, c, co] = sum_p X[p + off_tap, c] * dY[p, co].  The pixels go
+// Weight gradient  tc_conv21_bwd_u8 (which first computes dY, the conv2 data gradient, into shared memory):
+//   dW[tap, c, co] = sum_p X[p + off_tap, c] * dY[p, co].  The pixels go
 //   uint8 (shared memory, channel-major TMA box) -> fp16 pairs in REGISTERS (one PRMT per two pixels builds
 //   1024 + x; the offset is removed once per CTA through the bias partial), and are consumed as the A operand straight
-//   from registers (wgmma with A in registers); dY rows are SWIZZLE_64B TMA boxes used as an MN-major B operand with
-//   N = 32, read at two row offsets (0 and -21) so that one A fragment serves all four taps.  No 16-bit image of the
+//   from registers (wgmma with A in registers); dY rows are a SWIZZLE_64B shared-memory image used as an MN-major B
+//   operand, read at two row offsets (0 and -21) so that one A fragment serves all four taps.  No 16-bit image of the
 //   frames ever exists in shared or global memory.
 #pragma once
 #include "tc_base.cuh"
@@ -260,39 +261,54 @@ __global__ void __launch_bounds__(kConv1I8Threads, 1) tc_conv1_i8(const __grid_c
     }
 }
 
-// ------------------------------------------------------------------------------------ conv1 weight gradient (uint8 frames -> registers)
-// dW[tap, c, co] = sum_p X[p + off_tap, c] * dY[p, co] over the grid positions p of an image, off = {0, 1, 21, 22}
-// (taps (dy, dx) of the 2x2 window on the 21-wide grid).  Written over k = p + s_b with s_b = {0, 21}:
+// ------------------------------------------------------------------------------------ conv2 data gradient + conv1 weight gradient
+// One kernel computes d(act1) (the conv2 data gradient) and, from it, the conv1 weight and bias gradients, so that d(act1)
+// is written to HBM once and never read back.
+//
+// conv2 data gradient (warpgroup 1), per image: d(act1) = the full correlation of the zero-padded 11x11 d(act2) grid
+//   with the four stride-parity classes of W2 (one N = 128 GEMM, K = 4 taps x 64 channels), exactly as the window
+//   convolution tc_conv_win runs it: a TMA window of 140 rows of the image's d(act2) rows (128 GEMM rows + the largest tap
+//   shift of 12 rows), resident weights, m64n128k16 MMAs in the same tap and K order.  The epilogue (act1 > 0 mask, x
+//   kDact1Scale, saturating fp16) writes the image as the dY operand of the weight gradient straight into shared memory,
+//   and one TMA store per 128 rows copies it to d(act1) in HBM.
+// conv1 weight gradient (warpgroups 2 and 3): dW[tap, c, co] = sum_p X[p + off_tap, c] * dY[p, co] over the grid
+//   positions p of an image, off = {0, 1, 21, 22} (taps (dy, dx) of the 2x2 window on the 21-wide grid).  Written over
+//   k = p + s_b with s_b = {0, 21}:
 //       D_b[(h, c), co] = sum_k X[k + h, c] * dY[k - s_b, co],    tap = 2 b + h.
 //   A  (registers, 64 rows x 16 K per wgmma): warpgroup h holds channel c of the pixel stream X[k + h] as fp16 fragments;
 //       one fragment per K-step serves both tap groups b.
 //   B  (shared memory, MN-major SWIZZLE_64B): the dY rows of the step, rows [k0, k0 + 128) for b = 0 and rows
-//       [k0 - 21, k0 + 107) for b = 1.  The stages form one contiguous ring, so the b = 1 operand is the same tile moved
-//       21 rows back into the previous stage (the swizzle is a function of the address bits), and both are ONE N = 64
-//       operand: MN atom 0 (columns 0-31) starts at row k0 - 21 for b = 1, atom 1 (columns 32-63) 21 rows later for b = 0;
-//       stage 0 is preceded by a 24-row pad that receives the previous rows by a second small TMA box.  Negative rows and
-//       rows >= 441 are zero-filled by the TMA unit: images are independent and occupy 512-row slots, and a CTA owns whole
-//       images.
+//       [k0 - 21, k0 + 107) for b = 1, as ONE N = 64 operand: MN atom 0 (columns 0-31) starts at row k0 - 21 for b = 1,
+//       atom 1 (columns 32-63) 21 rows later for b = 0.  A dY image is [24-row zero halo | 512 rows] of 64 B: rows of
+//       positions that are not conv2 outputs (x = 20 or y = 20) and rows 441..511 stay zero, so the b = 1 operand of an
+//       image's first step and the padding rows of its last step read zeros.  Two dY images alternate, so the data
+//       gradient of image j + 1 runs under the weight gradient of image j.
 //   X  : channel-major frames [img][64 ch][448 rows] u8, staged in blocks of 128 positions (SWIZZLE_128B boxes of 64 full
 //        lines).  The h = 1 stream needs one pixel of the next block.
-//   dY : d(act1) on the 21x21 grid, fp16 [img][441][32] scaled by 2^12 (written by conv2's data gradient with a
-//        saturating conversion); rows of invalid positions (x = 20 or y = 20) are zero.
+//   dY : d(act1) on the 21x21 grid, fp16 [img][441][32] scaled by 2^12 (saturating conversion).
 //   The wgmma warps read their channel rows with 16-byte loads and expand uint8 -> fp16 with PRMTs (bytes (x, 0x64) =
-//   fp16 1024 + x; the offset is taken out again through the bias partial).  Four more warps accumulate the bias gradient
-//   (column sums of dY) from the staged tiles.  Partial tiles go to ws[cta][256][64] / wsb[cta][64] (first 32 columns
-//   used; row = tap * 64 + c) and are folded in fixed order by tc_fold_win.
-struct Conv1WgradU8Params {
+//   fp16 1024 + x; the offset is taken out again through the bias partial).  After publishing an image, warpgroup 1
+//   accumulates the bias gradient (column sums of dY) from it.  Partial tiles go to ws[cta][256][64] / wsb[cta][64]
+//   (first 32 columns used; row = tap * 64 + c) and are folded in fixed order by tc_fold_win.
+// Every output is bit-identical to the conv2 data gradient on tc_conv_win followed by a conv1 weight gradient that reads
+// d(act1) back: the same bf16 / fp16 products, the same fp32 accumulation order, the same CTA row ranges.
+struct Conv21BwdU8Params {
     const int64_t* rows;       // optional image gather (minibatch rows of the rollout)
     int n;                     // images of the minibatch
     int64_t rows_per_cta;      // multiple of 512 grid rows = whole images (M = n * 512)
+    const bf16* w2dg;          // conv2 data-gradient weights [128][4 taps x 64] (tc_pack_conv_s2_classes)
+    const uint32_t* m1;        // act1 > 0 bits: [n,100 cells] x 4 words
     float* ws;
     float* wsb;
 };
-// X blocks (8 KB: 64 channels x 128 positions) and dY steps (8 KB) in flight: 210 KB per SM, enough loads in flight to
-// cover the latency of the gathered reads.
-constexpr int kC1WXStages = 12, kC1WYStages = 14;
+// X blocks (8 KB: 64 channels x 128 positions) in flight; with the resident conv2 weights (64 KB), two d(act2) windows and
+// two dY images, six blocks fill the 227 KB of shared memory
+constexpr int kC1WXStages = 6, kC21WinStages = 2;
 constexpr int kC1WBlock = 64 * 128, kC1WYBytes = 128 * 64, kC1WYPadRows = 24, kC1WYPad = kC1WYPadRows * 64;
 constexpr int kC1WShift = 21;                     // grid rows between the two tap groups
+constexpr int kC21WinRows = 140, kC21WinBytes = 18 * 1024;      // 128 rows + the largest tap shift (12), 1 KB aligned
+constexpr int kC21W2Bytes = 4 * 128 * 128;                       // 4 taps x 128 output columns x 64 channels (bf16)
+constexpr int kC21ImgBytes = kC1WYPad + 4 * kC1WYBytes;          // zero halo + 512 rows of 64 B
 constexpr float kDact1Scale = 4096.0f;
 
 __device__ __forceinline__ uint32_t prmt(uint32_t a, uint32_t b, uint32_t sel) {
@@ -321,47 +337,72 @@ __device__ __forceinline__ uint4 lds128(uint32_t addr) {
     asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
     return v;
 }
+// fp32 pair -> fp16x2, saturating to +-65504 (d(act1) x kDact1Scale never becomes inf)
+__device__ __forceinline__ uint32_t pack_f16x2_sat(float lo, float hi) {
+    uint32_t d;
+    asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi), "f"(lo));
+    return d;
+}
+
+__device__ __forceinline__ void sts32(uint32_t addr, uint32_t v) { asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
+// TMA store of a shared-memory box (bulk-group completion); wait_read<N>: at most N groups may still be reading shared memory
+__device__ __forceinline__ void tma_store_3d(const void* tmap, uint32_t smem_src, int x, int y, int z) {
+    asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%1, %2, %3}], [%4];"
+                 ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(x), "r"(y), "r"(z), "r"(smem_src) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+template <int N> __device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
 
 // Per-warpgroup register budgets (setmaxnreg): the kernel launches at 128 registers per thread (512 threads, 1 CTA per
-// SM); the producer and bias warpgroups give registers back to the wgmma warpgroups, whose fragment build then keeps
-// more shared-memory loads in flight (measured: about 5 % less time per launch).  128 x 40 + 128 x 56 + 256 x 208 =
-// 65 536, the SM's register file.
+// SM); the producer warpgroup gives registers back to the weight-gradient warpgroups, whose fragment build then keeps more
+// shared-memory loads in flight.  The data-gradient warpgroup (64 accumulators) keeps the 128 it launched with.
 template <int R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 template <int R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
-constexpr int kC1WRegsProducer = 40, kC1WRegsBias = 56, kC1WRegsMma = 208;
-static_assert(128 * kC1WRegsProducer + 128 * kC1WRegsBias + 256 * kC1WRegsMma <= 65536, "register budgets exceed the SM");
+constexpr int kC1WRegsProducer = 40, kC21RegsDgrad = 128, kC1WRegsMma = 168;
+static_assert(128 * kC1WRegsProducer + 128 * kC21RegsDgrad + 256 * kC1WRegsMma <= 65536, "register budgets exceed the SM");
 
-// 512 threads: warp 0 = X producer, warp 1 = dY producer (warps 2-3 idle: warpgroup alignment), warpgroup 1 = bias sums,
-// warpgroups 2 and 3 = wgmma for the pixel streams h = 0 and h = 1
+// 512 threads: warp 0 = X producer, warp 1 = d(act2) window producer (warps 2-3 idle: warpgroup alignment), warpgroup 1 =
+// conv2 data gradient + bias sums, warpgroups 2 and 3 = wgmma for the pixel streams h = 0 and h = 1
 constexpr int kC1WThreads = 512;
-__global__ void __launch_bounds__(kC1WThreads, 1) tc_conv1_wgrad_u8(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmY,
-                                                                  const __grid_constant__ CUtensorMap tmYpad, const Conv1WgradU8Params p) {
-    constexpr int XS = kC1WXStages, YS = kC1WYStages;
+__global__ void __launch_bounds__(kC1WThreads, 1) tc_conv21_bwd_u8(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmWin,
+                                                                 const __grid_constant__ CUtensorMap tmY, const Conv21BwdU8Params p) {
+    constexpr int XS = kC1WXStages, WS = kC21WinStages;
     extern __shared__ uint8_t smem_raw[];
-    __shared__ uint64_t xfull[XS], xempty[XS], yfull[YS], yempty[YS];
+    __shared__ uint64_t xfull[XS], xempty[XS], wfull[WS], wempty[WS], yfull[2], yempty[2];
     __shared__ float sRed[32 * 32], sBias[32];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t* sX = smem;                                 // XS blocks of 8 KB
-    uint8_t* sYpad = smem + (size_t)XS * kC1WBlock;     // 24 rows in front of stage 0 (the ring's wrap-around halo)
-    uint8_t* sYb = sYpad + kC1WYPad;                    // YS stages of 8 KB, contiguous
+    uint8_t* sW2 = smem;                                       // conv2 data-gradient weights, 4 taps x 16 KB
+    uint8_t* sWin = sW2 + kC21W2Bytes;                         // WS d(act2) windows
+    uint8_t* sX = sWin + (size_t)WS * kC21WinBytes;            // XS blocks of 8 KB
+    uint8_t* sImg = sX + (size_t)XS * kC1WBlock;               // 2 dY images (512-B aligned: the SWIZZLE_64B pattern)
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     if (tid == 0) {
         // X block k is read by all eight wgmma warps as step k's main block and by the four h = 1 warps as step k - 1's halo;
-        // a dY stage is released by the eight wgmma warps and the bias group
+        // a window is released by the four data-gradient warps, a dY image by the eight wgmma warps
         for (int s = 0; s < XS; ++s) { mbar_init(&xfull[s], 1); mbar_init(&xempty[s], 12); }
-        for (int s = 0; s < YS; ++s) { mbar_init(&yfull[s], 1); mbar_init(&yempty[s], 8 + 1); }
+        for (int s = 0; s < WS; ++s) { mbar_init(&wfull[s], 1); mbar_init(&wempty[s], 4); }
+        for (int s = 0; s < 2; ++s) { mbar_init(&yfull[s], 1); mbar_init(&yempty[s], 8); }
         fence_barrier_init();
         tma_prefetch_desc(&tmX);
+        tma_prefetch_desc(&tmWin);
         tma_prefetch_desc(&tmY);
-        tma_prefetch_desc(&tmYpad);
     }
+    for (int idx = tid; idx < 4 * 128 * 8; idx += blockDim.x) {          // W2dg [128][256] -> 4 K-major SWIZZLE_128B taps
+        const int c16 = idx & 7, r = (idx >> 3) & 127, t = idx >> 10;
+        *reinterpret_cast<int4*>(sW2 + t * (128 * 128) + img_off(r, c16)) = ldg16(p.w2dg + r * 256 + t * 64 + c16 * 8);
+    }
+    for (int idx = tid; idx < 2 * kC21ImgBytes / 16; idx += blockDim.x) reinterpret_cast<int4*>(sImg)[idx] = make_int4(0, 0, 0, 0);
+    fence_proxy_async_smem();
     __syncthreads();
     const int64_t M = (int64_t)p.n * 512;
     const int64_t m_begin = (int64_t)blockIdx.x * p.rows_per_cta;
     int64_t m_end = m_begin + p.rows_per_cta;
     if (m_end > M) m_end = M;
     const int nsteps = m_end > m_begin ? (int)((m_end - m_begin) >> 7) : 0;
+    const int nimg = nsteps >> 2;
     const int64_t g0 = m_begin >> 7;                       // first global step (4 steps per image)
+    const int img0 = (int)(m_begin >> 9);
 
     if (warp < 4) {
         setmaxnreg_dec<kC1WRegsProducer>();
@@ -383,56 +424,118 @@ __global__ void __launch_bounds__(kC1WThreads, 1) tc_conv1_wgrad_u8(const __grid
                 tma_load_3d(smem_u32(sX + (size_t)xs * kC1WBlock), &tmX, (int)(g & 3) * 128, 0, z, &xfull[xs]);
             }
         } else if (warp == 1 && lane == 0) {
-            // =================== TMA producer 2: the dY rows of step k.  The tail of stage s is read by step k + 1 (b = 1),
-            // so stage s is reloaded (step k + YS) once steps k and k + 1 have both been consumed: the ring is YS - 1 steps deep.
-            for (int k = 0; k < nsteps; ++k) {
-                const int64_t g = g0 + k;
-                const int ys = k % YS;
-                if (k >= YS) mbar_wait2(&yempty[ys], ((k / YS) - 1) & 1, &yempty[(k + 1) % YS], ((k - YS + 1) / YS) & 1);
-                mbar_arrive_expect_tx(&yfull[ys], (uint32_t)(kC1WYBytes + (ys == 0 ? kC1WYPad : 0)));
-                tma_load_3d(smem_u32(sYb + (size_t)ys * kC1WYBytes), &tmY, 0, (int)(g & 3) * 128, (int)(g >> 2), &yfull[ys]);
-                if (ys == 0) tma_load_3d(smem_u32(sYpad), &tmYpad, 0, (int)(g & 3) * 128 - kC1WYPadRows, (int)(g >> 2), &yfull[ys]);
+            // =================== TMA producer 2: the d(act2) window of image j (rows 121 i .. 121 i + 139 of the padded
+            // 11x11 grids; rows past the last image are zero-filled)
+            for (int j = 0; j < nimg; ++j) {
+                const int s = j % WS;
+                if (j >= WS) mbar_wait(&wempty[s], ((j / WS) - 1) & 1);
+                mbar_arrive_expect_tx(&wfull[s], (uint32_t)(kC21WinRows * 128));
+                tma_load_2d(smem_u32(sWin + (size_t)s * kC21WinBytes), &tmWin, 0, (img0 + j) * 121, &wfull[s]);
             }
         }
     } else if (warp < 8) {
-        setmaxnreg_dec<kC1WRegsBias>();
-        // ======================= bias warps: bias gradient = column sums of dY from the staged tiles (fp32, fixed order)
-        const int tb = tid - 128;
-        const int rq = tb >> 2, c16 = tb & 3;
+        // ======================= conv2 data gradient of image j into dY image j & 1, then the bias sums of that image
+        const int wt = tid - 128, lane4 = lane >> 2, qd = lane & 3;
+        const uint32_t w_base = smem_u32(sW2);
+        const int rq = wt >> 2, c16 = wt & 3;                // bias sums: row group and 16-byte chunk of a 64-byte row
         float bsum[8];
 #pragma unroll
         for (int e = 0; e < 8; ++e) bsum[e] = 0.f;
-        for (int it = 0; it < nsteps; ++it) {
-            const int ys = it % YS;
-            if (tb < 32) mbar_wait(&yfull[ys], (it / YS) & 1);
+        for (int j = 0; j < nimg; ++j) {
+            const int i = img0 + j, buf = j & 1, s = j % WS;
+            const uint32_t img = smem_u32(sImg + (size_t)buf * kC21ImgBytes) + kC1WYPad;     // row 0 of the image
+            mbar_wait(&wfull[s], (j / WS) & 1);
+            // image j - 2 has left dY image `buf`: the weight gradient consumed it and its TMA store has read it
+            if (j >= 2) mbar_wait(&yempty[buf], ((j >> 1) - 1) & 1);
+            if (wt == 0) bulk_wait_read<1>();
             named_bar(1, 128);
-            const uint8_t* sY = sYb + (size_t)ys * kC1WYBytes;          // the step's own rows
+#pragma unroll 1
+            for (int h2 = 0; h2 < 2; ++h2) {
+                float d[64];
+                wgmma_fence();
+                const uint32_t win = smem_u32(sWin + (size_t)s * kC21WinBytes) + (uint32_t)(h2 * 64 * 128);
+                // taps t = (a, b): row shift (1 - a) * 11 + (1 - b), the order of tc_conv_win
+                constexpr int shift[4] = {12, 11, 1, 0};
 #pragma unroll
-            for (int ps = 0; ps < 4; ++ps) {
-                const int rr = ps * 32 + rq;
-                const int4 v = *reinterpret_cast<const int4*>(sY + img64_off(rr, c16));
-                const uint32_t w[4] = {(uint32_t)v.x, (uint32_t)v.y, (uint32_t)v.z, (uint32_t)v.w};
+                for (int t = 0; t < 4; ++t) {
+                    const uint64_t a = desc_kmajor(win + (uint32_t)shift[t] * 128u);
+                    const uint64_t b = desc_kmajor(w_base + (uint32_t)(t * 128 * 128));
 #pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                    const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&w[e]));
-                    bsum[2 * e] += f.x;
-                    bsum[2 * e + 1] += f.y;
+                    for (int kk = 0; kk < 4; ++kk) WgmmaBf16<128, 0, 0>::mma(d, a + 2 * kk, b + 2 * kk, (t | kk) != 0 ? 1u : 0u);
+                }
+                wgmma_commit();
+                // this thread's rows r and r + 8 of the 11x11 grid: cell (Y, X), its mask words, requested under the MMAs
+                int pos[2];
+                uint4 mb[2];
+#pragma unroll
+                for (int hr = 0; hr < 2; ++hr) {
+                    const int r = h2 * 64 + ((wt >> 5) << 4) + lane4 + 8 * hr;
+                    const int Y = (r * 5958) >> 16, X = r - Y * 11;           // r / 11 for r < 128
+                    const bool valid = Y < 10 && X < 10;
+                    pos[hr] = valid ? 2 * Y * 21 + 2 * X : -1;
+                    mb[hr] = make_uint4(0u, 0u, 0u, 0u);
+                    if (valid) {
+                        const int4 t = ldg16(p.m1 + ((int64_t)i * 100 + Y * 10 + X) * 4);
+                        mb[hr] = make_uint4((uint32_t)t.x, (uint32_t)t.y, (uint32_t)t.z, (uint32_t)t.w);
+                    }
+                }
+                wgmma_wait<0>();
+                wgmma_fence_operands(d);
+                if (h2 == 1 && lane == 0) mbar_arrive(&wempty[s]);
+                // epilogue on the accumulator fragment: column 8 jj + 2 qd (+1) = channel 8 (jj & 3) + 2 qd of class
+                // g = jj >> 2 = (py, px), stored at grid position (2 Y + py, 2 X + px) of the dY image
+#pragma unroll
+                for (int hr = 0; hr < 2; ++hr) {
+                    if (pos[hr] < 0) continue;
+                    const uint32_t mw[4] = {mb[hr].x, mb[hr].y, mb[hr].z, mb[hr].w};
+#pragma unroll
+                    for (int jj = 0; jj < 16; ++jj) {
+                        const int g = jj >> 2, c = 8 * (jj & 3) + 2 * qd;
+                        float f0 = d[4 * jj + 2 * hr] * kDact1Scale, f1 = d[4 * jj + 2 * hr + 1] * kDact1Scale;
+                        if (!((mw[g] >> c) & 1u)) f0 = 0.f;
+                        if (!((mw[g] >> (c + 1)) & 1u)) f1 = 0.f;
+                        const int q = pos[hr] + (g >> 1) * 21 + (g & 1);
+                        sts32(img + img64_off(q, c >> 3) + (uint32_t)((c & 7) * 2), pack_f16x2_sat(f0, f1));
+                    }
                 }
             }
+            // publish: the wgmma operand reads and the TMA store are async-proxy reads of what this warpgroup just wrote
+            fence_proxy_async_smem();
             named_bar(1, 128);
-            if (tb == 0) mbar_arrive(&yempty[ys]);
+            if (wt == 0) {
+                mbar_arrive(&yfull[buf]);
+#pragma unroll
+                for (int k = 0; k < 4; ++k) tma_store_3d(&tmY, img + (uint32_t)(k * kC1WYBytes), 0, k * 128, i);
+                bulk_commit();
+            }
+            // bias gradient = column sums of dY (fp32, fixed order: step by step, 32 rows apart per thread)
+#pragma unroll 1
+            for (int st = 0; st < 4; ++st) {
+#pragma unroll
+                for (int ps = 0; ps < 4; ++ps) {
+                    const uint4 v = lds128(img + (uint32_t)(st * kC1WYBytes) + img64_off(ps * 32 + rq, c16));
+                    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) {
+                        const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&w[e]));
+                        bsum[2 * e] += f.x;
+                        bsum[2 * e + 1] += f.y;
+                    }
+                }
+            }
         }
+        if (wt == 0) bulk_wait<0>();
 #pragma unroll
         for (int e = 0; e < 8; ++e) sRed[rq * 32 + c16 * 8 + e] = bsum[e];
         named_bar(1, 128);
-        if (tb < 32) {
+        if (wt < 32) {
             float t = 0.f;
 #pragma unroll
-            for (int l = 0; l < 32; ++l) t += sRed[l * 32 + tb];
-            p.wsb[(int64_t)blockIdx.x * 64 + tb] = t;
+            for (int l = 0; l < 32; ++l) t += sRed[l * 32 + wt];
+            p.wsb[(int64_t)blockIdx.x * 64 + wt] = t;
             // what the 1024 offset of every pixel added to each (tap, c) row: the CTA owns whole images, so the rows of the
             // b = 1 operand (shifted by 21, zero outside the image) sum to the same value as the rows of the b = 0 operand
-            sBias[tb] = t * kU8Bias;
+            sBias[wt] = t * kU8Bias;
         }
         named_bar(2, 384);                                  // sBias is ready for the wgmma warpgroups' drain
     } else {
@@ -452,7 +555,7 @@ __global__ void __launch_bounds__(kC1WThreads, 1) tc_conv1_wgrad_u8(const __grid
 #pragma unroll
         for (int e = 0; e < 32; ++e) d[e] = 0.f;
         for (int it = 0; it < nsteps; ++it) {
-            const int xm = it % XS, xh = (it + 1) % XS, ys = it % YS;
+            const int xm = it % XS, xh = (it + 1) % XS, buf = (it >> 2) & 1;
             mbar_wait(&xfull[xm], (it / XS) & 1);
             if (h == 1) mbar_wait(&xfull[xh], ((it + 1) / XS) & 1);
             uint32_t a[8][4];
@@ -479,14 +582,15 @@ __global__ void __launch_bounds__(kC1WThreads, 1) tc_conv1_wgrad_u8(const __grid
                 mbar_arrive(&xempty[xm]);
                 if (h == 1) { mbar_arrive(&xempty[xh]); if (it == 0) mbar_arrive(&xempty[xm]); }
             }
-            mbar_wait(&yfull[ys], (it / YS) & 1);
+            if ((it & 3) == 0) mbar_wait(&yfull[buf], (it >> 3) & 1);
             wgmma_fence();                                   // the A fragments were just written by ordinary instructions
-            const uint64_t yd = desc_mnmajor_sw64(smem_u32(sYb + (size_t)ys * kC1WYBytes) - kC1WShift * 64, kC1WShift * 64);
+            const uint32_t ystep = smem_u32(sImg + (size_t)buf * kC21ImgBytes) + (uint32_t)(kC1WYPad + (it & 3) * kC1WYBytes);
+            const uint64_t yd = desc_mnmajor_sw64(ystep - kC1WShift * 64, kC1WShift * 64);
 #pragma unroll
             for (int kk = 0; kk < 8; ++kk) wgmma_f16_rs_n64_tb(d, a[kk], yd + 64 * kk, (it | kk) != 0 ? 1u : 0u);
             wgmma_commit();
             wgmma_wait<0>();
-            if (lane == 0) mbar_arrive(&yempty[ys]);
+            if ((it & 3) == 3 && lane == 0) mbar_arrive(&yempty[buf]);
         }
         wgmma_fence_operands(d);
         named_bar(2, 384);
@@ -506,21 +610,23 @@ __global__ void __launch_bounds__(kC1WThreads, 1) tc_conv1_wgrad_u8(const __grid
     }
 }
 
-static int launch_conv1_wgrad_u8(const Conv1WgradU8Params& p, const void* frames_cm, int64_t n_images, const void* dact1_f16, int ctas,
-                                 cudaStream_t s, const char* what) {
-    const size_t smem = (size_t)kC1WXStages * kC1WBlock + kC1WYPad + (size_t)kC1WYStages * kC1WYBytes + 1024;
+// dact2b: d(act2) on the zero-padded 11x11 grids [n,121,64] bf16; dact1: fp16 x kDact1Scale [n,441,32] (written here)
+static int launch_conv21_bwd_u8(const Conv21BwdU8Params& p, const void* frames_cm, int64_t n_images, const bf16* dact2b, void* dact1_f16,
+                                int ctas, cudaStream_t s, const char* what) {
+    const size_t smem = (size_t)kC21W2Bytes + (size_t)kC21WinStages * kC21WinBytes + (size_t)kC1WXStages * kC1WBlock + 2 * (size_t)kC21ImgBytes + 1024;
     int rc;
     if (p.rows_per_cta % 512 != 0) return fail(B200RL_ERR_INVALID_ARGUMENT, "%s: a CTA must own whole images (512 grid rows)", what);
-    CUtensorMap tmX, tmY, tmYpad;
-    memset(&tmX, 0, sizeof(tmX)); memset(&tmY, 0, sizeof(tmY)); memset(&tmYpad, 0, sizeof(tmYpad));
-    // frames [img][64 ch][448 positions] u8: box = [64 ch][128 positions], SWIZZLE_128B; dY [img][441 rows][32 co] fp16 = 64-byte
-    // rows: box [128 rows][64 B], SWIZZLE_64B
+    CUtensorMap tmX, tmWin, tmY;
+    memset(&tmX, 0, sizeof(tmX)); memset(&tmWin, 0, sizeof(tmWin)); memset(&tmY, 0, sizeof(tmY));
+    // frames [img][64 ch][448 positions] u8: box = [64 ch][128 positions], SWIZZLE_128B; d(act2) rows [n * 121][64 ch] bf16:
+    // box = 140 rows, SWIZZLE_128B; dY [img][441 rows][32 co] fp16 = 64-byte rows: box [128 rows][64 B], SWIZZLE_64B (stores;
+    // rows >= 441 of a box are not written)
     if ((rc = make_tmap_3d_u8(&tmX, frames_cm, n_images, 64, 448, 448, 64, 128, what))) return rc;
+    if ((rc = make_tmap_2d(&tmWin, dact2b, (int64_t)p.n * 121, 64, kC21WinRows, what))) return rc;
     if ((rc = make_tmap_3d_u8(&tmY, dact1_f16, p.n, 441, 64, 64, 128, 64, what))) return rc;
-    if ((rc = make_tmap_3d_u8(&tmYpad, dact1_f16, p.n, 441, 64, 64, kC1WYPadRows, 64, what))) return rc;
     static SmemAttrCache attr;
-    if ((rc = attr.ensure(tc_conv1_wgrad_u8, smem, what))) return rc;
-    tc_conv1_wgrad_u8<<<ctas, kC1WThreads, smem, s>>>(tmX, tmY, tmYpad, p);
+    if ((rc = attr.ensure(tc_conv21_bwd_u8, smem, what))) return rc;
+    tc_conv21_bwd_u8<<<ctas, kC1WThreads, smem, s>>>(tmX, tmWin, tmY, p);
     return check_launch(what);
 }
 

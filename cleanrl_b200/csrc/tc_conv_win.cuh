@@ -40,14 +40,7 @@ struct WinParams {
     const float* bias;
     float scale;
     int relu;
-    int out_f16;             // store fp16 (saturating) instead of bf16: d(act1) feeding the uint8 conv1 weight gradient
 };
-
-__device__ __forceinline__ uint32_t pack_f16x2_sat(float lo, float hi) {
-    uint32_t d;
-    asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi), "f"(lo));
-    return d;
-}
 
 // Thread roles (384 threads): warpgroup 0 = TMA producer (warp 0; warps 1-3 only hold the warpgroup alignment that wgmma
 // requires); warpgroups 1 and 2 each run wgmma on 64 rows of every 128-row tile (accumulators in registers), hand the
@@ -235,15 +228,7 @@ __global__ void __launch_bounds__(kConvWinThreads, 1) tc_conv_win(const __grid_c
                     for (int e = 0; e < 32; ++e) if (!((mb[g] >> e) & 1u)) v[e] = 0u;
                 }
                 int4 w[4];
-                if (p.out_f16) {
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                        w[e].x = (int)pack_f16x2_sat(__uint_as_float(v[8 * e]), __uint_as_float(v[8 * e + 1]));
-                        w[e].y = (int)pack_f16x2_sat(__uint_as_float(v[8 * e + 2]), __uint_as_float(v[8 * e + 3]));
-                        w[e].z = (int)pack_f16x2_sat(__uint_as_float(v[8 * e + 4]), __uint_as_float(v[8 * e + 5]));
-                        w[e].w = (int)pack_f16x2_sat(__uint_as_float(v[8 * e + 6]), __uint_as_float(v[8 * e + 7]));
-                    }
-                } else if (p.relu) {
+                if (p.relu) {
 #pragma unroll
                     for (int e = 0; e < 4; ++e) {
                         w[e].x = (int)pack_bf16x2_relu(__uint_as_float(v[8 * e]), __uint_as_float(v[8 * e + 1]));
@@ -558,7 +543,7 @@ static int launch_conv_win_t(WinParams p, cudaStream_t s, const char* what) {
     if ((int64_t)p.G * p.Wp >= 65536 || p.G < 1)
         return fail(B200RL_ERR_INVALID_ARGUMENT, "%s: grid %d x width %d outside the epilogue's multiply-shift range", what, p.G, p.Wp);
     if (p.rows || p.tpi_shift) return fail(B200RL_ERR_INVALID_ARGUMENT, "%s: the channel-major kernel walks a contiguous linear grid", what);
-    if ((p.out_mode != WOUT_DENSE && p.out_mode != WOUT_DACT2) || p.out_f16)
+    if (p.out_mode != WOUT_DENSE && p.out_mode != WOUT_DACT2)
         return fail(B200RL_ERR_INVALID_ARGUMENT, "%s: only bf16 dense and conv3 data-gradient outputs in this kernel", what);
     int maxs = 0;
     for (int t = 0; t < NTAPS; ++t) maxs = p.shift[t] > maxs ? p.shift[t] : maxs;

@@ -25,8 +25,8 @@ ALGO = {
     "conv1_wgrad": (28224 + 14112) * 2, "fc_wgrad": (3136 + 512) * 2,
 }
 # uint8 rollout (round 2): conv1 reads the frames as bytes (row-major 28224 B forward, channel-major 28672 B for the
-# weight gradient whose dY operand is fp16)
-ALGO_U8 = {"conv1_fwd": 28224 + 12800 * 2 + 1600, "conv1_wgrad": 28672 + 14112 * 2}
+# weight gradient, which also computes the conv2 data gradient: d(act2) and the mask words in, fp16 d(act1) out)
+ALGO_U8 = {"conv1_fwd": 28224 + 12800 * 2 + 1600, "conv21_bwd": 7744 * 2 + 1600 + 28672 + 14112 * 2}
 
 
 def to_bytes(v, unit):
@@ -56,7 +56,7 @@ def main():
         seen[short] = k + 1
         layer = None
         if short.startswith("tc_conv1_i8"): layer = "conv1_fwd"
-        elif short.startswith("tc_conv1_wgrad_u8"): layer = "conv1_wgrad"
+        elif short.startswith("tc_conv21_bwd_u8"): layer = "conv21_bwd"
         elif short.startswith("tc_conv_win<32"): layer = "conv1_fwd"
         elif short.startswith("tc_conv_win<64, 2"): layer = "conv2_fwd"
         elif short.startswith("tc_conv_win<64, 1"): layer = "conv3_fwd" if k % 2 == 0 else "conv3_dgrad"
