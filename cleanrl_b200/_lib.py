@@ -96,6 +96,16 @@ SIGNATURES = {
     "b200rl_impala_bf16_pack": (_i, [_p, _i, _p, _p]),
     "b200rl_impala_bf16_forward": (_i, [_p, _p, _i64, _i, _p, _p, _p, _p, _p]),
     "b200rl_impala_bf16_backward": (_i, [_p, _p, _i64, _i, _p, _p, _p, _p, _p, _p, _sz, _p]),
+    "b200rl_impala_ppg_param_count": (_i64, [_i]),
+    "b200rl_impala_ppg_bf16_packed_bytes": (_sz, [_i]),
+    "b200rl_impala_ppg_bf16_workspace_bytes": (_sz, [_i64, _i]),
+    "b200rl_impala_ppg_bf16_pack": (_i, [_p, _i, _p, _p]),
+    "b200rl_impala_ppg_bf16_forward": (_i, [_p, _p, _i64, _i, _p, _p, _p, _p, _p]),
+    "b200rl_impala_ppg_bf16_backward": (_i, [_p, _p, _i64, _i, _p, _p, _p, _p, _p, _p, _sz, _p]),
+    "b200rl_clip_adam_ranges_f32": (_i, [_p, _p, _p, _p, _i64, _i64, _d, _p, _i, _i64, _d, _d, _d, _d, _d, _p, _p, _sz, _p]),
+    "b200rl_clip_adam_ranges_dyn_f32": (_i, [_p, _p, _p, _p, _i64, _p, _p, _i, _i, _d, _d, _d, _d, _p, _p, _sz, _p]),
+    "b200rl_ppg_aux_loss_workspace_bytes": (_sz, [_i64]),
+    "b200rl_ppg_aux_loss_f32": (_i, [_p, _i64, _p, _p, _p, _i64, _i, _d, _d, _p, _i64, _p, _p, _sz, _p]),
     "b200rl_lstm_agent_param_count": (_i64, [_i]),
     "b200rl_lstm_agent_bf16_packed_bytes": (_sz, [_i]),
     "b200rl_lstm_agent_bf16_acts_bytes": (_sz, [_i64, _i64]),

@@ -169,6 +169,10 @@ class TensorCoreAgent(KernelAgent):
     def _head_outputs(self):
         return self.num_actions + 1          # actor + critic
 
+    def _plan_actions(self):
+        """The ``A`` the plan is built for: its head is A actions + the plan's value outputs."""
+        return self._head_outputs() - 1
+
     def bind(self):
         self._tc, self._tc_dirty = None, True
         return super().bind()
@@ -188,7 +192,7 @@ class TensorCoreAgent(KernelAgent):
     def _tc_plan(self):
         f = self._flat
         if self._tc is None:
-            self._tc = self.plan_class(self._head_outputs() - 1, f.flat.device)
+            self._tc = self.plan_class(self._plan_actions(), f.flat.device)
             assert f.flat.numel() >= self._tc.param_count
         if self._tc_dirty:
             self._tc.pack(f.flat)
@@ -206,9 +210,9 @@ class TensorCoreAgent(KernelAgent):
             self._tc.pin()
 
     def _joint_head(self):
-        """``actor`` and ``critic`` as ONE layer over the flat buffer (adjacent in ``_param_order``): weight [A+1, hidden],
-        bias [A+1]."""
-        f, A1, H = self._flat, self.num_actions + 1, self.actor.in_features
+        """``actor`` and the value heads as ONE layer over the flat buffer (adjacent in ``_param_order``): weight
+        [_head_outputs(), hidden], bias [_head_outputs()]."""
+        f, A1, H = self._flat, self._head_outputs(), self.actor.in_features
         ow = (f.view_of(self.actor.weight)[0].data_ptr() - f.flat.data_ptr()) // 4
         ob = (f.view_of(self.actor.bias)[0].data_ptr() - f.flat.data_ptr()) // 4
         return nets.Linear(None, None, f.flat[ow:ow + A1 * H].view(A1, H), f.flat[ob:ob + A1],
@@ -568,6 +572,12 @@ class ImpalaAgent(TensorCoreAgent):
 
     # ------------------------------------------------------------------ forward
     def _forward_heads(self, x, rows=None, keep=False):
+        out = self._head_out(x, rows, keep)
+        A = self.num_actions
+        return out[:, :A], out[:, A]
+
+    def _head_out(self, x, rows=None, keep=False):
+        """The joint head's output [n, _head_outputs()] for frames ``x[rows]``."""
         if x.dtype != torch.uint8:
             x = x.to(torch.uint8)          # frames are integers 0..255 (the reference passes them as fp32)
         if self.precision == "bf16":
@@ -575,8 +585,7 @@ class ImpalaAgent(TensorCoreAgent):
             out = self._tc_plan().forward(x.contiguous(), rows, self._flat.flat)
             if keep:
                 self._tc_obs, self._tc_rows = x, rows
-            A = self.num_actions
-            return out[:, :A], out[:, A]
+            return out
         x = ops.nhwc_to_nchw_u8(x.contiguous(), rows)          # [n, 3, 64, 64] uint8; /255 inside the first convolution
         saved = []
         h = x
@@ -600,8 +609,7 @@ class ImpalaAgent(TensorCoreAgent):
         out = self.head.fwd(hid)
         if keep:
             self._saved = dict(seqs=saved, h0=h0, hid=hid, last_shape=tuple(h.shape))
-        A = self.num_actions
-        return out[:, :A], out[:, A]
+        return out
 
     def forward_train(self, b_obs, mb_inds):
         self.flat
@@ -615,7 +623,7 @@ class ImpalaAgent(TensorCoreAgent):
             return
         q = self._saved
         self.head.bwd_weight(q["hid"], dhead)
-        d_hid = self.head.bwd_data(dhead, q["hid"], "relu")                    # through the ReLU after the Linear
+        d_hid = self.head.bwd_data(self._dhead_into_hidden(dhead), q["hid"], "relu")   # through the ReLU after the Linear
         self.fc.bwd_weight(q["h0"], d_hid)
         d = self.fc.bwd_data(d_hid, q["h0"], "relu").view(q["last_shape"])     # through the ReLU after Flatten
         for si in (2, 1, 0):
@@ -631,6 +639,139 @@ class ImpalaAgent(TensorCoreAgent):
             if si > 0:
                 d = s["conv"].bwd_data(d_c, None, None, in_hw=tuple(rec["x"].shape[-2:]))
         self._saved = None
+
+    def _dhead_into_hidden(self, dhead):
+        """The head gradient that flows on into the hidden layer (all of it: every head reads ``hidden``)."""
+        return dhead
+
+
+def layer_init_normed(layer, norm_dim, scale=1.0):
+    """cleanrl/ppg_procgen.py:101-105: every output unit rescaled to L2 norm ``scale``, bias zeroed; consumes no RNG."""
+    with torch.no_grad():
+        layer.weight.data *= scale / layer.weight.norm(dim=norm_dim, p=2, keepdim=True)
+        layer.bias *= 0
+    return layer
+
+
+class PPGResidualBlock(nn.Module):
+    """Parameter container with the reference's names and initialisation (cleanrl/ppg_procgen.py:124-132)."""
+
+    def __init__(self, channels, scale):
+        super().__init__()
+        scale = np.sqrt(scale)
+        conv0 = nn.Conv2d(in_channels=channels, out_channels=channels, kernel_size=3, padding=1)
+        self.conv0 = layer_init_normed(conv0, norm_dim=(1, 2, 3), scale=scale)
+        conv1 = nn.Conv2d(in_channels=channels, out_channels=channels, kernel_size=3, padding=1)
+        self.conv1 = layer_init_normed(conv1, norm_dim=(1, 2, 3), scale=scale)
+
+
+class PPGConvSequence(nn.Module):
+    """cleanrl/ppg_procgen.py:143-165: conv3x3 -> max_pool(3, stride 2, padding 1) -> two residual blocks."""
+
+    def __init__(self, input_shape, out_channels, scale):
+        super().__init__()
+        self._input_shape = input_shape
+        self._out_channels = out_channels
+        conv = nn.Conv2d(in_channels=self._input_shape[0], out_channels=self._out_channels, kernel_size=3, padding=1)
+        self.conv = layer_init_normed(conv, norm_dim=(1, 2, 3), scale=1.0)
+        nblocks = 2
+        scale = scale / np.sqrt(nblocks)
+        self.res_block0 = PPGResidualBlock(self._out_channels, scale=scale)
+        self.res_block1 = PPGResidualBlock(self._out_channels, scale=scale)
+
+    def get_output_shape(self):
+        _c, h, w = self._input_shape
+        return (self._out_channels, (h + 1) // 2, (w + 1) // 2)
+
+
+class PPGAgent(ImpalaAgent):
+    """IMPALA-CNN agent of phasic policy gradient (reference: cleanrl/ppg_procgen.py:168-211): the ImpalaAgent trunk with
+    ``layer_init_normed`` initialisation and three heads, ``actor``, ``critic`` and ``aux_critic``.  Same module tree and
+    ``state_dict`` keys, same construction order, so a seed yields the reference's weights.
+
+    The three heads run as ONE joint head of A + 2 outputs, [logits | value | aux_value].  ``critic`` reads
+    ``hidden.detach()`` in every method of the reference: its column of the head gradient reaches ``critic.weight`` and
+    ``critic.bias`` only and is left out of the hidden layer's gradient (fp32: a copy of ``dhead`` with that column zeroed;
+    bf16: ops.ImpalaPPGBf16 skips the column)."""
+
+    plan_class = ops.ImpalaPPGBf16
+
+    def __init__(self, envs):
+        TensorCoreAgent.__init__(self)
+        h, w, c = envs.single_observation_space.shape
+        shape = (c, h, w)
+        conv_seqs = []
+        chans = [16, 32, 32]
+        scale = 1 / np.sqrt(len(chans))
+        for out_channels in chans:
+            conv_seq = PPGConvSequence(shape, out_channels, scale=scale)
+            shape = conv_seq.get_output_shape()
+            conv_seqs.append(conv_seq)
+        encodertop = nn.Linear(in_features=shape[0] * shape[1] * shape[2], out_features=256)
+        encodertop = layer_init_normed(encodertop, norm_dim=1, scale=1.4)
+        conv_seqs += [nn.Flatten(), nn.ReLU(), encodertop, nn.ReLU()]
+        self.network = nn.Sequential(*conv_seqs)
+        self.actor = layer_init_normed(nn.Linear(256, envs.single_action_space.n), norm_dim=1, scale=0.1)
+        self.critic = layer_init_normed(nn.Linear(256, 1), norm_dim=1, scale=0.1)
+        self.aux_critic = layer_init_normed(nn.Linear(256, 1), norm_dim=1, scale=0.1)
+        self.num_actions = int(envs.single_action_space.n)
+        if self.num_actions + 2 > 24:
+            raise ValueError(f"PPGAgent supports at most 22 actions (got {self.num_actions})")
+        self._feat_shape = shape
+
+    def _param_order(self):
+        net = [p for p in self.network.parameters()]
+        return net + [self.actor.weight, self.critic.weight, self.aux_critic.weight,
+                      self.actor.bias, self.critic.bias, self.aux_critic.bias]
+
+    def _head_outputs(self):
+        return self.num_actions + 2          # actor + critic + aux_critic
+
+    def _plan_actions(self):
+        return self.num_actions
+
+    def aux_critic_ranges(self):
+        """Element ranges [(lo, hi), ...] of ``aux_critic.weight`` and ``aux_critic.bias`` in the flat parameter vector."""
+        f = self.flat
+        out = []
+        for p in (self.aux_critic.weight, self.aux_critic.bias):
+            lo = (f.view_of(p)[0].data_ptr() - f.flat.data_ptr()) // 4
+            out.append((lo, lo + p.numel()))
+        return out
+
+    def alloc_head_grad(self, M, device):
+        """(dhead [M, A+2], its dlogits view, its dvalue view); the ``aux_value`` column stays zero: the policy phase's
+        loss does not read ``aux_critic``."""
+        A = self.num_actions
+        d = torch.zeros(M, A + 2, dtype=torch.float32, device=device)
+        return d, d[:, :A], d[:, A]
+
+    def _dhead_into_hidden(self, dhead):
+        d = dhead.clone()
+        d[:, self.num_actions] = 0           # critic(hidden.detach())
+        return d
+
+    def forward_aux(self, b_obs, rows):
+        """Auxiliary-phase forward over ``b_obs[rows]`` (gather fused, activations kept): [n, A + 2]."""
+        self.flat
+        return self._head_out(b_obs, rows=rows, keep=True)
+
+    # -- reference API (cleanrl/ppg_procgen.py:205-211)
+    def get_pi_value_and_aux_value(self, x):
+        """(normalised logits [n, A] as ``Categorical.logits``, value [n, 1], aux_value [n, 1])."""
+        self.flat
+        out = self._head_out(x)
+        A = self.num_actions
+        lg = out[:, :A]
+        return lg - lg.logsumexp(dim=-1, keepdim=True), out[:, A:A + 1].clone(), out[:, A + 1:A + 2].clone()
+
+    def get_pi(self, x, rows=None):
+        """Normalised logits [n, A] of the policy for ``x`` (or ``x[rows]``, gathered by the network), as
+        ``Categorical(logits=...).logits``."""
+        self.flat
+        out = self._head_out(x, rows=rows)
+        lg = out[:, :self.num_actions]
+        return lg - lg.logsumexp(dim=-1, keepdim=True)
 
 
 def _normal_noise(n, D, device):

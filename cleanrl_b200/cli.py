@@ -126,6 +126,29 @@ def ppo_procgen_args(exp_name="ppo_procgen"):
     return _make("Args", _override(_COMMON, exp_name=exp_name) + algo + _RUNTIME + _EXTRA)
 
 
+def ppg_procgen_args(exp_name="ppg_procgen"):
+    """cleanrl/ppg_procgen.py:19-98."""
+    algo = [r for r in _override(_ALGO, env_id="starpilot", total_timesteps=int(25e6), learning_rate=5e-4, num_envs=64,
+                                 num_steps=256, anneal_lr=False, gamma=0.999, num_minibatches=8)
+            if r[0] not in ("update_epochs", "norm_adv")]
+    at = [r[0] for r in algo].index("clip_coef")
+    algo.insert(at, ("adv_norm_fullbatch", bool, True, "Toggle full batch advantage normalization as used in PPG code"))
+    ppg = [
+        ("n_iteration", int, 32, "N_pi: the number of policy update in the policy phase "),
+        ("e_policy", int, 1, "E_pi: the number of policy update in the policy phase "),
+        ("v_value", int, 1, "E_V: the number of policy update in the policy phase "),
+        ("e_auxiliary", int, 6, "E_aux:the K epochs to update the policy"),
+        ("beta_clone", float, 1.0, "the behavior cloning coefficient"),
+        ("num_aux_rollouts", int, 4, "the number of mini batch in the auxiliary phase"),
+        ("n_aux_grad_accum", int, 1, "the number of gradient accumulation in mini batch"),
+    ]
+    runtime = _RUNTIME + [
+        ("num_phases", int, 0, "the number of phases (computed in runtime)"),
+        ("aux_batch_rollouts", int, 0, "the number of rollouts in the auxiliary phase (computed in runtime)"),
+    ]
+    return _make("Args", _override(_COMMON, exp_name=exp_name) + algo + ppg + runtime + _EXTRA)
+
+
 def ppo_atari_multigpu_envpool_args(exp_name="ppo_atari_multigpu_envpool"):
     """The script the reference defers (docs/rl-algorithms/ppo.md:1020): ppo_atari_multigpu.py's data parallelism over
     ppo_atari_envpool.py's vector env.  Fields = the multi-GPU script's, env defaults = the envpool script's."""

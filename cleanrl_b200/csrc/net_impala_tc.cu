@@ -22,6 +22,9 @@
 //                 CTA's fixed band range, per-CTA partials folded in a fixed order (deterministic), bias = column sums.
 //   fc / heads    fc 2048 -> 256 on tc_gemm_tma (forward and data gradient) and tc_wgrad_tma (folded by tc_fold_fc, bias by
 //                 tc_colsum_*); heads (A+1 <= kMaxHeads) on CUDA cores in fp32 (tc_heads_* with 256 hidden units).
+//   PPG variant   cleanrl/ppg_procgen.py:168-211: the same trunk with a third head, [logits | value | aux_value] = A + 2
+//                 outputs.  `critic` (column A) reads a detached copy of the hidden layer: its dhead column reaches its own
+//                 weight and bias only, never the hidden layer's data gradient.  b200rl_impala_ppg_*.
 #include <cuda.h>
 #include <algorithm>
 #include <cstring>
@@ -459,11 +462,11 @@ __global__ void pack_fc(const float* __restrict__ w, bf16* __restrict__ fwd, bf1
     dg[(size_t)(pp * 32 + c) * 256 + o] = v;
 }
 // ---------------------------------------------------------------- host plan
-struct ImpalaLayout {       // flat fp32 parameter offsets (ImpalaAgent._param_order) and packed bf16 offsets
-    int A;
+struct ImpalaLayout {       // flat fp32 parameter offsets (ImpalaAgent / PPGAgent._param_order) and packed bf16 offsets
+    int A1;                 // head outputs: A + 1 (actor | critic) or A + 2 (actor | critic | aux_critic)
     int64_t cw[15], cb[15], fcw, fcb, hw, hb, total;
     int64_t pf[15], pd[15], pfc, pfcd, packed_total;
-    explicit ImpalaLayout(int A_) : A(A_) {
+    explicit ImpalaLayout(int A1_) : A1(A1_) {
         int64_t o = 0, q = 0;
         const int cin[3] = {3, 16, 32}, cout[3] = {16, 32, 32};
         for (int s = 0; s < 3; ++s)
@@ -476,8 +479,8 @@ struct ImpalaLayout {       // flat fp32 parameter offsets (ImpalaAgent._param_o
             }
         fcw = o; o += 256 * 2048;
         fcb = o; o += 256;
-        hw = o; o += (int64_t)(A + 1) * 256;
-        hb = o; o += A + 1;
+        hw = o; o += (int64_t)A1 * 256;
+        hb = o; o += A1;
         total = o;
         pfc = q; q += 256 * 2048;
         pfcd = q; q += 256 * 2048;
@@ -512,7 +515,8 @@ struct ImpalaActs {         // byte offsets in the (zero-initialised) activation
     }
 };
 
-static bool heads_ok(int A) { return A >= 1 && A + 1 <= kMaxHeads; }
+// A actions plus `values` value heads (1: actor-critic, 2: PPG's critic and aux_critic)
+static bool heads_ok(int A, int values = 1) { return A >= 1 && A + values <= kMaxHeads; }
 constexpr int64_t kMaxN = (int64_t)1 << 17;
 
 static Geo geo(int H, int fold = 0) {
@@ -568,8 +572,12 @@ static size_t wgrad_ws_floats() { return (size_t)kWgradCtas * 32 * 288; }
 using namespace b200rl;
 using namespace b200rl::imp;
 
-extern "C" int64_t b200rl_impala_param_count(int A) { return A >= 1 ? ImpalaLayout(A).total : -1; }
-extern "C" size_t b200rl_impala_bf16_packed_bytes(int A) { return heads_ok(A) ? (size_t)ImpalaLayout(A).packed_total * 2 : 0; }
+extern "C" int64_t b200rl_impala_param_count(int A) { return A >= 1 ? ImpalaLayout(A + 1).total : -1; }
+extern "C" size_t b200rl_impala_bf16_packed_bytes(int A) { return heads_ok(A) ? (size_t)ImpalaLayout(A + 1).packed_total * 2 : 0; }
+extern "C" int64_t b200rl_impala_ppg_param_count(int A) { return A >= 1 ? ImpalaLayout(A + 2).total : -1; }
+extern "C" size_t b200rl_impala_ppg_bf16_packed_bytes(int A) {
+    return heads_ok(A, 2) ? (size_t)ImpalaLayout(A + 2).packed_total * 2 : 0;
+}
 extern "C" size_t b200rl_impala_bf16_acts_bytes(int64_t n) { return n >= 0 && n <= kMaxN ? (size_t)ImpalaActs(n).total : 0; }
 extern "C" int b200rl_impala_bf16_acts_layout(int64_t n, int64_t* offsets) {
     B200RL_REQUIRE(offsets, "impala_acts_layout: null pointer");
@@ -589,17 +597,23 @@ extern "C" int b200rl_impala_bf16_acts_layout(int64_t n, int64_t* offsets) {
 // the backward workspace = [big part: weight-gradient partials, sized for the largest n | small part], each the largest
 // its launches need: heads, fc, convolutions
 static size_t impala_big_bytes() { return std::max(wgrad_tma_bytes(kMaxN, 256, 2048), wgrad_ws_floats() * 4); }
-extern "C" size_t b200rl_impala_bf16_workspace_bytes(int64_t n, int A) {
-    if (n < 1 || n > kMaxN || !heads_ok(A)) return 0;
-    const size_t small = std::max({heads_partial_bytes(n, A + 1, 256), colsum_ws(n, 256), (size_t)kWgradCtas * 32 * 4});
+static size_t impala_workspace_bytes(int64_t n, int A1) {
+    const size_t small = std::max({heads_partial_bytes(n, A1, 256), colsum_ws(n, 256), (size_t)kWgradCtas * 32 * 4});
     return impala_big_bytes() + small + 512;
 }
+extern "C" size_t b200rl_impala_bf16_workspace_bytes(int64_t n, int A) {
+    return n < 1 || n > kMaxN || !heads_ok(A) ? 0 : impala_workspace_bytes(n, A + 1);
+}
+extern "C" size_t b200rl_impala_ppg_bf16_workspace_bytes(int64_t n, int A) {
+    return n < 1 || n > kMaxN || !heads_ok(A, 2) ? 0 : impala_workspace_bytes(n, A + 2);
+}
 
-extern "C" int b200rl_impala_bf16_pack(const float* params, int A, void* packed, void* stream) {
+// `values` = 1 (actor | critic) or 2 (the PPG variant's actor | critic | aux_critic)
+static int impala_pack(const float* params, int A, int values, void* packed, void* stream) {
     B200RL_REQUIRE(params && packed, "impala_pack: null pointer");
-    B200RL_REQUIRE(heads_ok(A), "impala_pack: A=%d outside [1,%d]", A, kMaxHeads - 1);
+    B200RL_REQUIRE(heads_ok(A, values), "impala_pack: A=%d outside [1,%d]", A, kMaxHeads - values);
     B200RL_REQUIRE(aligned(params, 16) && aligned(packed, 16), "impala_pack: misaligned buffer");
-    const ImpalaLayout L(A);
+    const ImpalaLayout L(A + values);
     bf16* P = reinterpret_cast<bf16*>(packed);
     cudaStream_t s = (cudaStream_t)stream;
     ProfScope ps(s, "pack_weights", 0, (double)L.total * 4 + (double)L.packed_total * 2);
@@ -612,6 +626,12 @@ extern "C" int b200rl_impala_bf16_pack(const float* params, int A, void* packed,
     pack_fc<<<2048, 256, 0, s>>>(params + L.fcw, P + L.pfc, P + L.pfcd);
     return check_launch("impala_pack", 16);
 }
+extern "C" int b200rl_impala_bf16_pack(const float* params, int A, void* packed, void* stream) {
+    return impala_pack(params, A, 1, packed, stream);
+}
+extern "C" int b200rl_impala_ppg_bf16_pack(const float* params, int A, void* packed, void* stream) {
+    return impala_pack(params, A, 2, packed, stream);
+}
 
 namespace {
 ConvP conv_defaults(const Geo& g) { ConvP p; memset(&p, 0, sizeof(p)); p.g = g; p.scale = 1.f; return p; }
@@ -621,16 +641,17 @@ WgradP wgrad_defaults(const Geo& g, float* ws, float* wsb) {
 const int kH[3] = {64, 32, 16};           // conv input size of each sequence
 }  // namespace
 
-extern "C" int b200rl_impala_bf16_forward(const uint8_t* obs, const int64_t* rows, int64_t n, int A, const float* params,
-                                          const void* packed, void* acts, float* head_out, void* stream) {
+static int impala_forward(const uint8_t* obs, const int64_t* rows, int64_t n, int A, int values, const float* params,
+                          const void* packed, void* acts, float* head_out, void* stream) {
     B200RL_REQUIRE(n >= 0, "impala_forward: negative n");
     B200RL_REQUIRE(obs && params && packed && acts && head_out, "impala_forward: null pointer");
-    B200RL_REQUIRE(heads_ok(A), "impala_forward: A=%d outside [1,%d]", A, kMaxHeads - 1);
+    B200RL_REQUIRE(heads_ok(A, values), "impala_forward: A=%d outside [1,%d]", A, kMaxHeads - values);
     B200RL_REQUIRE(n <= kMaxN, "impala_forward: n=%lld above %lld", (long long)n, (long long)kMaxN);
     B200RL_REQUIRE(aligned(params, 16) && aligned(packed, 16) && aligned(acts, 256) && aligned(head_out, 4) &&
                    aligned(rows, 8), "impala_forward: misaligned buffer");
     if (n == 0) return B200RL_OK;
-    const ImpalaLayout L(A);
+    const int A1 = A + values;
+    const ImpalaLayout L(A1);
     const ImpalaActs Q(n);
     const bf16* P = reinterpret_cast<const bf16*>(packed);
     uint8_t* ab = reinterpret_cast<uint8_t*>(acts);
@@ -686,22 +707,32 @@ extern "C" int b200rl_impala_bf16_forward(const uint8_t* obs, const int64_t* row
     g.mask_out = reinterpret_cast<uint32_t*>(ab + Q.mhid);
     { ProfScope ps(s, "fc_fwd", 2.0 * n * 256 * 2048, (double)n * (2048 + 256) * 2 + 256.0 * 2048 * 2);
       if ((rc = launch_gemm_tma<64, 6>(g, s, "impala/fc"))) return rc; }
-    ProfScope ps(s, "heads_fwd", 2.0 * n * 256 * (A + 1), (double)n * (512 + 4 * (A + 1)));
-    return heads_fwd<256>(T(Q.hid), params + L.hw, params + L.hb, n, A + 1, head_out, s, "impala/heads");
+    ProfScope ps(s, "heads_fwd", 2.0 * n * 256 * A1, (double)n * (512 + 4 * A1));
+    return heads_fwd<256>(T(Q.hid), params + L.hw, params + L.hb, n, A1, head_out, s, "impala/heads");
+}
+extern "C" int b200rl_impala_bf16_forward(const uint8_t* obs, const int64_t* rows, int64_t n, int A, const float* params,
+                                          const void* packed, void* acts, float* head_out, void* stream) {
+    return impala_forward(obs, rows, n, A, 1, params, packed, acts, head_out, stream);
+}
+extern "C" int b200rl_impala_ppg_bf16_forward(const uint8_t* obs, const int64_t* rows, int64_t n, int A, const float* params,
+                                              const void* packed, void* acts, float* head_out, void* stream) {
+    return impala_forward(obs, rows, n, A, 2, params, packed, acts, head_out, stream);
 }
 
-extern "C" int b200rl_impala_bf16_backward(const uint8_t* obs, const int64_t* rows, int64_t n, int A, const float* params,
-                                           const void* packed, void* acts, const float* dhead, float* grads,
-                                           void* workspace, size_t workspace_bytes, void* stream) {
+// values == 2: head column A (PPG's critic) read a detached hidden layer, so it stays out of the hidden layer's gradient
+static int impala_backward(const uint8_t* obs, const int64_t* rows, int64_t n, int A, int values, const float* params,
+                           const void* packed, void* acts, const float* dhead, float* grads,
+                           void* workspace, size_t workspace_bytes, void* stream) {
     B200RL_REQUIRE(n >= 1, "impala_backward: n must be >= 1");
     B200RL_REQUIRE(obs && params && packed && acts && dhead && grads && workspace, "impala_backward: null pointer");
-    B200RL_REQUIRE(heads_ok(A), "impala_backward: A=%d outside [1,%d]", A, kMaxHeads - 1);
+    B200RL_REQUIRE(heads_ok(A, values), "impala_backward: A=%d outside [1,%d]", A, kMaxHeads - values);
     B200RL_REQUIRE(n <= kMaxN, "impala_backward: n=%lld above %lld", (long long)n, (long long)kMaxN);
     B200RL_REQUIRE(aligned(params, 16) && aligned(packed, 16) && aligned(acts, 256) && aligned(workspace, 256) &&
                    aligned(dhead, 4) && aligned(grads, 16) && aligned(rows, 8), "impala_backward: misaligned buffer");
-    const size_t need = b200rl_impala_bf16_workspace_bytes(n, A);
+    const int A1 = A + values;
+    const size_t need = impala_workspace_bytes(n, A1);
     if (workspace_bytes < need) return fail(B200RL_ERR_WORKSPACE, "impala_backward: workspace %zu < %zu", workspace_bytes, need);
-    const ImpalaLayout L(A);
+    const ImpalaLayout L(A1);
     const ImpalaActs Q(n);
     const bf16* P = reinterpret_cast<const bf16*>(packed);
     uint8_t* ab = reinterpret_cast<uint8_t*>(acts);
@@ -709,13 +740,13 @@ extern "C" int b200rl_impala_bf16_backward(const uint8_t* obs, const int64_t* ro
     cudaStream_t s = (cudaStream_t)stream;
     float* wsbig = reinterpret_cast<float*>(workspace);
     float* wssmall = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(workspace) + impala_big_bytes());
-    const int A1 = A + 1;
     int rc;
     // ---- heads
     {
         ProfScope ps(s, "heads_bwd", 4.0 * n * 256 * A1, (double)n * (1024 + 8 * A1));
         if ((rc = heads_bwd_weight<256>(dhead, T(Q.hid), n, A1, wssmall, grads + L.hw, grads + L.hb, s, "impala/heads_bwd"))) return rc;
-        if ((rc = heads_bwd_data<256>(dhead, params + L.hw, ab + Q.mhid, n, A1, T(Q.dhid), s, "impala/heads_bwd"))) return rc;
+        if ((rc = heads_bwd_data<256>(dhead, params + L.hw, ab + Q.mhid, n, A1, T(Q.dhid), s, "impala/heads_bwd",
+                                      values == 2 ? A : -1))) return rc;
     }
     // ---- fc: dW = dhid^T . h0 (row splits folded in order), db = column sums, dh0 = (dhid . Wfc) * (h0 > 0)
     {
@@ -797,4 +828,14 @@ extern "C" int b200rl_impala_bf16_backward(const uint8_t* obs, const int64_t* ro
         Gn = G; G = d.out;
     }
     return B200RL_OK;
+}
+extern "C" int b200rl_impala_bf16_backward(const uint8_t* obs, const int64_t* rows, int64_t n, int A, const float* params,
+                                           const void* packed, void* acts, const float* dhead, float* grads,
+                                           void* workspace, size_t workspace_bytes, void* stream) {
+    return impala_backward(obs, rows, n, A, 1, params, packed, acts, dhead, grads, workspace, workspace_bytes, stream);
+}
+extern "C" int b200rl_impala_ppg_bf16_backward(const uint8_t* obs, const int64_t* rows, int64_t n, int A, const float* params,
+                                               const void* packed, void* acts, const float* dhead, float* grads,
+                                               void* workspace, size_t workspace_bytes, void* stream) {
+    return impala_backward(obs, rows, n, A, 2, params, packed, acts, dhead, grads, workspace, workspace_bytes, stream);
 }

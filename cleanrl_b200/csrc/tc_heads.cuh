@@ -63,13 +63,14 @@ __global__ void __launch_bounds__(256) tc_heads_fwd(const bf16* __restrict__ hid
         if (lane < A1) out[row * A1 + lane] = mine;     // one coalesced store per row
     }
 }
-// dhid_pre[n][HT] (bf16) = (dhead[n][A1] . Wh[A1][HT]) * (hid > 0).  Thread = 8 consecutive hidden units of one
+// dhid_pre[n][HT] (bf16) = (dhead[n][A1] . Wh[A1][HT]) * (hid > 0), leaving head `skip_col` out of the product (-1 = none:
+// a head that reads a detached copy of the hidden layer).  Thread = 8 consecutive hidden units of one
 // row (one mask byte in, one 16-byte store out).  Weights are staged transposed, sWt[a][e][group], so the 32 lanes
 // of a warp (consecutive groups) hit 32 different banks.
 template <int HT = 512>
 __global__ void __launch_bounds__(256) tc_heads_bwd_data(const float* __restrict__ dhead, const float* __restrict__ Wh,
                                                          const uint8_t* __restrict__ hid_bits, int64_t n, int A1, int H,
-                                                         bf16* __restrict__ dhid) {
+                                                         int skip_col, bf16* __restrict__ dhid) {
     constexpr int G = HT / 8;                           // groups of 8 per row
     extern __shared__ float sWt[];                      // [A1][8][G]
     for (int i = threadIdx.x; i < A1 * HT; i += blockDim.x) {
@@ -86,6 +87,7 @@ __global__ void __launch_bounds__(256) tc_heads_bwd_data(const float* __restrict
 #pragma unroll
         for (int e = 0; e < 8; ++e) o[e] = 0.f;
         for (int a = 0; a < A1; ++a) {
+            if (a == skip_col) continue;
             const float d = __ldg(dhead + row * A1 + a);
 #pragma unroll
             for (int e = 0; e < 8; ++e) o[e] = fmaf(d, sWt[a * HT + e * G + g], o[e]);
@@ -193,13 +195,13 @@ static int heads_bwd_weight(const float* dhead, const bf16* hid, int64_t n, int 
     tc_heads_fold<<<(unsigned)ceil_div(A1 * (H + 2), 32), 256, 0, s>>>(part, 2 * nb, A1, H, dW, db);
     return check_launch(what, 2);
 }
-// dhid = (dhead . Wh) * (hid > 0), hid_bits = one mask byte per 8 hidden units
+// dhid = (dhead . Wh) * (hid > 0) without head `skip_col` (-1 = all heads), hid_bits = one mask byte per 8 hidden units
 template <int H>
 static int heads_bwd_data(const float* dhead, const float* Wh, const uint8_t* hid_bits, int64_t n, int A1, bf16* dhid,
-                          cudaStream_t s, const char* what) {
+                          cudaStream_t s, const char* what, int skip_col = -1) {
     static_assert(H == 128 || H == 256 || H == 512, "head input width");
     const int grid = (int)(ceil_div(n * H, 2048) < (int64_t)num_sms() * 8 ? ceil_div(n * H, 2048) : (int64_t)num_sms() * 8);
-    tc_heads_bwd_data<H><<<grid, 256, (size_t)A1 * H * sizeof(float), s>>>(dhead, Wh, hid_bits, n, A1, H, dhid);
+    tc_heads_bwd_data<H><<<grid, 256, (size_t)A1 * H * sizeof(float), s>>>(dhead, Wh, hid_bits, n, A1, H, skip_col, dhid);
     return check_launch(what);
 }
 

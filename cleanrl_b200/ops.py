@@ -237,6 +237,89 @@ def clip_adam_dyn(params, grads, exp_avg, exp_avg_sq, step_scalars, beta1=0.9, b
     return params
 
 
+def clip_adam_ranges(params, grads, exp_avg, exp_avg_sq, step, lr, ranges, range_step, range_lr=0.0, beta1=0.9,
+                     beta2=0.999, eps=1e-8, max_norm=0.5, norm_out=None):
+    """``clip_adam`` with torch's per-tensor semantics for the element ranges ``ranges`` = [(lo, hi), ...] (at most 4) of
+    the flat vector: ``range_step == 0`` freezes them (a tensor whose ``grad is None``: left out of the clip norm, weights
+    and moments untouched), ``range_step >= 1`` updates them with their own ``(range_step, range_lr)`` while every other
+    element uses ``(step, lr)`` (reference: cleanrl/ppg_procgen.py:393-394,465-466 with ``aux_critic``)."""
+    import ctypes
+    lib = _lib.load()
+    P = params.numel()
+    f = torch.float32
+    for n_, t in (("params", params), ("grads", grads), ("exp_avg", exp_avg), ("exp_avg_sq", exp_avg_sq)):
+        _contig(t, n_)
+        assert t.numel() == P
+    flat = [int(v) for r in ranges for v in r]
+    arr = (ctypes.c_int64 * max(len(flat), 1))(*flat)
+    ws = _workspace(params.device, "adam", lib.b200rl_clip_adam_workspace_bytes(P))
+    rc = lib.b200rl_clip_adam_ranges_f32(
+        _ptr(params, f, "params"), _ptr(grads, f, "grads"), _ptr(exp_avg, f, "exp_avg"), _ptr(exp_avg_sq, f, "exp_avg_sq"), P,
+        int(step), float(lr), arr, len(ranges), int(range_step), float(range_lr), float(beta1), float(beta2), float(eps),
+        -1.0 if max_norm is None else float(max_norm), _ptr(norm_out, f, "norm_out", True), ws.data_ptr(), ws.numel(), _stream())
+    _lib.check(rc, "clip_adam_ranges")
+    return params
+
+
+def clip_adam_ranges_dyn(params, grads, exp_avg, exp_avg_sq, step_scalars, ranges, frozen=False, beta1=0.9, beta2=0.999,
+                         eps=1e-8, max_norm=0.5, norm_out=None):
+    """``clip_adam_ranges`` with the step-dependent scalars in device memory: ``step_scalars`` f32[4] =
+    ``adam_step_scalars(step, lr) + adam_step_scalars(range_step, range_lr)``; what a captured CUDA graph replays."""
+    import ctypes
+    lib = _lib.load()
+    P = params.numel()
+    f = torch.float32
+    for n_, t in (("params", params), ("grads", grads), ("exp_avg", exp_avg), ("exp_avg_sq", exp_avg_sq)):
+        _contig(t, n_)
+        assert t.numel() == P
+    assert step_scalars.numel() == 4 and step_scalars.is_contiguous()
+    flat = [int(v) for r in ranges for v in r]
+    arr = (ctypes.c_int64 * max(len(flat), 1))(*flat)
+    ws = _workspace(params.device, "adam", lib.b200rl_clip_adam_workspace_bytes(P))
+    rc = lib.b200rl_clip_adam_ranges_dyn_f32(
+        _ptr(params, f, "params"), _ptr(grads, f, "grads"), _ptr(exp_avg, f, "exp_avg"), _ptr(exp_avg_sq, f, "exp_avg_sq"), P,
+        _ptr(step_scalars, f, "step_scalars"), arr, len(ranges), int(bool(frozen)), float(beta1), float(beta2), float(eps),
+        -1.0 if max_norm is None else float(max_norm), _ptr(norm_out, f, "norm_out", True), ws.data_ptr(), ws.numel(), _stream())
+    _lib.check(rc, "clip_adam_ranges_dyn")
+    return params
+
+
+PPG_AUX_STAT_NAMES = ("kl_loss", "aux_value_loss", "real_value_loss")
+
+
+def ppg_aux_loss(head_out, rows, old_logits, returns, beta_clone, inv_accum=1.0, dhead=None, stats=None):
+    """Fused auxiliary-phase loss of phasic policy gradient + its gradient (reference: cleanrl/ppg_procgen.py:449-461).
+    ``head_out`` [n, A + 2] = [logits | value | aux_value]; row i is compared with ``old_logits[rows[i]]`` [*, A] and
+    ``returns[rows[i]]``.  ``rows`` must index inside ``old_logits`` / ``returns``: the kernel does not check them.
+    Returns (stats f32[>= 3]: kl_loss, aux_value_loss, real_value_loss; dhead [n, A + 2])."""
+    lib = _lib.load()
+    n, A2 = head_out.shape
+    A = A2 - 2
+    dev = head_out.device
+    f = torch.float32
+    assert head_out.stride(1) == 1
+    if dhead is None:
+        dhead = torch.empty(n, A2, dtype=f, device=dev)
+    assert dhead.shape == (n, A2) and dhead.stride(1) == 1
+    if stats is None:
+        stats = torch.zeros(4, dtype=f, device=dev)
+    old_logits = _contig(old_logits, "old_logits").view(-1, old_logits.shape[-1])
+    returns = _contig(returns, "returns").view(-1)
+    assert old_logits.shape[1] == A and old_logits.shape[0] == returns.numel()
+    if rows is not None:
+        _contig(rows, "rows")
+        assert rows.numel() == n
+    else:
+        assert returns.numel() == n
+    ws = _workspace(dev, "ppg_aux", lib.b200rl_ppg_aux_loss_workspace_bytes(n))
+    rc = lib.b200rl_ppg_aux_loss_f32(
+        _ptr(head_out, f, "head_out"), head_out.stride(0), _ptr(rows, torch.int64, "rows", True),
+        _ptr(old_logits, f, "old_logits"), _ptr(returns, f, "returns"), n, A, float(beta_clone), float(inv_accum),
+        _ptr(dhead, f, "dhead"), dhead.stride(0), _ptr(stats, f, "stats"), ws.data_ptr(), ws.numel(), _stream())
+    _lib.check(rc, "ppg_aux_loss")
+    return stats, dhead
+
+
 # ----------------------------------------------------------------- fp32 layers
 ACT = {None: 0, "none": 0, "relu": 1, "tanh": 2}
 
@@ -579,6 +662,7 @@ class ImpalaCNNBf16(_TensorCorePlan):
     """The tensor-core IMPALA-CNN (procgen frames uint8 [*, 64, 64, 3]); its activation workspaces are keyed by n."""
 
     NET, NAME = "impala", "tensor-core IMPALA-CNN"
+    VALUE_HEADS = 1          # head outputs = A + VALUE_HEADS
 
     def act_tensors(self, n):
         """Named views of the activation workspace of batch size ``n`` (layout: b200rl_impala_bf16_acts_layout)."""
@@ -604,11 +688,11 @@ class ImpalaCNNBf16(_TensorCorePlan):
         if rows is not None:
             _contig(rows, "rows")
         if head_out is None:
-            head_out = torch.empty(n, self.A + 1, dtype=torch.float32, device=self.device)
-        rc = _lib.load().b200rl_impala_bf16_forward(_ptr(obs, torch.uint8, "obs"), _ptr(rows, torch.int64, "rows", True), n,
-                                                    self.A, _ptr(flat_params, torch.float32, "params"), self.packed.data_ptr(),
-                                                    self.acts(n).data_ptr(), _ptr(head_out, torch.float32, "head_out"), _stream())
-        _lib.check(rc, "impala_bf16_forward")
+            head_out = torch.empty(n, self.A + self.VALUE_HEADS, dtype=torch.float32, device=self.device)
+        rc = self._c("forward")(_ptr(obs, torch.uint8, "obs"), _ptr(rows, torch.int64, "rows", True), n,
+                                self.A, _ptr(flat_params, torch.float32, "params"), self.packed.data_ptr(),
+                                self.acts(n).data_ptr(), _ptr(head_out, torch.float32, "head_out"), _stream())
+        _lib.check(rc, f"{self.NET}_bf16_forward")
         return head_out
 
     def backward(self, obs, rows, flat_params, dhead, flat_grads):
@@ -617,11 +701,23 @@ class ImpalaCNNBf16(_TensorCorePlan):
         _contig(dhead, "dhead")
         n = dhead.shape[0]
         ws = self.workspace(n)
-        rc = _lib.load().b200rl_impala_bf16_backward(_ptr(obs, torch.uint8, "obs"), _ptr(rows, torch.int64, "rows", True), n,
-                                                     self.A, _ptr(flat_params, torch.float32, "params"), self.packed.data_ptr(),
-                                                     self.acts(n).data_ptr(), _ptr(dhead, torch.float32, "dhead"),
-                                                     _ptr(flat_grads, torch.float32, "grads"), ws.data_ptr(), ws.numel(), _stream())
-        _lib.check(rc, "impala_bf16_backward")
+        rc = self._c("backward")(_ptr(obs, torch.uint8, "obs"), _ptr(rows, torch.int64, "rows", True), n,
+                                 self.A, _ptr(flat_params, torch.float32, "params"), self.packed.data_ptr(),
+                                 self.acts(n).data_ptr(), _ptr(dhead, torch.float32, "dhead"),
+                                 _ptr(flat_grads, torch.float32, "grads"), ws.data_ptr(), ws.numel(), _stream())
+        _lib.check(rc, f"{self.NET}_bf16_backward")
+
+
+class ImpalaPPGBf16(ImpalaCNNBf16):
+    """The tensor-core IMPALA-CNN of phasic policy gradient (cleanrl/ppg_procgen.py:168-211): the same trunk and activation
+    workspace with the joint head [logits | value | aux_value] (A + 2 outputs); ``backward`` keeps the ``value`` column of
+    ``dhead`` out of the hidden layer's gradient (``critic`` reads ``hidden.detach()``)."""
+
+    NET, NAME, MAX_A, VALUE_HEADS = "impala_ppg", "tensor-core IMPALA-CNN (PPG heads)", 22, 2
+
+    def _c(self, name):
+        # the activation workspace does not depend on the heads: the IMPALA plan's layout serves both
+        return super()._c(name) if not name.startswith("acts_") else getattr(_lib.load(), f"b200rl_impala_bf16_{name}")
 
 
 class LSTMAgentBf16(_TensorCorePlan):

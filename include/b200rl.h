@@ -176,6 +176,39 @@ int b200rl_clip_adam_dyn_f32(float* params, const float* grads, float* exp_avg, 
                              double max_norm, int world_size, float* norm_out,
                              void* workspace, size_t workspace_bytes, void* stream);
 
+/* clip + Adam with per-tensor semantics for a few tensors (torch.optim.Adam keeps one `step` per tensor and, like
+ * clip_grad_norm_, skips a tensor whose grad is None; cleanrl/ppg_procgen.py relies on both for `aux_critic`).
+ * ranges: HOST array of nranges <= 4 element ranges [ranges[2r], ranges[2r+1]) of the flat vector.
+ *   range_step == 0: the ranges are frozen: left out of the clip norm, parameters and both moments untouched;
+ *   range_step >= 1: the ranges are updated with (range_step, range_lr), every other element with (step, lr).
+ * The clip norm is taken over the elements that are updated; max_norm < 0 disables clipping.  4-B aligned buffers;
+ * workspace as b200rl_clip_adam_workspace_bytes(P). */
+int b200rl_clip_adam_ranges_f32(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, int64_t P,
+                                int64_t step, double lr, const int64_t* ranges, int nranges, int64_t range_step,
+                                double range_lr, double beta1, double beta2, double eps, double max_norm,
+                                float* norm_out, void* workspace, size_t workspace_bytes, void* stream);
+/* The same with the step-dependent scalars in DEVICE memory (what a captured CUDA graph replays): step_scalars[0..1] =
+ * b200rl_adam_step_scalars(step, lr) for every element, [2..3] = those of (range_step, range_lr) for the ranges, not read
+ * when `frozen` is non-zero. */
+int b200rl_clip_adam_ranges_dyn_f32(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, int64_t P,
+                                    const float* step_scalars, const int64_t* ranges, int nranges, int frozen,
+                                    double beta1, double beta2, double eps, double max_norm, float* norm_out,
+                                    void* workspace, size_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------ phasic policy gradient: auxiliary loss ------
+ * cleanrl/ppg_procgen.py:449-461 on the joint head output head_out [n][A + 2] = [logits | value | aux_value] (row stride
+ * ld_head): kl_loss = mean KL(Categorical(old_logits) || Categorical(logits)), aux_value_loss = 0.5 mean (aux_value - R)^2,
+ * real_value_loss = 0.5 mean (value - R)^2, loss = (aux_value_loss + beta_clone * kl_loss + real_value_loss) * inv_accum.
+ * Row i reads old_logits[rows[i]][A] and returns[rows[i]] (rows null = i).  Both logit sets are normalised by
+ * log-sum-exp in the kernel; a KL term with p_old == 0 is 0, one with p_new == 0 < p_old is +inf (torch's rule).
+ * Writes dhead [n][A + 2] (row stride ld_dhead) = d loss / d head_out and stats[0..2] = kl_loss, aux_value_loss,
+ * real_value_loss.  1 <= A <= 22, 1 <= n <= 2^22.  Two launches, sums folded in a fixed order (deterministic). */
+size_t b200rl_ppg_aux_loss_workspace_bytes(int64_t n);
+int b200rl_ppg_aux_loss_f32(const float* head_out, int64_t ld_head, const int64_t* rows, const float* old_logits,
+                            const float* returns, int64_t n, int A, double beta_clone, double inv_accum,
+                            float* dhead, int64_t ld_dhead, float* stats, void* workspace, size_t workspace_bytes,
+                            void* stream);
+
 /* ------------------------------------------------ fp32 network layers ------
  * Exact-arithmetic (fp32 FMA, CUDA cores) layers in the reference's own NCHW /
  * [out,in] layouts.  They carry configs 1 and 4 (64-wide MLPs,
@@ -388,6 +421,21 @@ int b200rl_impala_bf16_forward(const uint8_t* obs, const int64_t* rows, int64_t 
 int b200rl_impala_bf16_backward(const uint8_t* obs, const int64_t* rows, int64_t n, int A, const float* params,
                                 const void* packed, void* acts, const float* dhead, float* grads,
                                 void* workspace, size_t workspace_bytes, void* stream);
+
+/* The PPG variant (cleanrl/ppg_procgen.py:168-211): the same trunk, packed weights and activation workspace
+ * (b200rl_impala_bf16_acts_bytes / _acts_layout) with a third head: head_out / dhead are [n][A + 2] =
+ * [logits | value | aux_value], 1 <= A <= 22.  Flat parameters in PPGAgent._param_order: the trunk, then actor.weight,
+ * critic.weight, aux_critic.weight, actor.bias, critic.bias, aux_critic.bias.  `critic` reads a detached hidden layer:
+ * backward uses dhead column A for the critic's own weight and bias only, not for the hidden layer's gradient. */
+int64_t b200rl_impala_ppg_param_count(int A);
+size_t b200rl_impala_ppg_bf16_packed_bytes(int A);
+size_t b200rl_impala_ppg_bf16_workspace_bytes(int64_t n, int A);
+int b200rl_impala_ppg_bf16_pack(const float* params, int A, void* packed, void* stream);
+int b200rl_impala_ppg_bf16_forward(const uint8_t* obs, const int64_t* rows, int64_t n, int A, const float* params,
+                                   const void* packed, void* acts, float* head_out, void* stream);
+int b200rl_impala_ppg_bf16_backward(const uint8_t* obs, const int64_t* rows, int64_t n, int A, const float* params,
+                                    const void* packed, void* acts, const float* dhead, float* grads,
+                                    void* workspace, size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------- recurrent agent, bf16 tensor cores ---
  * cleanrl/ppo_atari_lstm.py:117-160: NatureCNN trunk over ONE grayscale frame, nn.LSTM(512, 128) with the state reset by
