@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""Per-launch times of the convolutions of the bf16 NatureCNN (conv1 forward on the uint8 rollout, the three window
-convolutions conv2 / conv3 forward and conv3 data gradient, and conv21_bwd: the conv2 data gradient fused with the conv1
-weight gradient) at the two batch sizes of a PPO iteration: n = 1024 (a rollout step) and n = 32 768 (a minibatch).
+"""Per-launch times of the convolutions and the fc layer of the bf16 NatureCNN (conv1 forward on the uint8 rollout, the
+three window convolutions conv2 / conv3 forward and conv3 data gradient, conv21_bwd: the conv2 data gradient fused with
+the conv1 weight gradient, and the fc Linear(3136, 512) forward, data gradient and weight gradient) at the two batch
+sizes of a PPO iteration: n = 1024 (a rollout step) and n = 32 768 (a minibatch).
 
     python bench_conv_win.py [--reps R] [--sizes 1024,32768]
 
@@ -20,7 +21,7 @@ import torch
 sys.path.insert(0, str(Path(__file__).resolve().parent))
 from cleanrl_b200 import _lib, build, ops  # noqa: E402
 
-KERNELS = ("conv1_fwd", "conv2_fwd", "conv3_fwd", "conv3_dgrad", "conv21_bwd")
+KERNELS = ("conv1_fwd", "conv2_fwd", "conv3_fwd", "conv3_dgrad", "conv21_bwd", "fc_fwd", "fc_dgrad", "fc_wgrad")
 
 
 def measure(lib, n, reps, dev):

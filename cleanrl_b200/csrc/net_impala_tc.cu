@@ -764,7 +764,7 @@ static int impala_backward(const uint8_t* obs, const int64_t* rows, int64_t n, i
         g.Bw = P + L.pfcd; g.N = 2048; g.out = T(Q.ga); g.ldo = 2048;
         g.mask_bits = reinterpret_cast<const uint32_t*>(ab + Q.mh0);
         ProfScope ps(s, "fc_dgrad", 2.0 * n * 256 * 2048, (double)n * (2048 + 256) * 2 + 256.0 * 2048 * 2);
-        if ((rc = launch_gemm_tma<128, 4>(g, s, "impala/fc_dgrad"))) return rc;
+        if ((rc = launch_gemm_tma<128, 3>(g, s, "impala/fc_dgrad"))) return rc;
     }
     // ---- sequences in reverse; G = gradient of the current stream tensor (ping-pong ga / gb), gy = d(y0)
     bf16* G = T(Q.ga);

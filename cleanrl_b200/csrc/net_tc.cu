@@ -253,7 +253,7 @@ static int trunk_fwd(const NatureLayout& L, const NatureActs& Q, const float* pa
     { ProfScope ps(s, "fc_fwd", 2.0 * n * 512 * 3136, (double)n * (3136 + 512) * 2 + 512.0 * 3136 * 2);
       // small batches (rollout step): narrower N tiles => 4x more CTAs for the same work
       if (n <= 8192) { if ((rc = launch_gemm_tma<64, 6>(p, s, "naturecnn/fc"))) return rc; }
-      else if ((rc = launch_gemm_tma<128, 4>(p, s, "naturecnn/fc"))) return rc; }
+      else if ((rc = launch_gemm_tma<128, 3>(p, s, "naturecnn/fc"))) return rc; }
     return B200RL_OK;
 }
 
@@ -283,7 +283,7 @@ static int trunk_bwd(const NatureLayout& L, const NatureActs& Q, const bf16* P, 
         p.Bw = P + L.wfcdg; p.N = 3136; p.out = act + Q.dact3a; p.out2 = act + Q.dact3b; p.dual_dact3 = 1;
         p.ldo = 3136; p.mask_bits = reinterpret_cast<const uint32_t*>(act + Q.m3);
         { ProfScope ps(s, "fc_dgrad", 2.0 * n * 512 * 3136, (double)n * ((3136 + 512) * 2 + 392) + 512.0 * 3136 * 2);
-          if ((rc = launch_gemm_tma<128, 4>(p, s, "naturecnn/fc_dgrad"))) return rc; }
+          if ((rc = launch_gemm_tma<128, 3>(p, s, "naturecnn/fc_dgrad"))) return rc; }
     }
     WGradWinParams gw;
     WinParams wp;
@@ -364,7 +364,7 @@ static int wide_head_fwd(const NatureLayout& L, const bf16* P, const bf16* hid, 
     gemm_rowmajor(p, hid, n, 8);
     p.Bw = P + L.whf; p.N = L.G; p.bias = reinterpret_cast<const float*>(P + L.hbp);
     p.out_f32 = out; p.ldo = A1; p.ncols_f32 = A1;
-    return launch_gemm_tma<128, 4>(p, s, "wide_heads");
+    return launch_gemm_tma<128, 3>(p, s, "wide_heads");
 }
 
 // wide head backward: dhead [n, A1] fp32 -> bf16 [n, G] (left at the start of wssmall); dW = dhead_bf16^T . hid on wgmma
@@ -387,7 +387,7 @@ static int wide_head_bwd(const NatureLayout& L, const bf16* P, const float* dhea
     p.Bw = P + L.whdg; p.N = 512; p.out = dhid; p.ldo = 512;
     p.mask_bits = hid_bits;
     if (n <= 8192) { if ((rc = launch_gemm_tma<64, 6>(p, s, "wide_heads_dgrad"))) return rc; }
-    else if ((rc = launch_gemm_tma<128, 4>(p, s, "wide_heads_dgrad"))) return rc;
+    else if ((rc = launch_gemm_tma<128, 3>(p, s, "wide_heads_dgrad"))) return rc;
     return B200RL_OK;
 }
 }  // namespace b200rl

@@ -357,8 +357,6 @@ template <int N> __device__ __forceinline__ void bulk_wait() { asm volatile("cp.
 // Per-warpgroup register budgets (setmaxnreg): the kernel launches at 128 registers per thread (512 threads, 1 CTA per
 // SM); the producer warpgroup gives registers back to the weight-gradient warpgroups, whose fragment build then keeps more
 // shared-memory loads in flight.  The data-gradient warpgroup (64 accumulators) keeps the 128 it launched with.
-template <int R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
-template <int R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 constexpr int kC1WRegsProducer = 40, kC21RegsDgrad = 128, kC1WRegsMma = 168;
 static_assert(128 * kC1WRegsProducer + 128 * kC21RegsDgrad + 256 * kC1WRegsMma <= 65536, "register budgets exceed the SM");
 
