@@ -114,6 +114,13 @@ SIGNATURES = {
     "b200rl_lstm_agent_bf16_pack": (_i, [_p, _i, _p, _p]),
     "b200rl_lstm_agent_bf16_forward": (_i, [_p, _p, _i64, _i64, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "b200rl_lstm_agent_bf16_backward": (_i, [_p, _p, _i64, _i64, _i, _p, _p, _p, _p, _p, _p, _p, _sz, _p]),
+    "b200rl_sac_policy_f32": (_i, [_p, _i64, _i64, _i, _p, _i64, _p, _i64, _p]),
+    "b200rl_sac_critic_loss_workspace_bytes": (_sz, [_i64]),
+    "b200rl_sac_critic_loss_f32": (_i, [_p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _p, _p, _p, _i64, _i, _d,
+                                        _p, _p, _i64, _p, _i64, _p, _p, _sz, _p]),
+    "b200rl_sac_actor_loss_workspace_bytes": (_sz, [_i64]),
+    "b200rl_sac_actor_loss_f32": (_i, [_p, _i64, _p, _i64, _p, _i64, _i64, _i, _p, _i, _p, _p, _p, _p, _d, _d, _d, _d,
+                                       _p, _i64, _p, _p, _sz, _p]),
 }
 
 

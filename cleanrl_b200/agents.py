@@ -976,3 +976,215 @@ def dqn_sync_target(q_network, target_network, tau=1.0):
     else:
         t.mul_(1.0 - tau).add_(q, alpha=tau)
     target_network.params_updated()
+
+
+# ------------------------------------------------------------------------ discrete SAC (cleanrl/sac_atari.py)
+def sac_layer_init(layer, bias_const=0.0):
+    """sac_atari.py:102-105: kaiming-normal weight, constant bias."""
+    nn.init.kaiming_normal_(layer.weight)
+    torch.nn.init.constant_(layer.bias, bias_const)
+    return layer
+
+
+class _SACNet(QNetworkAgent):
+    """NatureCNN with an A-wide head under the reference's SAC module names: ``conv`` (Conv2d 0/2/4, ReLU, Flatten),
+    ``fc1`` and the head ``head_name``, initialised by ``sac_layer_init`` in the reference's construction order (each
+    layer's default initialisation, then kaiming: the same generator consumption).  The parameter order is the NatureCNN
+    plan's, so the bf16 plan and the fp32 chain of ``QNetworkAgent`` run it unchanged."""
+
+    head_name = None
+
+    def __init__(self, envs):
+        TensorCoreAgent.__init__(self)
+        obs_shape = tuple(envs.single_observation_space.shape)
+        assert obs_shape == (4, 84, 84), "NatureCNN geometry is 4x84x84"
+        self.conv = nn.Sequential(
+            sac_layer_init(nn.Conv2d(obs_shape[0], 32, kernel_size=8, stride=4)), nn.ReLU(),
+            sac_layer_init(nn.Conv2d(32, 64, kernel_size=4, stride=2)), nn.ReLU(),
+            sac_layer_init(nn.Conv2d(64, 64, kernel_size=3, stride=1)), nn.Flatten())
+        self.fc1 = sac_layer_init(nn.Linear(64 * 7 * 7, 512))
+        setattr(self, self.head_name, sac_layer_init(nn.Linear(512, envs.single_action_space.n)))
+        self.num_actions = int(envs.single_action_space.n)
+
+    def _layers(self, in_div):
+        c = self.conv
+        return nets.Chain([nets.Conv(c[0], "relu", in_div=in_div), nets.Conv(c[2], "relu"), nets.Conv(c[4], "relu"),
+                           nets.Linear(self.fc1, "relu"), nets.Linear(getattr(self, self.head_name), None)])
+
+    def _build_plan(self):
+        self.chain = self._layers(255.0)
+
+
+class SoftQNetwork(_SACNet):
+    """sac_atari.py:112-135: ``forward(x)`` takes frames (0..255) and returns Q-values [n, A]."""
+
+    head_name = "fc_q"
+
+
+class SACActor(_SACNet):
+    """sac_atari.py:138-171.  ``forward(x)`` takes frames already divided by 255 and returns logits; ``get_action(x)``
+    takes frames and returns (action, log_softmax, probs): the action is ``ops.categorical_sample`` on ``noise_fn``'s
+    exponential noise (bit-identical to ``Categorical.sample()`` under the same generator state)."""
+
+    head_name = "fc_logits"
+
+    def _build_plan(self):
+        super()._build_plan()
+        self.chain_scaled = self._layers(1.0)
+
+    def logits(self, frames, rows=None, keep=False):
+        return self.q_values(frames, rows=rows, keep=keep)
+
+    def forward(self, x):
+        self.flat
+        if self.precision == "bf16":
+            # the tensor-core plan consumes frames: x * 255 restores them exactly for inputs that were frames / 255
+            return self.q_values(torch.round(x.float() * 255.0).clamp_(0, 255).to(torch.uint8))
+        return self.chain_scaled.fwd(x.float().contiguous())
+
+    def get_action(self, x):
+        logits = self.logits(x)
+        n, A = logits.shape
+        action, _, _, _ = ops.categorical_sample(logits, self.noise_fn(n, A, logits.device))
+        log_prob, probs = ops.sac_policy(logits)
+        return action, log_prob, probs
+
+
+SAC_ADAM_EPS = 1e-4          # all three optimisers (sac_atari.py:215-223)
+
+
+class SACState:
+    """The device-resident part of a SAC update that is not a network: the temperature (``alpha`` f32[1], and with
+    autotune ``log_alpha`` and its Adam moments), the update count, the logged statistics (``qstats`` =
+    ``ops.SAC_CRITIC_STAT_NAMES``, ``astats`` = ``ops.SAC_ACTOR_STAT_NAMES``) and the scratch of the update.  A bf16
+    update whose noise draw is graph-safe is replayed as one CUDA graph (``use_graph``) up to ``graph_max_batch`` rows:
+    on an H100 the replay saved 0.1-0.6 ms of a 1.5-2 ms update at batch 64 (launch-bound) and was 0.15-0.2 ms slower
+    than eager launches at batch 1024 (bench_sac.py)."""
+
+    use_graph = True
+    graph_max_batch = 256
+
+    def __init__(self, num_actions, device, autotune=True, alpha=0.2, target_entropy_scale=0.89):
+        f32 = torch.float32
+        self.A, self.device, self.autotune = int(num_actions), device, bool(autotune)
+        # -scale * log(1 / A) as the reference evaluates it: fp32 tensor arithmetic (sac_atari.py:226)
+        self.target_entropy = float(-target_entropy_scale * torch.log(1 / torch.tensor(self.A)))
+        self.log_alpha = torch.zeros(1, dtype=f32, device=device)
+        self.alpha = torch.full((1,), 1.0 if autotune else float(alpha), dtype=f32, device=device)
+        self.exp_avg = torch.zeros(1, dtype=f32, device=device)
+        self.exp_avg_sq = torch.zeros(1, dtype=f32, device=device)
+        self.qstats = torch.zeros(4, dtype=f32, device=device)
+        self.astats = torch.zeros(4, dtype=f32, device=device)
+        self.step = 0
+        self._bufs = {}
+        self._graphs = {}
+        self._pool = None
+
+    def buffers(self, B):
+        """Fixed scratch of a batch size: dq1, dq2, dlogits, y, the two noise draws, the loss kernels' workspaces and the
+        graph's input slots."""
+        b = self._bufs.get(B)
+        if b is None:
+            f32, dev, A = torch.float32, self.device, self.A
+            b = {k: torch.zeros(B, A, dtype=f32, device=dev) for k in ("dq1", "dq2", "dl", "noise1", "noise2")}
+            b["y"] = torch.zeros(B, dtype=f32, device=dev)
+            b["rows"] = torch.zeros(B, dtype=torch.int64, device=dev)
+            b["actions"] = torch.zeros(B, dtype=torch.int64, device=dev)
+            b["rewards"] = torch.zeros(B, dtype=f32, device=dev)
+            b["dones"] = torch.zeros(B, dtype=f32, device=dev)
+            b["dyn"] = torch.zeros(6, dtype=f32, device=dev)
+            lib = ops._lib.load()
+            b["ws_critic"] = torch.zeros(lib.b200rl_sac_critic_loss_workspace_bytes(B), dtype=torch.uint8, device=dev)
+            b["ws_actor"] = torch.zeros(lib.b200rl_sac_actor_loss_workspace_bytes(B), dtype=torch.uint8, device=dev)
+            self._bufs[B] = b
+        return b
+
+    def step_scalars(self, step, q_lr, policy_lr):
+        """``adam_step_scalars`` of the q, actor and temperature optimisers (the last uses q_lr, sac_atari.py:223)."""
+        return ops.adam_step_scalars(step, q_lr) + ops.adam_step_scalars(step, policy_lr) + ops.adam_step_scalars(step, q_lr)
+
+
+def _sac_update_body(actor, qf1, qf2, qf1_target, qf2_target, frames, next_frames, rows, next_rows, actions, rewards, dones,
+                     st, buf, dyn, gamma):
+    """Steps 1-4 of sac_atari.py:271-314 on device buffers; every (step, lr) scalar comes from ``dyn`` (device f32[6])."""
+    # 1. soft-Q target: the actor on next_obs (its sample is drawn and not used) and both target networks
+    nl = actor.logits(next_frames, rows=next_rows)
+    actor.draw_noise_into(buf["noise1"])
+    q1t = qf1_target.q_values(next_frames, rows=next_rows)
+    q2t = qf2_target.q_values(next_frames, rows=next_rows)
+    # 2. critic loss, backward and the q optimiser (qf1 and qf2 are separate flat buffers; Adam is elementwise)
+    q1 = qf1.q_values(frames, rows=rows, keep=True)
+    q2 = qf2.q_values(frames, rows=rows, keep=True)
+    ops.sac_critic_loss(nl, q1t, q2t, q1, q2, actions, rewards, dones, gamma, st.alpha, y=buf["y"], dq1=buf["dq1"],
+                        dq2=buf["dq2"], stats=st.qstats, workspace=buf["ws_critic"])
+    qf1.backward(buf["dq1"])
+    qf2.backward(buf["dq2"])
+    for q in (qf1, qf2):
+        f = q.flat
+        ops.clip_adam_dyn(f.flat, f.grad, f.exp_avg, f.exp_avg_sq, dyn[0:2], eps=SAC_ADAM_EPS, max_norm=None)
+        q.params_updated()
+    # 3. actor loss on the post-step Q values (the plans repack before these forwards), backward, actor optimiser;
+    # 4. the temperature step inside the same kernel, after every row has used the old alpha
+    lo = actor.logits(frames, rows=rows, keep=True)
+    actor.draw_noise_into(buf["noise2"])
+    q1 = qf1.q_values(frames, rows=rows)
+    q2 = qf2.q_values(frames, rows=rows)
+    if st.autotune:
+        ops.sac_actor_loss(lo, q1, q2, st.alpha, st.target_entropy, st.log_alpha, st.exp_avg, st.exp_avg_sq, dyn[4:6],
+                           eps=SAC_ADAM_EPS, dlogits=buf["dl"], stats=st.astats, workspace=buf["ws_actor"])
+    else:
+        ops.sac_actor_loss(lo, q1, q2, st.alpha, dlogits=buf["dl"], stats=st.astats, workspace=buf["ws_actor"])
+    actor.backward(buf["dl"])
+    f = actor.flat
+    ops.clip_adam_dyn(f.flat, f.grad, f.exp_avg, f.exp_avg_sq, dyn[2:4], eps=SAC_ADAM_EPS, max_norm=None)
+    actor.params_updated()
+
+
+@torch.no_grad()
+def sac_update(actor, qf1, qf2, qf1_target, qf2_target, ring, batch, state, gamma, q_lr, policy_lr):
+    """One discrete-SAC update (reference: sac_atari.py:271-314) on a ``DeviceReplayRing`` batch: three actor / target
+    forwards on next_obs, the fused soft-Q target + critic loss, both critic backwards and Adam steps, the actor forward
+    and the post-step Q forwards, the fused actor loss + temperature step, the actor backward and Adam step.  Adam
+    eps = 1e-4, no clipping.  Two [B, A] noise draws stand for the reference's two unused ``Categorical.sample()`` calls,
+    so the rollout's actions stay on its generator stream.  Nothing is read back to the host; the statistics are in
+    ``state.qstats`` / ``state.astats``.  bf16 with a graph-safe noise draw and at most ``state.graph_max_batch`` rows
+    replays one CUDA graph per batch size."""
+    B = int(batch["rows"].numel())
+    buf = state.buffers(B)
+    state.step += 1
+    for net in (qf1, qf2, actor):
+        net.flat.step = state.step
+    buf["dyn"].copy_(torch.tensor(state.step_scalars(state.step, q_lr, policy_lr), dtype=torch.float32), non_blocking=True)
+    nets_ = (actor, qf1, qf2, qf1_target, qf2_target)
+    graph = state.use_graph and B <= state.graph_max_batch and all(n.uses_tc_plan() for n in nets_) and actor.graph_friendly
+    args = (ring.frames, ring.next_frames)
+    if not graph:
+        _sac_update_body(actor, qf1, qf2, qf1_target, qf2_target, *args, batch["rows"], batch["next_rows"],
+                         batch["actions"], batch["rewards"], batch["dones"], state, buf, buf["dyn"], gamma)
+        return state
+    same = batch["next_rows"] is batch["rows"]
+    for k in ("rows", "actions", "rewards", "dones"):
+        buf[k].copy_(batch[k].reshape(-1))
+    if not same:
+        buf.setdefault("next_rows", torch.zeros_like(buf["rows"])).copy_(batch["next_rows"])
+    for t in (qf1_target, qf2_target):
+        t._tc_plan()                          # the target repack stays outside the graph
+    key = (B, same, args[0].data_ptr(), args[1].data_ptr())
+    g = state._graphs.get(key)
+    if g is None:
+        for n in (actor, qf1, qf2):
+            n.params_updated()                # the graph starts by packing the online networks' weights
+        g = torch.cuda.CUDAGraph()
+        if state._pool is None:
+            state._pool = torch.cuda.graph_pool_handle()
+        with torch.cuda.graph(g, pool=state._pool):
+            _sac_update_body(actor, qf1, qf2, qf1_target, qf2_target, *args, buf["rows"],
+                             buf["rows"] if same else buf["next_rows"], buf["actions"], buf["rewards"], buf["dones"],
+                             state, buf, buf["dyn"], gamma)
+        for n in nets_:
+            n.pin_workspaces()
+        state._graphs[key] = g
+    g.replay()
+    for n in (actor, qf1, qf2):
+        n.params_updated()                    # no python ran inside the replay: the packed operand copies are stale
+    return state

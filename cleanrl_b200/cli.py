@@ -242,6 +242,29 @@ def c51_atari_args(exp_name="c51_atari"):
     return _make("Args", common + algo + extra)
 
 
+def sac_atari_args(exp_name="sac_atari"):
+    """cleanrl/sac_atari.py:27-74."""
+    common = list(_override(_COMMON, exp_name=exp_name))
+    algo = [
+        ("env_id", str, "BeamRiderNoFrameskip-v4", "the id of the environment"),
+        ("total_timesteps", int, 5000000, "total timesteps of the experiments"),
+        ("buffer_size", int, int(1e6), "the replay memory buffer size"),
+        ("gamma", float, 0.99, "the discount factor gamma"),
+        ("tau", float, 1.0, "target smoothing coefficient (default: 1)"),
+        ("batch_size", int, 64, "the batch size of sample from the reply memory"),
+        ("learning_starts", int, 2e4, "timestep to start learning"),
+        ("policy_lr", float, 3e-4, "the learning rate of the policy network optimizer"),
+        ("q_lr", float, 3e-4, "the learning rate of the Q network network optimizer"),
+        ("update_frequency", int, 4, "the frequency of training updates"),
+        ("target_network_frequency", int, 8000, "the frequency of updates for the target networks"),
+        ("alpha", float, 0.2, "Entropy regularization coefficient."),
+        ("autotune", bool, True, "automatic tuning of the entropy coefficient"),
+        ("target_entropy_scale", float, 0.89, "coefficient for scaling the autotune entropy target"),
+    ]
+    extra = [r for r in _EXTRA if r[0] != "gae_kernel"]
+    return _make("Args", common + algo + extra)
+
+
 def parse(cls, argv=None):
     return tyro.cli(cls, args=argv)
 

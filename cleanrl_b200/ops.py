@@ -1086,3 +1086,84 @@ def c51_loss(logits, next_logits, atoms, actions, rewards, dones, gamma, v_min, 
                                  _ptr(stats, f, "stats"), ws.data_ptr(), ws.numel(), _stream())
     _lib.check(rc, "c51_loss")
     return stats, dlogits
+
+
+# ------------------------------------------------------------------------ SAC
+SAC_CRITIC_STAT_NAMES = ("qf1_values", "qf2_values", "qf1_loss", "qf2_loss")
+SAC_ACTOR_STAT_NAMES = ("actor_loss", "alpha_loss", "alpha", "log_alpha")
+
+
+def sac_policy(logits):
+    """Actor.get_action's (log_softmax, probs) of the logits [n, A] (reference: sac_atari.py:164-170)."""
+    lib = _lib.load()
+    n, A = logits.shape
+    assert logits.stride(1) == 1
+    f = torch.float32
+    logp = torch.empty(n, A, dtype=f, device=logits.device)
+    probs = torch.empty(n, A, dtype=f, device=logits.device)
+    rc = lib.b200rl_sac_policy_f32(_ptr(logits, f, "logits"), logits.stride(0), n, A, _ptr(logp, f, "logp"), A,
+                                   _ptr(probs, f, "probs"), A, _stream())
+    _lib.check(rc, "sac_policy")
+    return logp, probs
+
+
+def sac_critic_loss(next_logits, q1_target, q2_target, q1, q2, actions, rewards, dones, gamma, alpha, y=None, dq1=None,
+                    dq2=None, stats=None, workspace=None):
+    """Soft-Q target, both critic losses and dL/dq1, dL/dq2 (reference: sac_atari.py:274-290); ``alpha`` is a device
+    f32 [1].  ``workspace``: a caller-owned uint8 buffer (what a captured CUDA graph keeps), else a shared one.  Returns (stats f32[4] = qf1_values, qf2_values, qf1_loss, qf2_loss; y [B]; dq1 [B, A]; dq2 [B, A])."""
+    lib = _lib.load()
+    B, A = q1.shape
+    for n_, t in (("next_logits", next_logits), ("q1_target", q1_target), ("q2_target", q2_target), ("q2", q2)):
+        if tuple(t.shape) != (B, A):
+            raise ValueError(f"sac_critic_loss: {n_} shape {tuple(t.shape)} != {(B, A)}")
+    for t in (next_logits, q1_target, q2_target, q1, q2):
+        assert t.stride(1) == 1
+    f = torch.float32
+    dev = q1.device
+    y = torch.empty(B, dtype=f, device=dev) if y is None else y
+    dq1 = torch.empty(B, A, dtype=f, device=dev) if dq1 is None else dq1
+    dq2 = torch.empty(B, A, dtype=f, device=dev) if dq2 is None else dq2
+    stats = torch.zeros(4, dtype=f, device=dev) if stats is None else stats
+    actions = _contig(actions.reshape(-1), "actions")
+    if actions.dtype != torch.int64:
+        actions = actions.long()
+    ws = workspace if workspace is not None else _workspace(dev, "sac_critic", lib.b200rl_sac_critic_loss_workspace_bytes(B))
+    rc = lib.b200rl_sac_critic_loss_f32(
+        _ptr(next_logits, f, "next_logits"), next_logits.stride(0), _ptr(q1_target, f, "q1_target"), q1_target.stride(0),
+        _ptr(q2_target, f, "q2_target"), q2_target.stride(0), _ptr(q1, f, "q1"), q1.stride(0), _ptr(q2, f, "q2"),
+        q2.stride(0), _ptr(actions, torch.int64, "actions"), _ptr(_contig(rewards.reshape(-1), "rewards"), f, "rewards"),
+        _ptr(_contig(dones.reshape(-1), "dones"), f, "dones"), _ptr(alpha, f, "alpha"), B, A, float(gamma),
+        _ptr(y, f, "y"), _ptr(dq1, f, "dq1"), dq1.stride(0), _ptr(dq2, f, "dq2"), dq2.stride(0), _ptr(stats, f, "stats"),
+        ws.data_ptr(), ws.numel(), _stream())
+    _lib.check(rc, "sac_critic_loss")
+    return stats, y, dq1, dq2
+
+
+def sac_actor_loss(logits, q1, q2, alpha, target_entropy=0.0, log_alpha=None, exp_avg=None, exp_avg_sq=None,
+                   step_scalars=None, eps=1e-4, dlogits=None, stats=None, workspace=None):
+    """Actor loss + dL/dlogits (reference: sac_atari.py:293-305) and, when ``log_alpha`` is given (autotune), the
+    temperature loss, one Adam step of ``log_alpha`` (moments ``exp_avg`` / ``exp_avg_sq``, ``step_scalars`` f32[2] from
+    ``adam_step_scalars``, all device memory) and ``alpha = exp(log_alpha)`` (sac_atari.py:307-314).  ``workspace`` as
+    in ``sac_critic_loss``.
+    Returns (stats f32[4] = actor_loss, alpha_loss, alpha, log_alpha; dlogits [B, A])."""
+    lib = _lib.load()
+    B, A = logits.shape
+    for n_, t in (("q1", q1), ("q2", q2)):
+        if tuple(t.shape) != (B, A):
+            raise ValueError(f"sac_actor_loss: {n_} shape {tuple(t.shape)} != {(B, A)}")
+    for t in (logits, q1, q2):
+        assert t.stride(1) == 1
+    f = torch.float32
+    dev = logits.device
+    dlogits = torch.empty(B, A, dtype=f, device=dev) if dlogits is None else dlogits
+    stats = torch.zeros(4, dtype=f, device=dev) if stats is None else stats
+    autotune = log_alpha is not None
+    ws = workspace if workspace is not None else _workspace(dev, "sac_actor", lib.b200rl_sac_actor_loss_workspace_bytes(B))
+    rc = lib.b200rl_sac_actor_loss_f32(
+        _ptr(logits, f, "logits"), logits.stride(0), _ptr(q1, f, "q1"), q1.stride(0), _ptr(q2, f, "q2"), q2.stride(0), B, A,
+        _ptr(alpha, f, "alpha"), int(autotune), _ptr(log_alpha, f, "log_alpha", True), _ptr(exp_avg, f, "exp_avg", True),
+        _ptr(exp_avg_sq, f, "exp_avg_sq", True), _ptr(step_scalars, f, "step_scalars", True), float(target_entropy),
+        0.9, 0.999, float(eps), _ptr(dlogits, f, "dlogits"), dlogits.stride(0), _ptr(stats, f, "stats"), ws.data_ptr(),
+        ws.numel(), _stream())
+    _lib.check(rc, "sac_actor_loss")
+    return stats, dlogits

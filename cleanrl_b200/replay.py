@@ -8,6 +8,11 @@ Replaces the host-side numpy ``ReplayBuffer`` of cleanrl_utils/buffers.py:250-43
 * ``sample`` draws the SAME index stream from numpy's global RNG (buffers.py:390-399: ``randint(1, size) + pos``
   when full, ``randint(0, pos)`` otherwise, then ``randint(0, n_envs)``) but returns ROW INDICES into the ring:
   the network kernels gather the frames themselves (no 2 x 231 MB host fancy-index + H2D per batch of 8192).
+
+``optimize_memory_usage=False`` is the layout sac_atari.py uses (buffers.py:301-303, 358-363, 217-225, 397-415): a
+second device ring ``next_observations`` written from ``real_next_obs``, ``randint(0, size if full else pos)`` then the
+env index, and ``sample`` rows that index both ``frames`` and ``next_frames``.  Both uint8 rings live in HBM (56.4 GB at
+``buffer_size = 1e6``); a ring that does not fit in free device memory is an error at construction.
 """
 from __future__ import annotations
 
@@ -16,12 +21,22 @@ import torch
 
 
 class DeviceReplayRing:
-    def __init__(self, buffer_size, obs_shape, n_envs, device):
+    def __init__(self, buffer_size, obs_shape, n_envs, device, optimize_memory_usage=True):
         self.buffer_size = max(int(buffer_size) // int(n_envs), 1)     # buffers.py:300 (size per env)
         self.n_envs = int(n_envs)
         self.device = device
         self.obs_shape = tuple(obs_shape)
-        self.observations = torch.zeros((self.buffer_size, self.n_envs) + self.obs_shape, dtype=torch.uint8, device=device)
+        self.optimize_memory_usage = bool(optimize_memory_usage)
+        shape = (self.buffer_size, self.n_envs) + self.obs_shape
+        if not self.optimize_memory_usage:
+            need = 2 * int(np.prod(shape))
+            free = torch.cuda.mem_get_info(device)[0] if torch.device(device).type == "cuda" else need
+            if need > free:
+                raise RuntimeError(f"the replay buffer (observations and next_observations, uint8) needs {need / 1e9:.1f} GB "
+                                   f"of device memory, {free / 1e9:.1f} GB are free: lower --buffer-size (it is not "
+                                   "spilled to the host)")
+        self.observations = torch.zeros(shape, dtype=torch.uint8, device=device)
+        self.next_observations = None if self.optimize_memory_usage else torch.zeros(shape, dtype=torch.uint8, device=device)
         self.actions = torch.zeros((self.buffer_size, self.n_envs), dtype=torch.int64, device=device)
         self.rewards = torch.zeros((self.buffer_size, self.n_envs), dtype=torch.float32, device=device)
         self.dones = torch.zeros((self.buffer_size, self.n_envs), dtype=torch.float32, device=device)
@@ -36,12 +51,20 @@ class DeviceReplayRing:
         """The ring as a flat list of frames [size * n_envs, 4, 84, 84] (row = slot * n_envs + env)."""
         return self.observations.view((self.buffer_size * self.n_envs,) + self.obs_shape)
 
+    @property
+    def next_frames(self):
+        """The frames ``next_rows`` index: ``frames`` itself, or the ``next_observations`` ring."""
+        if self.optimize_memory_usage:
+            return self.frames
+        return self.next_observations.view((self.buffer_size * self.n_envs,) + self.obs_shape)
+
     def add(self, obs, next_obs, action, reward, done, infos=None):
         """buffers.py:339-375."""
         dev = self.device
         self.observations[self.pos].copy_(torch.from_numpy(np.ascontiguousarray(obs)).to(torch.uint8), non_blocking=False)
-        self.observations[(self.pos + 1) % self.buffer_size].copy_(
-            torch.from_numpy(np.ascontiguousarray(next_obs)).to(torch.uint8), non_blocking=False)
+        nxt = self.observations[(self.pos + 1) % self.buffer_size] if self.optimize_memory_usage else \
+            self.next_observations[self.pos]
+        nxt.copy_(torch.from_numpy(np.ascontiguousarray(next_obs)).to(torch.uint8), non_blocking=False)
         self.actions[self.pos].copy_(torch.as_tensor(np.asarray(action).reshape(self.n_envs), dtype=torch.int64))
         self.rewards[self.pos].copy_(torch.as_tensor(np.asarray(reward, dtype=np.float32).reshape(self.n_envs)))
         self.dones[self.pos].copy_(torch.as_tensor(np.asarray(done, dtype=np.float32).reshape(self.n_envs)))
@@ -51,8 +74,10 @@ class DeviceReplayRing:
             self.pos = 0
 
     def sample_indices(self, batch_size):
-        """Host index draw, bit-identical to buffers.py:390-399 (numpy global RNG)."""
-        if self.full:
+        """Host index draw, bit-identical to buffers.py:390-399 / 217-225 (numpy global RNG)."""
+        if not self.optimize_memory_usage:
+            batch_inds = np.random.randint(0, self.buffer_size if self.full else self.pos, size=batch_size)
+        elif self.full:
             batch_inds = (np.random.randint(1, self.buffer_size, size=batch_size) + self.pos) % self.buffer_size
         else:
             batch_inds = np.random.randint(0, self.pos, size=batch_size)
@@ -60,10 +85,14 @@ class DeviceReplayRing:
         return batch_inds, env_indices
 
     def sample(self, batch_size):
-        """Returns dict(rows, next_rows: int64 device row indices into ``frames``; actions [B], rewards [B], dones [B])."""
+        """Returns dict(rows: int64 device row indices into ``frames``, next_rows: into ``next_frames``; actions [B],
+        rewards [B], dones [B])."""
         bi, ei = self.sample_indices(batch_size)
         rows = torch.from_numpy(bi * self.n_envs + ei).to(self.device)
-        next_rows = torch.from_numpy(((bi + 1) % self.buffer_size) * self.n_envs + ei).to(self.device)
+        if self.optimize_memory_usage:
+            next_rows = torch.from_numpy(((bi + 1) % self.buffer_size) * self.n_envs + ei).to(self.device)
+        else:
+            next_rows = rows
         return {"rows": rows, "next_rows": next_rows,
                 "actions": self.actions.view(-1)[rows], "rewards": self.rewards.view(-1)[rows],
                 "dones": self.dones.view(-1)[rows], "batch_inds": bi, "env_indices": ei}

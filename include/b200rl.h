@@ -534,6 +534,39 @@ int b200rl_c51_loss_f32(const float* logits, int64_t ld, const float* next_logit
                         float* dlogits, int64_t ld_d, float* stats,
                         void* workspace, size_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------- discrete soft actor-critic ---
+ * cleanrl/sac_atari.py on [n, A] head outputs (row strides ld*), 2 <= A <= 32.  The temperature is device memory:
+ * alpha f32 [1]; with autotune also log_alpha f32 [1] and its Adam moments exp_avg, exp_avg_sq f32 [1].
+ *
+ * b200rl_sac_policy_f32: Actor.get_action's log_softmax (logp) and Categorical probabilities (probs) of the logits; either
+ *   output may be NULL.  The sampled action is b200rl_categorical_sample_f32 on the same logits.
+ * b200rl_sac_critic_loss_f32: the soft-Q target and both critic losses (sac_atari.py:274-290) in one pass:
+ *   y = r + ((1 - d) * gamma) * sum_a p'(a) (min(q1t, q2t)(a) - alpha * logp'(a)), p' / logp' from the actor's logits on
+ *   next_obs (next_logits); dq_k [B, A] = 2 (q_k[a] - y) / B at the taken action, 0 elsewhere; y f32 [B] may be NULL.
+ *   stats f32 [4] = mean q1[a], mean q2[a], qf1_loss, qf2_loss.
+ * b200rl_sac_actor_loss_f32: the actor loss and its gradient (sac_atari.py:293-305): f = alpha * logp - min(q1, q2),
+ *   actor_loss = mean over B x A of p f, dlogits [B, A] = p (f - sum_a p f) / (B A).  With autotune (sac_atari.py:307-314)
+ *   alpha_loss = mean(p (-exp(log_alpha) (logp + target_entropy))) and one Adam step of log_alpha (beta1, beta2, eps,
+ *   step_scalars f32 [2] as b200rl_adam_step_scalars in device memory), then alpha = exp(log_alpha); every block reads the
+ *   old alpha before it is rewritten.  stats f32 [4] = actor_loss, alpha_loss (0 without autotune), alpha, log_alpha.
+ * Fixed-order reductions: bitwise reproducible.  workspace: the matching *_workspace_bytes(B), 16-byte aligned.
+ */
+int b200rl_sac_policy_f32(const float* logits, int64_t ld, int64_t n, int A, float* logp, int64_t ld_logp,
+                          float* probs, int64_t ld_probs, void* stream);
+size_t b200rl_sac_critic_loss_workspace_bytes(int64_t B);
+int b200rl_sac_critic_loss_f32(const float* next_logits, int64_t ld_next, const float* q1_target, int64_t ld_q1t,
+                               const float* q2_target, int64_t ld_q2t, const float* q1, int64_t ld_q1, const float* q2,
+                               int64_t ld_q2, const int64_t* actions, const float* rewards, const float* dones,
+                               const float* alpha, int64_t B, int A, double gamma, float* y, float* dq1, int64_t ld_dq1,
+                               float* dq2, int64_t ld_dq2, float* stats, void* workspace, size_t workspace_bytes,
+                               void* stream);
+size_t b200rl_sac_actor_loss_workspace_bytes(int64_t B);
+int b200rl_sac_actor_loss_f32(const float* logits, int64_t ld, const float* q1, int64_t ld_q1, const float* q2,
+                              int64_t ld_q2, int64_t B, int A, float* alpha, int autotune, float* log_alpha,
+                              float* exp_avg, float* exp_avg_sq, const float* step_scalars, double target_entropy,
+                              double beta1, double beta2, double eps, float* dlogits, int64_t ld_d, float* stats,
+                              void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
