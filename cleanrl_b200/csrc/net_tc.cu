@@ -238,14 +238,17 @@ static int trunk_fwd(const NatureLayout& L, const NatureActs& Q, const float* pa
     win_defaults(wp); win_conv2(wp, act + Q.act1, n);
     wp.Bw = P + L.w2f; wp.N = 64; wp.vH = 9; wp.vW = 9; wp.out_mode = WOUT_DENSE; wp.out = act + Q.act2;
     wp.bias = params + L.c2b; wp.relu = 1; wp.mask_out = reinterpret_cast<uint32_t*>(act + Q.m2);
+    // small batches (rollout step): 64-position tiles => twice the tiles per CTA and a shorter first window
     { ProfScope ps(s, "conv2_fwd", 2.0 * n * 81 * 64 * 512, (double)n * ((12800 + 5184) * 2 + 648));
-      if ((rc = launch_conv_win_t<128, 2, 2, 4>(wp, s, "naturecnn/conv2"))) return rc; }
+      if (n <= 8192) { if ((rc = launch_conv_win_t<64, 2, 6, 4>(wp, s, "naturecnn/conv2"))) return rc; }
+      else if ((rc = launch_conv_win_t<128, 2, 2, 4>(wp, s, "naturecnn/conv2"))) return rc; }
     // conv3: 3x3 window conv -> act3 [n,7,7,64]
     win_defaults(wp); win_conv3(wp, act + Q.act2, n);
     wp.Bw = P + L.w3f; wp.N = 64; wp.vH = 7; wp.vW = 7; wp.out_mode = WOUT_DENSE; wp.out = act + Q.act3;
     wp.bias = params + L.c3b; wp.relu = 1; wp.mask_out = reinterpret_cast<uint32_t*>(act + Q.m3);
     { ProfScope ps(s, "conv3_fwd", 2.0 * n * 49 * 64 * 576, (double)n * ((5184 + 3136) * 2 + 392));
-      if ((rc = launch_conv_win_t<128, 1, 4, 9>(wp, s, "naturecnn/conv3"))) return rc; }
+      if (n <= 8192) { if ((rc = launch_conv_win_t<64, 1, 8, 9>(wp, s, "naturecnn/conv3"))) return rc; }
+      else if ((rc = launch_conv_win_t<128, 1, 4, 9>(wp, s, "naturecnn/conv3"))) return rc; }
     // fc -> hidden [n,512]
     gemm_rowmajor(p, act + Q.act3, n, 49);
     p.Bw = P + L.wfcf; p.N = 512; p.out = act + Q.hid; p.ldo = 512; p.bias = params + L.fcb; p.relu = 1;
@@ -418,7 +421,7 @@ extern "C" int b200rl_frames_to_s2d_u8(const uint8_t* obs, const int64_t* rows, 
     B200RL_REQUIRE(n <= (int64_t)1 << 28, "frames_to_s2d_u8: n too large");
     cudaStream_t s = (cudaStream_t)stream;
     ProfScope ps(s, "frames_to_s2d", 0, (double)n * (28224 + 28224 + 28672));
-    tc_frames_to_s2d_u8<<<(unsigned)(n * 4), 256, 0, s>>>(obs, rows, n, out_rm, out_cm);
+    tc_frames_to_s2d_u8<<<(unsigned)n, kS2dThreads, 0, s>>>(obs, rows, n, out_rm, out_cm);
     return check_launch("frames_to_s2d_u8");
 }
 

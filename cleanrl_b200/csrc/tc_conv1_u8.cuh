@@ -46,39 +46,55 @@ __device__ __forceinline__ uint32_t img64_off(int r, int c) { return (uint32_t)(
 // ------------------------------------------------------------------------------------ frame conversion (once per env step)
 // uint8 frames [n,4,84,84] (NCHW, as the env delivers them) -> row-major u8 [n,441,64] and channel-major u8 [n,64,448]
 // space-to-depth(4) pixels: channel = c*16 + sy*4 + sx of source pixel (4Y+sy, 4X+sx), grid row = Y*21 + X.
-// One block per (frame, colour plane c): the 84x84 plane is staged in shared memory (coalesced 16-byte reads).
-__global__ void __launch_bounds__(256) tc_frames_to_s2d_u8(const uint8_t* __restrict__ obs, const int64_t* __restrict__ rows, int64_t n,
-                                                           uint8_t* __restrict__ out_rm, uint8_t* __restrict__ out_cm) {
-    __shared__ __align__(16) uint8_t plane[7056];
-    const int64_t i = blockIdx.x >> 2;
-    const int c = blockIdx.x & 3;
+// One block per frame: the whole 4 x 84 x 84 frame is staged in shared memory with 16-byte loads (7 per thread, all in
+// flight before the barrier).  Both outputs are then written as whole lines: a 32-bit word of a plane row holds the 4
+// sx pixels of one position, so a row-major position is 16 such words (4 consecutive threads store its 64 bytes), and
+// 4 positions x 4 sx of a channel-major (c, sy) group are a 4 x 4 byte transpose of 4 words (one PRMT pair per output
+// word, each stored with the neighbouring threads' words of the same channel row).
+constexpr int kS2dThreads = 256;
+__global__ void __launch_bounds__(kS2dThreads) tc_frames_to_s2d_u8(const uint8_t* __restrict__ obs, const int64_t* __restrict__ rows,
+                                                                   int64_t n, uint8_t* __restrict__ out_rm, uint8_t* __restrict__ out_cm) {
+    __shared__ __align__(16) uint8_t frame[28224];
+    const int64_t i = blockIdx.x;
     const int64_t img = rows ? rows[i] : i;
-    const int4* src = reinterpret_cast<const int4*>(obs + img * 28224 + c * 7056);
-    for (int t = threadIdx.x; t < 441; t += 256) reinterpret_cast<int4*>(plane)[t] = __ldg(src + t);
+    const int4* src = reinterpret_cast<const int4*>(obs + img * 28224);
+#pragma unroll
+    for (int k = 0; k < 7; ++k) {
+        const int t = threadIdx.x + k * kS2dThreads;
+        if (t < 1764) reinterpret_cast<int4*>(frame)[t] = __ldg(src + t);
+    }
     __syncthreads();
-    // row-major: 16 bytes (4 rows of 4 pixels) per grid position
-    for (int pos = threadIdx.x; pos < 441; pos += 256) {
-        const int Y = pos / 21, X = pos - Y * 21;
-        const uint8_t* p = plane + (Y * 4) * 84 + X * 4;
+    // row-major [441][64]: 16-byte chunk c of position pos = rows 4Y .. 4Y+3 of plane c at column 4X
+    int4* rm = reinterpret_cast<int4*>(out_rm + i * 441 * 64);
+    for (int t = threadIdx.x; t < 441 * 4; t += kS2dThreads) {
+        const int pos = t >> 2, c = t & 3;
+        const int Y = (pos * 3121) >> 16, X = pos - Y * 21;                   // pos / 21 for pos < 512
+        const uint8_t* p = frame + c * 7056 + (Y * 4) * 84 + X * 4;
         int4 v;
         v.x = *reinterpret_cast<const int*>(p); v.y = *reinterpret_cast<const int*>(p + 84);
         v.z = *reinterpret_cast<const int*>(p + 168); v.w = *reinterpret_cast<const int*>(p + 252);
-        *reinterpret_cast<int4*>(out_rm + (i * 441 + pos) * 64 + c * 16) = v;
+        rm[t] = v;
     }
-    // channel-major: channel (sy, sx) of this plane, 4 consecutive grid rows per 32-bit store (448-byte rows, zero tail)
-    for (int t = threadIdx.x; t < 16 * 112; t += 256) {
-        const int ch = t / 112, q = t - ch * 112;
-        const int sy = ch >> 2, sx = ch & 3;
-        uint32_t w = 0;
+    // channel-major [64][448]: group (c, sy, q) = positions 4q .. 4q+3 of the 4 channels c*16 + sy*4 + sx (zero past 441)
+    uint8_t* cm = out_cm + i * 64 * 448;
+    for (int t = threadIdx.x; t < 16 * 112; t += kS2dThreads) {
+        const int g = t / 112, q = t - g * 112;                                // g = c * 4 + sy
+        const uint8_t* prow = frame + (g >> 2) * 7056 + (g & 3) * 84;
+        uint32_t w[4];
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
-            const int pos = q * 4 + e;
-            if (pos < 441) {
-                const int Y = pos / 21, X = pos - Y * 21;
-                w |= (uint32_t)plane[(Y * 4 + sy) * 84 + X * 4 + sx] << (8 * e);
-            }
+            const int pos = q * 4 + e, pc = pos < 441 ? pos : 440;           // the tail reads a valid word, stores 0
+            const int Y = (pc * 3121) >> 16, X = pc - Y * 21;
+            const uint32_t v = *reinterpret_cast<const uint32_t*>(prow + (Y * 4) * 84 + X * 4);
+            w[e] = pos < 441 ? v : 0u;
         }
-        *reinterpret_cast<uint32_t*>(out_cm + (i * 64 + c * 16 + ch) * 448 + q * 4) = w;
+        const uint32_t lo01 = __byte_perm(w[0], w[1], 0x5140), hi01 = __byte_perm(w[0], w[1], 0x7362);
+        const uint32_t lo23 = __byte_perm(w[2], w[3], 0x5140), hi23 = __byte_perm(w[2], w[3], 0x7362);
+        uint32_t* dst = reinterpret_cast<uint32_t*>(cm + (g * 4) * 448) + q;
+        dst[0] = __byte_perm(lo01, lo23, 0x5410);                             // sx = 0: byte e = position 4q + e
+        dst[112] = __byte_perm(lo01, lo23, 0x7632);
+        dst[224] = __byte_perm(hi01, hi23, 0x5410);
+        dst[336] = __byte_perm(hi01, hi23, 0x7632);
     }
 }
 
@@ -137,12 +153,13 @@ struct Conv1U8Params {
 // of the tile, both parities, and the epilogue straight from the accumulator fragments.
 constexpr int kConv1I8Threads = 384;
 template <int STAGES>
-__global__ void __launch_bounds__(kConv1I8Threads, 1) tc_conv1_i8(const __grid_constant__ CUtensorMap tmA, const Conv1U8Params p, int total_tiles) {
+__global__ void __launch_bounds__(kConv1I8Threads, 1) tc_conv1_i8(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
+                                                                   const Conv1U8Params p, int total_tiles) {
     constexpr int BN = 64, WR = 144, NTAPS = 4;
     constexpr int STAGE_BYTES = WR * 128;           // 18432 = 18 x 1024
     constexpr int B_CHUNK = BN * 64;                // one tap of the limb image: 64 rows x 64 B (SWIZZLE_64B)
     extern __shared__ uint8_t smem_raw[];
-    __shared__ uint64_t full_bar[STAGES], empty_bar[STAGES];
+    __shared__ uint64_t full_bar[STAGES], empty_bar[STAGES], w_bar;
     __shared__ __align__(16) float s_sc[32], s_bias[32];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     const int tid = threadIdx.x, warp = tid >> 5;
@@ -151,17 +168,12 @@ __global__ void __launch_bounds__(kConv1I8Threads, 1) tc_conv1_i8(const __grid_c
 
     if (tid == 0) {
         for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }   // 8 consumer warps
+        mbar_init(&w_bar, 1);
         fence_barrier_init();
         tma_prefetch_desc(&tmA);
-    }
-    for (int idx = tid; idx < NTAPS * BN * 4; idx += blockDim.x) {          // 16-byte chunks of the limb image
-        const int c16 = idx & 3;
-        const int t = (idx >> 2) & 3;
-        const int r = idx >> 4;
-        *reinterpret_cast<int4*>(sW + t * B_CHUNK + img64_off(r, c16)) = ldg16(p.limbs + r * 256 + t * 64 + c16 * 16);
+        tma_prefetch_desc(&tmW);
     }
     if (tid < 32) { s_sc[tid] = p.sc[32 + tid]; s_bias[tid] = p.bias[tid]; }      // sc[32 + co] = s_co / 2^14 / 255
-    fence_proxy_async_smem();
     __syncthreads();
     // a tile = 128 pair rows = 256 grid positions; 2 tiles per image (441 positions used)
     const int tile_begin = (int)(((int64_t)total_tiles * blockIdx.x) / gridDim.x);
@@ -187,6 +199,11 @@ __global__ void __launch_bounds__(kConv1I8Threads, 1) tc_conv1_i8(const __grid_c
                 if (q >= (uint32_t)STAGES) mbar_wait(&empty_bar[s], ((q / STAGES) - 1) & 1);
                 mbar_arrive_expect_tx(&full_bar[s], (uint32_t)STAGE_BYTES);
                 tma_load_3d(smem_u32(sRing + (size_t)s * STAGE_BYTES), &tmA, 0, (tile & 1) * 128, z, &full_bar[s]);
+                if (q == 0) {       // the limb image, one [64 rows x 64 B] SWIZZLE_64B box per tap, behind the first window
+                    mbar_arrive_expect_tx(&w_bar, (uint32_t)(NTAPS * B_CHUNK));
+#pragma unroll
+                    for (int t = 0; t < NTAPS; ++t) tma_load_3d(smem_u32(sW + t * B_CHUNK), &tmW, t * 64, 0, 0, &w_bar);
+                }
             }
         }
     } else if (warp >= 4) {
@@ -201,6 +218,7 @@ __global__ void __launch_bounds__(kConv1I8Threads, 1) tc_conv1_i8(const __grid_c
         for (int e = 0; e < 2; ++e)
 #pragma unroll
             for (int c = 0; c < 32; ++c) acc[e][c] = 0;
+        if (tile_begin < tile_end) mbar_wait(&w_bar, 0);
         for (int tile = tile_begin; tile < tile_end; ++tile) {
             const uint32_t q = (uint32_t)(tile - tile_begin), s = q % STAGES;
             mbar_wait(&full_bar[s], (q / STAGES) & 1);
@@ -635,15 +653,18 @@ static int launch_conv1_i8(const Conv1U8Params& p, const void* frames_rm, cudaSt
     const int total = p.n * 2;                     // 2 tiles of 128 pair rows (256 grid positions) per image (441 used)
     int grid = num_sms();
     if (grid > total) grid = total;
-    CUtensorMap tmA;
+    CUtensorMap tmA, tmW;
     memset(&tmA, 0, sizeof(tmA));
+    memset(&tmW, 0, sizeof(tmW));
     // the row-major image [441][64 B] viewed as 221 pair rows of 128 B (image stride 28 224 B = 220.5 rows: the second
     // half of row 220 belongs to the next image and only ever feeds invalid positions); SWIZZLE_128B boxes of 144 rows
     int rc = make_tmap_pairs_u8(&tmA, frames_rm, p.n_images, what);
     if (rc) return rc;
+    // the limbs [64 rows][4 taps x 64 B]: one SWIZZLE_64B box [64 rows][64 B] per tap
+    if ((rc = make_tmap_3d_u8(&tmW, p.limbs, 1, 64, 256, 256, 64, 64, what))) return rc;
     static SmemAttrCache attr;
     if ((rc = attr.ensure(tc_conv1_i8<STAGES>, smem, what))) return rc;
-    tc_conv1_i8<STAGES><<<grid, kConv1I8Threads, smem, s>>>(tmA, p, total);
+    tc_conv1_i8<STAGES><<<grid, kConv1I8Threads, smem, s>>>(tmA, tmW, p, total);
     return check_launch(what);
 }
 

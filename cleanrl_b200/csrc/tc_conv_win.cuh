@@ -46,20 +46,25 @@ struct WinParams {
 // requires); warpgroups 1 and 2 each run wgmma on 64 rows of every 128-row tile (accumulators in registers), hand the
 // accumulators to a row-major shared-memory tile and run the epilogue with one thread per row (a second thread per row
 // takes the odd 32-column groups).
+// The resident weight image arrives by TMA on a barrier of its own, issued right behind the first window: a CTA's first
+// MMAs wait for both copies in flight together, not for every thread's share of a load of the whole image first.  At
+// the rollout's n = 1024 a CTA runs only a few tiles, so that wait is a visible part of the launch.
 constexpr int kConvWinThreads = 384;
 template <int BN>
 __host__ __device__ constexpr size_t conv_win_acc_bytes() { return (size_t)128 * (BN + 4) * sizeof(float); }
 template <int BN, int CPR, int STAGES, int NTAPS>
-__global__ void __launch_bounds__(kConvWinThreads, 1) tc_conv_win(const __grid_constant__ CUtensorMap tmA, const WinParams p,
+__global__ void __launch_bounds__(kConvWinThreads, 1) tc_conv_win(const __grid_constant__ CUtensorMap tmA,
+                                                                  const __grid_constant__ CUtensorMap tmW, const WinParams p,
                                                                   int total_tiles) {
     constexpr int B_CHUNK = BN * 128;
     constexpr int LDA = BN + 4;                          // fp32 accumulator tile row pitch (conflict-free row reads)
     extern __shared__ uint8_t smem_raw[];
-    __shared__ uint64_t full_bar[STAGES], empty_bar[STAGES];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    __shared__ uint64_t full_bar[STAGES], empty_bar[STAGES], w_bar;
+    // aligned by an offset from smem_raw (not through an integer): the accumulator tile's accesses stay shared-memory
+    // instructions instead of generic ones
+    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     const int tid = threadIdx.x, warp = tid >> 5;
     const int nchunks = p.ntaps * CPR;
-    const int K = nchunks * 64;
     const int IMG = p.WR * 128;                 // one 64-channel column image of the window
     const int STAGE_BYTES = IMG * CPR;
     uint8_t* sW = smem;
@@ -68,18 +73,11 @@ __global__ void __launch_bounds__(kConvWinThreads, 1) tc_conv_win(const __grid_c
 
     if (tid == 0) {
         for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }   // 8 consumer warps
+        mbar_init(&w_bar, 1);
         fence_barrier_init();
         tma_prefetch_desc(&tmA);
+        tma_prefetch_desc(&tmW);
     }
-    for (int idx = tid; idx < nchunks * BN * 8; idx += blockDim.x) {
-        const int c16 = idx & 7;
-        int t = idx >> 3;
-        const int r = t % BN; const int j = t / BN;
-        int4 v = make_int4(0, 0, 0, 0);
-        if (r < p.N) v = ldg16(p.Bw + (int64_t)r * K + j * 64 + c16 * 8);
-        *reinterpret_cast<int4*>(sW + (size_t)j * B_CHUNK + img_off(r, c16)) = v;
-    }
-    fence_proxy_async_smem();
     __syncthreads();
     // each CTA walks a CONTIGUOUS range of tiles: with the minibatch gather every image (3-4 tiles) is then
     // touched by one SM only (TLB / L2 locality), and the image indices of tile+1 can be prefetched
@@ -115,6 +113,10 @@ __global__ void __launch_bounds__(kConvWinThreads, 1) tc_conv_win(const __grid_c
 #pragma unroll
                     for (int c = 0; c < CPR; ++c) tma_load_2d(dst + c * IMG, &tmA, c * 64, tile * 128, &full_bar[s]);
                 }
+                if (q == 0) {       // the weight image, one [BN rows x 64 channels] box per K chunk (rows >= N zero-filled)
+                    mbar_arrive_expect_tx(&w_bar, (uint32_t)(nchunks * B_CHUNK));
+                    for (int j = 0; j < nchunks; ++j) tma_load_2d(smem_u32(sW + (size_t)j * B_CHUNK), &tmW, j * 64, 0, &w_bar);
+                }
             }
         }
     } else if (warp >= 4) {
@@ -131,6 +133,7 @@ __global__ void __launch_bounds__(kConvWinThreads, 1) tc_conv_win(const __grid_c
         float d[BN / 2];
 #pragma unroll
         for (int e = 0; e < BN / 2; ++e) d[e] = 0.f;
+        if (tile_begin < tile_end) mbar_wait(&w_bar, 0);
         for (int tile = tile_begin; tile < tile_end; ++tile) {
             const uint32_t q = (uint32_t)(tile - tile_begin), s = q % STAGES;
             // the row -> (image, Y, X) -> output offset arithmetic, done while the tile's MMAs run
@@ -297,14 +300,16 @@ static int launch_conv_win(const WinParams& p, cudaStream_t s, const char* what)
     const int total = p.tpi_shift ? (int)((int64_t)p.n << p.tpi_shift) : (int)ceil_div(p.M, 128);
     int grid = num_sms();
     if (grid > total) grid = total;
-    CUtensorMap tmA;
+    CUtensorMap tmA, tmW;
     memset(&tmA, 0, sizeof(tmA));
+    memset(&tmW, 0, sizeof(tmW));
     int rc;
     // the window is a TMA box [WR rows x 64 channels] per column chunk: of the linear grid, or of one image
     if (p.tpi_shift) rc = make_tmap_3d(&tmA, p.A, p.n_images, p.G, (int64_t)CPR * 64, p.WR, what);
     else rc = make_tmap_2d(&tmA, p.A, p.M, (int64_t)CPR * 64, p.WR, what);
     if (rc) return rc;
-    tc_conv_win<BN, CPR, STAGES, NTAPS><<<grid, kConvWinThreads, smem, s>>>(tmA, p, total);
+    if ((rc = make_tmap_2d(&tmW, p.Bw, p.N, (int64_t)NTAPS * CPR * 64, BN, what))) return rc;      // packed [N][K] weights
+    tc_conv_win<BN, CPR, STAGES, NTAPS><<<grid, kConvWinThreads, smem, s>>>(tmA, tmW, p, total);
     return check_launch(what);
 }
 
@@ -318,10 +323,12 @@ static int launch_conv_win(const WinParams& p, cudaStream_t s, const char* what)
 // The two consumer warpgroups take alternate tiles, each with its own accumulators and stages, so one warpgroup's
 // epilogue runs under the other's MMAs; a stage is released as soon as its MMAs have completed.  The epilogue
 // transposes the accumulators (rows = channels) through shared memory into position rows and applies exactly the fp32
-// operations of tc_conv_win, one thread per position; the packed rows are then stored as whole 128-byte lines by 8
-// lanes per position (DESIGN.md section 4).  Every output is the same bf16 products summed over the same
-// K sequence (taps, column chunks, k16 steps in order; the first MMA with scale-d = 0), and the results are
-// bit-identical to tc_conv_win.
+// operations of tc_conv_win, one thread per position (two at BP = 64, one per 32-channel group); the packed rows are
+// then stored as whole 128-byte lines by 8 lanes per position (DESIGN.md section 4).  Every output is the same bf16
+// products summed over the same K sequence (taps, column chunks, k16 steps in order; the first MMA with scale-d = 0),
+// and the results are bit-identical to tc_conv_win and between BP = 64 and BP = 128.
+// BP = 64 is for small batches (the rollout step): at n = 1024 it doubles the tiles per CTA and shortens the first
+// window a CTA waits for (conv3: 88 rows instead of 152), which leaves room for more stages.
 // The conv2 data gradient (Cout = 128, K = 256) stays on tc_conv_win: with two m64 halves per warpgroup, its epilogue
 // (128 channels per position) outlasts the other warpgroup's MMAs, and it measured about 3 % slower.
 constexpr int kConvWinTThreads = 384;
@@ -344,19 +351,25 @@ __device__ __forceinline__ void stage_acc_transposed(float* st, int wg_tid, cons
 }
 
 template <int BP, int CPR, int STAGES, int NTAPS>
-__global__ void __launch_bounds__(kConvWinTThreads, 1) tc_conv_win_t(const __grid_constant__ CUtensorMap tmA, const WinParams p,
+__global__ void __launch_bounds__(kConvWinTThreads, 1) tc_conv_win_t(const __grid_constant__ CUtensorMap tmA,
+                                                                     const __grid_constant__ CUtensorMap tmW, const WinParams p,
                                                                      int total_tiles) {
-    static_assert(BP % 128 == 0, "one thread per position row of a 128-row slice");
+    static_assert(BP == 64 || BP % 128 == 0, "the epilogue's 128 threads per warpgroup cover whole position rows");
     static_assert(STAGES % 2 == 0, "each consumer warpgroup owns every other stage");
-    constexpr int RPT = BP / 128;                        // position rows per epilogue thread
+    // BP >= 128: one thread per position, RPT positions per thread; BP = 64: two threads per position, one per 32-channel
+    // group g (= mask word)
+    constexpr int TPP = BP >= 128 ? 1 : 2;               // epilogue threads per position
+    constexpr int PPR = 128 / TPP;                       // positions per pass of the warpgroup
+    constexpr int RPT = BP >= 128 ? BP / 128 : 1;        // passes (position rows per epilogue thread)
     constexpr int A_CHUNK = 64 * 128;                    // one 64-channel K chunk of the 64 weight rows
     constexpr int LDS = kConvWinTLds;
     extern __shared__ uint8_t smem_raw[];
-    __shared__ uint64_t full_bar[STAGES], empty_bar[STAGES];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    __shared__ uint64_t full_bar[STAGES], empty_bar[STAGES], w_bar;
+    // aligned by an offset from smem_raw (not through an integer): the staging tile's accesses stay shared-memory
+    // instructions instead of generic ones
+    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     const int tid = threadIdx.x, warp = tid >> 5;
     const int nchunks = NTAPS * CPR;
-    const int K = nchunks * 64;
     const int IMG = p.WR * 128;
     const int STAGE_BYTES = IMG * CPR;
     uint8_t* sW = smem;
@@ -365,24 +378,19 @@ __global__ void __launch_bounds__(kConvWinTThreads, 1) tc_conv_win_t(const __gri
 
     if (tid == 0) {
         for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 4); }   // the consuming warpgroup's 4 warps
+        mbar_init(&w_bar, 1);
         fence_barrier_init();
         tma_prefetch_desc(&tmA);
+        tma_prefetch_desc(&tmW);
     }
-    for (int idx = tid; idx < nchunks * 64 * 8; idx += blockDim.x) {
-        const int c16 = idx & 7;
-        const int t = idx >> 3;
-        const int r = t & 63, j = t >> 6;
-        int4 v = make_int4(0, 0, 0, 0);
-        if (r < p.N) v = ldg16(p.Bw + (int64_t)r * K + j * 64 + c16 * 8);
-        *reinterpret_cast<int4*>(sW + (size_t)j * A_CHUNK + img_off(r, c16)) = v;
-    }
-    fence_proxy_async_smem();
     __syncthreads();
     const int tile_begin = (int)(((int64_t)total_tiles * blockIdx.x) / gridDim.x);
     const int tile_end = (int)(((int64_t)total_tiles * (blockIdx.x + 1)) / gridDim.x);
 
     if (warp == 0) {
-        // ======================= TMA producer: one [WR rows x 64 channels] box per column chunk, tiles in order
+        // ======================= TMA producer: one [WR rows x 64 channels] box per column chunk, tiles in order.  The
+        // weight image (one [64 rows x 64 channels] box per K chunk, on a barrier of its own) goes out right after the
+        // first window, so both are in flight together instead of the window waiting for a load of the whole image.
         if (tid == 0) {
             uint32_t q = 0;
             for (int tile = tile_begin; tile < tile_end; ++tile, ++q) {
@@ -392,6 +400,10 @@ __global__ void __launch_bounds__(kConvWinTThreads, 1) tc_conv_win_t(const __gri
                 mbar_arrive_expect_tx(&full_bar[s], (uint32_t)STAGE_BYTES);
 #pragma unroll
                 for (int c = 0; c < CPR; ++c) tma_load_2d(dst + c * IMG, &tmA, c * 64, tile * BP, &full_bar[s]);
+                if (q == 0) {
+                    mbar_arrive_expect_tx(&w_bar, (uint32_t)(nchunks * A_CHUNK));
+                    for (int j = 0; j < nchunks; ++j) tma_load_2d(smem_u32(sW + (size_t)j * A_CHUNK), &tmW, j * 64, 0, &w_bar);
+                }
             }
         }
     } else if (warp >= 4) {
@@ -402,9 +414,11 @@ __global__ void __launch_bounds__(kConvWinTThreads, 1) tc_conv_win_t(const __gri
         const uint32_t w_base = smem_u32(sW);
         const uint32_t mW = (65536u + (uint32_t)p.Wp - 1u) / (uint32_t)p.Wp;
         constexpr int NW = 2;                                // 32-channel groups = mask words per position
+        const int pw = wt % PPR, gq = wt / PPR;              // this thread's position in a pass and (TPP = 2) its group
         float d[BP / 2];
 #pragma unroll
         for (int e = 0; e < BP / 2; ++e) d[e] = 0.f;
+        if (tile_begin + wg < tile_end) mbar_wait(&w_bar, 0);
         for (int tile = tile_begin + wg; tile < tile_end; tile += 2) {
             const uint32_t q = (uint32_t)(tile - tile_begin), s = q % STAGES;
             mbar_wait(&full_bar[s], (q / STAGES) & 1);
@@ -428,7 +442,7 @@ __global__ void __launch_bounds__(kConvWinTThreads, 1) tc_conv_win_t(const __gri
             uint32_t mb[RPT][NW];
 #pragma unroll
             for (int rr = 0; rr < RPT; ++rr) {
-                const int64_t r = (int64_t)tile * BP + rr * 128 + wt;
+                const int64_t r = (int64_t)tile * BP + rr * PPR + pw;
                 const int i = (int)(r / p.G);
                 const int rem = (int)(r - (int64_t)i * p.G);
                 const int Y = (int)(((uint32_t)rem * mW) >> 16), X = rem - Y * p.Wp;
@@ -456,16 +470,21 @@ __global__ void __launch_bounds__(kConvWinTThreads, 1) tc_conv_win_t(const __gri
             named_bar(1 + wg, 128);
 #pragma unroll
             for (int rr = 0; rr < RPT; ++rr) {
-                float* srow = st + (rr * 128 + wt) * LDS;
+                float* srow = st + (rr * PPR + pw) * LDS;
 #pragma unroll
                 for (int g = 0; g < NW; ++g) {
-                    if (!valid[rr] || g * 32 >= p.N) continue;
+                    if (TPP == 2 && g != gq) continue;
+                    if (TPP == 1 && (!valid[rr] || g * 32 >= p.N)) continue;
                     uint32_t v[32];
 #pragma unroll
                     for (int e = 0; e < 8; ++e) {
                         const float4 f = *reinterpret_cast<const float4*>(srow + g * 32 + 4 * e);
                         v[4 * e] = __float_as_uint(f.x); v[4 * e + 1] = __float_as_uint(f.y);
                         v[4 * e + 2] = __float_as_uint(f.z); v[4 * e + 3] = __float_as_uint(f.w);
+                    }
+                    if (TPP == 2) {
+                        named_bar(1 + wg, 128);                 // group 1's packed bytes land on fp32 values of group 0
+                        if (!valid[rr] || g * 32 >= p.N) continue;
                     }
                     if (p.bias) {
                         const float4* bp = reinterpret_cast<const float4*>(p.bias + g * 32);
@@ -516,7 +535,7 @@ __global__ void __launch_bounds__(kConvWinTThreads, 1) tc_conv_win_t(const __gri
                     for (int e = 0; e < 4; ++e) brow[e] = w[e];
                 }
                 // the row's output offsets in its 16 padding bytes (-1: the position is not stored)
-                *reinterpret_cast<longlong2*>(srow + 64) = make_longlong2(valid[rr] ? o1[rr] : -1, o2[rr]);
+                if (gq == 0) *reinterpret_cast<longlong2*>(srow + 64) = make_longlong2(valid[rr] ? o1[rr] : -1, o2[rr]);
             }
             named_bar(1 + wg, 128);
             // coalesced stores: 8 lanes per position row, so a warp store writes 4 whole 128-byte rows (512 contiguous
@@ -555,10 +574,12 @@ static int launch_conv_win_t(WinParams p, cudaStream_t s, const char* what) {
     const int total = (int)ceil_div(p.M, BP);
     int grid = num_sms();
     if (grid > total) grid = total;
-    CUtensorMap tmA;
+    CUtensorMap tmA, tmW;
     memset(&tmA, 0, sizeof(tmA));
+    memset(&tmW, 0, sizeof(tmW));
     if (int rc = make_tmap_2d(&tmA, p.A, p.M, (int64_t)CPR * 64, p.WR, what)) return rc;
-    tc_conv_win_t<BP, CPR, STAGES, NTAPS><<<grid, kConvWinTThreads, smem, s>>>(tmA, p, total);
+    if (int rc = make_tmap_2d(&tmW, p.Bw, 64, (int64_t)NTAPS * CPR * 64, 64, what)) return rc;     // packed [64][K] weights
+    tc_conv_win_t<BP, CPR, STAGES, NTAPS><<<grid, kConvWinTThreads, smem, s>>>(tmA, tmW, p, total);
     return check_launch(what);
 }
 
