@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Per-launch times of the convolutions and the fc layer of the bf16 NatureCNN (conv1 forward on the uint8 rollout, the
-three window convolutions conv2 / conv3 forward and conv3 data gradient, conv21_bwd: the conv2 data gradient fused with
+fused conv2 -> conv3 forward (conv23_fwd), the conv3 data gradient, conv21_bwd: the conv2 data gradient fused with
 the conv1 weight gradient, and the fc Linear(3136, 512) forward, data gradient and weight gradient) at the two batch
 sizes of a PPO iteration: n = 1024 (a rollout step) and n = 32 768 (a minibatch).
 
@@ -21,7 +21,9 @@ import torch
 sys.path.insert(0, str(Path(__file__).resolve().parent))
 from cleanrl_b200 import _lib, build, ops  # noqa: E402
 
-KERNELS = ("conv1_fwd", "conv2_fwd", "conv3_fwd", "conv3_dgrad", "conv21_bwd", "fc_fwd", "fc_dgrad", "fc_wgrad")
+KERNELS = ("conv1_fwd", "conv23_fwd", "conv3_dgrad", "conv21_bwd", "fc_fwd", "fc_dgrad", "fc_wgrad")
+# a library built before conv2 and conv3 forward were fused reports them as two launches (A/B runs against it)
+OLD_NAMES = {"conv23_fwd": ("conv2_fwd", "conv3_fwd")}
 
 
 def measure(lib, n, reps, dev):
@@ -55,8 +57,9 @@ def measure(lib, n, reps, dev):
     buf = ctypes.create_string_buffer(1 << 16)
     _lib.check(lib.b200rl_profile_summary(buf, 1 << 16), "profile_summary")
     prof = {r["name"]: r for r in json.loads(buf.value.decode())}
+    names = [m for k in KERNELS for m in ((k,) if k in prof else OLD_NAMES.get(k, (k,)))]
     return {k: {"us": round(1e3 * prof[k]["ms"] / prof[k]["launches"], 2),
-                "GB/s": round(prof[k]["bytes"] / (prof[k]["ms"] * 1e-3) / 1e9, 1)} for k in KERNELS}
+                "GB/s": round(prof[k]["bytes"] / (prof[k]["ms"] * 1e-3) / 1e9, 1)} for k in names}
 
 
 def main():

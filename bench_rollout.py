@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Where a rollout step of the bf16 NatureCNN goes: one tensor-core policy step on the uint8 rollout slot (frame
-conversion to space-to-depth rows, then ``NatureCNNAgent.sample_into``: conv1 on the integer tensor cores, conv2, conv3,
-fc, the heads and the categorical sampler), at the env batch of bench.py's rollout (n = 1024) and at the chunk sizes of
+conversion to space-to-depth rows, then ``NatureCNNAgent.sample_into``: conv1 on the integer tensor cores, conv2 -> conv3
+in one kernel, fc, the heads and the categorical sampler), at the env batch of bench.py's rollout (n = 1024) and at the chunk sizes of
 its end-to-end loop (256 and 512).
 
     python bench_rollout.py [--sizes 1024,512,256] [--reps 200] [--replays 2000]
@@ -30,7 +30,9 @@ from cleanrl_b200 import _lib, build, ops  # noqa: E402
 from cleanrl_b200.agents import NatureCNNAgent  # noqa: E402
 from cleanrl_b200.synthetic_envs import SyntheticAtariVec  # noqa: E402
 
-KERNELS = ("frames_to_s2d", "conv1_fwd", "conv2_fwd", "conv3_fwd", "fc_fwd", "heads_fwd", "categorical_sample")
+KERNELS = ("frames_to_s2d", "conv1_fwd", "conv23_fwd", "fc_fwd", "heads_fwd", "categorical_sample")
+# a library built before conv2 and conv3 forward were fused reports them as two launches (A/B runs against it)
+OLD_NAMES = {"conv23_fwd": ("conv2_fwd", "conv3_fwd")}
 HBM_BPS, BF16_FLOPS = 3.35e12, 989e12
 
 
@@ -125,7 +127,7 @@ def measure(lib, n, reps, replays, dev):
         torch.cuda.synchronize()
         sm_mhz = clock.stop()
     launches, floor_sum, eager_sum = {}, 0.0, 0.0
-    for k in KERNELS:
+    for k in (m for k in KERNELS for m in ((k,) if k in prof else OLD_NAMES.get(k, (k,)))):
         r = prof[k]
         cnt = r["launches"]
         us = 1e3 * r["ms"] / cnt

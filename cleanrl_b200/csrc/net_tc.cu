@@ -15,13 +15,16 @@
 //   is an image-index indirection inside the conv1 kernels.
 //
 // Kernels
-//   tc_conv_win<BN,CPR,STAGES,NTAPS>   stride-1 "window" convolution (conv1/2/3 forward, conv3/conv2 data-gradient):
+//   tc_conv_win<BN,CPR,STAGES,NTAPS>   stride-1 "window" convolution (conv1 forward, conv2 data gradient; with the channels
+//       on the MMA's M side, tc_conv_win_t, the conv3 data gradient):
 //       GEMM rows enumerate grid positions, so tap (dy,dx) of row r is row r + dy*Wp + dx.  A persistent CTA
 //       stages ONE window of 128+maxshift rows per tile as a TMA box (cp.async.bulk.tensor; for conv1 a 3-D box
 //       whose image coordinate is the minibatch gather) and every tap is a wgmma descriptor whose start address is
 //       shifted by whole 128-byte rows (legal for SWIZZLE_128B: the pattern is a function of the smem address
 //       bits).  Weights stay resident in smem.  Warp 0 = TMA producer, two warpgroups run wgmma on 64 rows each and
 //       the epilogue; ReLU masks are exchanged between forward and backward as bits.
+//   tc_conv23_fwd                conv2 -> conv3 forward in one persistent kernel, one image per tile: conv2's epilogue
+//       writes act2 into a shared-memory operand image that conv3's MMAs read (and to HBM for the backward).
 //   tc_wgrad_win                 conv weight gradients: dW^T[(tap,c), co] = sum_r X[r+shift_tap, c] * dY[r, co]; the same
 //       row images are read as MN-major operands (rows = reduction index), taps again by row shifts; the bias
 //       gradient (column sums of dY) is accumulated by the four dY warps from the staged tiles.
@@ -35,6 +38,7 @@
 #include <algorithm>
 #include "tc_base.cuh"
 #include "tc_conv_win.cuh"
+#include "tc_conv23.cuh"
 #include "tc_conv1_u8.cuh"
 #include "tc_gemm_tma.cuh"
 #include "tc_wgrad_win.cuh"
@@ -162,15 +166,6 @@ static void win_conv1(WinParams& p, const bf16* x0, const int64_t* rows, int64_t
     p.n_images = rows ? (int64_t)1 << 24 : n;    // gather indices are the caller's contract (never range-checked)
     p.ntaps = 4; p.shift[0] = 0; p.shift[1] = 1; p.shift[2] = 21; p.shift[3] = 22; p.WR = round8(128 + 22);
 }
-static void win_conv2(WinParams& p, const bf16* act1, int64_t n) {                         // 2x2 taps on the 10x10 cell grid
-    p.A = act1; p.n = (int)n; p.G = 100; p.Wp = 10; p.M = n * 100;
-    p.ntaps = 4; p.shift[0] = 0; p.shift[1] = 1; p.shift[2] = 10; p.shift[3] = 11; p.WR = round8(128 + 11);
-}
-static void win_conv3(WinParams& p, const bf16* act2, int64_t n) {                         // 3x3 taps on the 9x9 grid
-    p.A = act2; p.n = (int)n; p.G = 81; p.Wp = 9; p.M = n * 81;
-    p.ntaps = 9; for (int ky = 0; ky < 3; ++ky) for (int kx = 0; kx < 3; ++kx) p.shift[ky * 3 + kx] = ky * 9 + kx;
-    p.WR = round8(128 + 20);
-}
 static void wgw_defaults(WGradWinParams& w) { memset(&w, 0, sizeof(w)); }
 
 // row splits of the window weight gradients: one or two waves of CTAs on the 132 SMs of an H100
@@ -233,22 +228,14 @@ static int trunk_fwd(const NatureLayout& L, const NatureActs& Q, const float* pa
                      cudaStream_t s) {
     int rc;
     KGemmParams p;
-    WinParams wp;
-    // conv2: 2x2 window conv on the 128-channel cells -> act2 [n,9,9,64]
-    win_defaults(wp); win_conv2(wp, act + Q.act1, n);
-    wp.Bw = P + L.w2f; wp.N = 64; wp.vH = 9; wp.vW = 9; wp.out_mode = WOUT_DENSE; wp.out = act + Q.act2;
-    wp.bias = params + L.c2b; wp.relu = 1; wp.mask_out = reinterpret_cast<uint32_t*>(act + Q.m2);
-    // small batches (rollout step): 64-position tiles => twice the tiles per CTA and a shorter first window
-    { ProfScope ps(s, "conv2_fwd", 2.0 * n * 81 * 64 * 512, (double)n * ((12800 + 5184) * 2 + 648));
-      if (n <= 8192) { if ((rc = launch_conv_win_t<64, 2, 6, 4>(wp, s, "naturecnn/conv2"))) return rc; }
-      else if ((rc = launch_conv_win_t<128, 2, 2, 4>(wp, s, "naturecnn/conv2"))) return rc; }
-    // conv3: 3x3 window conv -> act3 [n,7,7,64]
-    win_defaults(wp); win_conv3(wp, act + Q.act2, n);
-    wp.Bw = P + L.w3f; wp.N = 64; wp.vH = 7; wp.vW = 7; wp.out_mode = WOUT_DENSE; wp.out = act + Q.act3;
-    wp.bias = params + L.c3b; wp.relu = 1; wp.mask_out = reinterpret_cast<uint32_t*>(act + Q.m3);
-    { ProfScope ps(s, "conv3_fwd", 2.0 * n * 49 * 64 * 576, (double)n * ((5184 + 3136) * 2 + 392));
-      if (n <= 8192) { if ((rc = launch_conv_win_t<64, 1, 8, 9>(wp, s, "naturecnn/conv3"))) return rc; }
-      else if ((rc = launch_conv_win_t<128, 1, 4, 9>(wp, s, "naturecnn/conv3"))) return rc; }
+    // conv2 (2x2 window conv on the 128-channel cells) -> act2 [n,9,9,64] -> conv3 (3x3) -> act3 [n,7,7,64], one kernel:
+    // act2 reaches HBM for the backward but is not read back
+    Conv23Params cp;
+    cp.n = (int)n; cp.b2 = params + L.c2b; cp.b3 = params + L.c3b; cp.act2 = act + Q.act2; cp.act3 = act + Q.act3;
+    cp.m2 = reinterpret_cast<uint32_t*>(act + Q.m2); cp.m3 = reinterpret_cast<uint32_t*>(act + Q.m3);
+    { ProfScope ps(s, "conv23_fwd", 2.0 * n * 81 * 64 * 512 + 2.0 * n * 49 * 64 * 576,
+                   (double)n * (12800 * 2 + 5184 * 2 + 648 + 3136 * 2 + 392));
+      if ((rc = launch_conv23_fwd(act + Q.act1, P + L.w2f, P + L.w3f, cp, s, "naturecnn/conv23"))) return rc; }
     // fc -> hidden [n,512]
     gemm_rowmajor(p, act + Q.act3, n, 49);
     p.Bw = P + L.wfcf; p.N = 512; p.out = act + Q.hid; p.ldo = 512; p.bias = params + L.fcb; p.relu = 1;

@@ -314,21 +314,18 @@ static int launch_conv_win(const WinParams& p, cudaStream_t s, const char* what)
 }
 
 // ------------------------------------------------------------------ kernel 1d: window convolution, channels on the MMA's M side
-// The same window convolution with the operand roles swapped, for Cout = 64 (conv2 / conv3 forward, conv3 data
-// gradient).  A is the resident weight image (M = Cout); B is the staged pixel window, a K-major operand whose
-// descriptor start moves by whole 128-byte rows per tap (N = BP grid positions), so every wgmma is m64nBPk16.  Per
+// The same window convolution with the operand roles swapped, for Cout = 64 (the conv3 data gradient; conv2 and conv3
+// forward run fused in tc_conv23_fwd, tc_conv23.cuh, which keeps this kernel's MMA layout and epilogue).  A is the
+// resident weight image (M = Cout); B is the staged pixel window, a K-major operand whose descriptor start moves by whole 128-byte rows per tap (N = BP grid positions), so every wgmma is m64nBPk16.  Per
 // 64 x BP x 16 step that is 2 KB of weights and BP x 32 B of window from shared memory, against 2 KB + 2 KB per
 // 64 x 64 x 16 with positions on M and Cout on N: at BP = 128 the operand traffic drops from 128 B to 96 B per
 // tensor-core cycle, under the 128 B per cycle an SM's shared memory delivers.
 // The two consumer warpgroups take alternate tiles, each with its own accumulators and stages, so one warpgroup's
 // epilogue runs under the other's MMAs; a stage is released as soon as its MMAs have completed.  The epilogue
 // transposes the accumulators (rows = channels) through shared memory into position rows and applies exactly the fp32
-// operations of tc_conv_win, one thread per position (two at BP = 64, one per 32-channel group); the packed rows are
-// then stored as whole 128-byte lines by 8 lanes per position (DESIGN.md section 4).  Every output is the same bf16
-// products summed over the same K sequence (taps, column chunks, k16 steps in order; the first MMA with scale-d = 0),
-// and the results are bit-identical to tc_conv_win and between BP = 64 and BP = 128.
-// BP = 64 is for small batches (the rollout step): at n = 1024 it doubles the tiles per CTA and shortens the first
-// window a CTA waits for (conv3: 88 rows instead of 152), which leaves room for more stages.
+// operations of tc_conv_win, one thread per position; the packed rows are then stored as whole 128-byte lines by 8 lanes
+// per position (DESIGN.md section 4).  Every output is the same bf16 products summed over the same K sequence (taps,
+// column chunks, k16 steps in order; the first MMA with scale-d = 0), and the results are bit-identical to tc_conv_win.
 // The conv2 data gradient (Cout = 128, K = 256) stays on tc_conv_win: with two m64 halves per warpgroup, its epilogue
 // (128 channels per position) outlasts the other warpgroup's MMAs, and it measured about 3 % slower.
 constexpr int kConvWinTThreads = 384;
@@ -354,13 +351,10 @@ template <int BP, int CPR, int STAGES, int NTAPS>
 __global__ void __launch_bounds__(kConvWinTThreads, 1) tc_conv_win_t(const __grid_constant__ CUtensorMap tmA,
                                                                      const __grid_constant__ CUtensorMap tmW, const WinParams p,
                                                                      int total_tiles) {
-    static_assert(BP == 64 || BP % 128 == 0, "the epilogue's 128 threads per warpgroup cover whole position rows");
+    static_assert(BP % 128 == 0, "the epilogue's 128 threads per warpgroup cover whole position rows");
     static_assert(STAGES % 2 == 0, "each consumer warpgroup owns every other stage");
-    // BP >= 128: one thread per position, RPT positions per thread; BP = 64: two threads per position, one per 32-channel
-    // group g (= mask word)
-    constexpr int TPP = BP >= 128 ? 1 : 2;               // epilogue threads per position
-    constexpr int PPR = 128 / TPP;                       // positions per pass of the warpgroup
-    constexpr int RPT = BP >= 128 ? BP / 128 : 1;        // passes (position rows per epilogue thread)
+    constexpr int PPR = 128;                             // positions per pass of the warpgroup (one thread per position)
+    constexpr int RPT = BP / 128;                        // passes (position rows per epilogue thread)
     constexpr int A_CHUNK = 64 * 128;                    // one 64-channel K chunk of the 64 weight rows
     constexpr int LDS = kConvWinTLds;
     extern __shared__ uint8_t smem_raw[];
@@ -414,7 +408,7 @@ __global__ void __launch_bounds__(kConvWinTThreads, 1) tc_conv_win_t(const __gri
         const uint32_t w_base = smem_u32(sW);
         const uint32_t mW = (65536u + (uint32_t)p.Wp - 1u) / (uint32_t)p.Wp;
         constexpr int NW = 2;                                // 32-channel groups = mask words per position
-        const int pw = wt % PPR, gq = wt / PPR;              // this thread's position in a pass and (TPP = 2) its group
+        const int pw = wt;                                   // this thread's position in a pass
         float d[BP / 2];
 #pragma unroll
         for (int e = 0; e < BP / 2; ++e) d[e] = 0.f;
@@ -473,18 +467,13 @@ __global__ void __launch_bounds__(kConvWinTThreads, 1) tc_conv_win_t(const __gri
                 float* srow = st + (rr * PPR + pw) * LDS;
 #pragma unroll
                 for (int g = 0; g < NW; ++g) {
-                    if (TPP == 2 && g != gq) continue;
-                    if (TPP == 1 && (!valid[rr] || g * 32 >= p.N)) continue;
+                    if (!valid[rr] || g * 32 >= p.N) continue;
                     uint32_t v[32];
 #pragma unroll
                     for (int e = 0; e < 8; ++e) {
                         const float4 f = *reinterpret_cast<const float4*>(srow + g * 32 + 4 * e);
                         v[4 * e] = __float_as_uint(f.x); v[4 * e + 1] = __float_as_uint(f.y);
                         v[4 * e + 2] = __float_as_uint(f.z); v[4 * e + 3] = __float_as_uint(f.w);
-                    }
-                    if (TPP == 2) {
-                        named_bar(1 + wg, 128);                 // group 1's packed bytes land on fp32 values of group 0
-                        if (!valid[rr] || g * 32 >= p.N) continue;
                     }
                     if (p.bias) {
                         const float4* bp = reinterpret_cast<const float4*>(p.bias + g * 32);
@@ -535,7 +524,7 @@ __global__ void __launch_bounds__(kConvWinTThreads, 1) tc_conv_win_t(const __gri
                     for (int e = 0; e < 4; ++e) brow[e] = w[e];
                 }
                 // the row's output offsets in its 16 padding bytes (-1: the position is not stored)
-                if (gq == 0) *reinterpret_cast<longlong2*>(srow + 64) = make_longlong2(valid[rr] ? o1[rr] : -1, o2[rr]);
+                *reinterpret_cast<longlong2*>(srow + 64) = make_longlong2(valid[rr] ? o1[rr] : -1, o2[rr]);
             }
             named_bar(1 + wg, 128);
             // coalesced stores: 8 lanes per position row, so a warp store writes 4 whole 128-byte rows (512 contiguous

@@ -19,7 +19,9 @@ METRICS = ["gpu__time_duration.sum", "dram__bytes_read.sum", "dram__bytes_write.
 
 # algorithmic bytes per sample (DESIGN.md "kernels" table; the same figures as the ProfScope calls in net_tc.cu)
 ALGO = {
-    "conv1_fwd": (28224 + 12800) * 2 + 1600, "conv2_fwd": (12800 + 5184) * 2 + 648, "conv3_fwd": (5184 + 3136) * 2 + 392,
+    "conv1_fwd": (28224 + 12800) * 2 + 1600, "conv23_fwd": 12800 * 2 + 5184 * 2 + 648 + 3136 * 2 + 392,
+    # conv2 and conv3 forward as the two launches of a build before tc_conv23_fwd (A/B captures against it)
+    "conv2_fwd": (12800 + 5184) * 2 + 648, "conv3_fwd": (5184 + 3136) * 2 + 392,
     "fc_fwd": (3136 + 512) * 2, "fc_dgrad": (3136 + 512) * 2 + 392, "conv3_dgrad": (7744 + 6400 + 7744) * 2 + 648,
     "conv2_dgrad": (7744 + 14112) * 2 + 1600, "conv3_wgrad": (5184 + 5184) * 2, "conv2_wgrad": (12800 + 6400) * 2,
     "conv1_wgrad": (28224 + 14112) * 2, "fc_wgrad": (3136 + 512) * 2,
@@ -58,6 +60,8 @@ def main():
         if short.startswith("tc_conv1_i8"): layer = "conv1_fwd"
         elif short.startswith("tc_conv21_bwd_u8"): layer = "conv21_bwd"
         elif short.startswith("tc_conv_win<32"): layer = "conv1_fwd"
+        elif short.startswith("tc_conv23_fwd"): layer = "conv23_fwd"
+        elif short.startswith("tc_conv_win_t"): layer = "conv3_dgrad"
         elif short.startswith("tc_conv_win<64, 2"): layer = "conv2_fwd"
         elif short.startswith("tc_conv_win<64, 1"): layer = "conv3_fwd" if k % 2 == 0 else "conv3_dgrad"
         elif short.startswith("tc_conv_win<128"): layer = "conv2_dgrad"
