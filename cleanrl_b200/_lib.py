@@ -121,6 +121,16 @@ SIGNATURES = {
     "b200rl_sac_actor_loss_workspace_bytes": (_sz, [_i64]),
     "b200rl_sac_actor_loss_f32": (_i, [_p, _i64, _p, _i64, _p, _i64, _i64, _i, _p, _i, _p, _p, _p, _p, _d, _d, _d, _d,
                                        _p, _i64, _p, _p, _sz, _p]),
+    "b200rl_sacc_param_count": (_i64, [_i, _i, _i]),
+    "b200rl_sacc_workspace_bytes": (_sz, [_i64]),
+    "b200rl_sacc_critic_fwd_f32": (_i, [_p, _i64, _p, _i64, _p, _p, _i64, _p, _i64, _i, _i, _p, _p, _p, _p, _p]),
+    "b200rl_sacc_actor_fwd_f32": (_i, [_p, _p, _i64, _p, _i64, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i, _d,
+                                       _p, _p, _p, _p, _p, _d, _d, _d, _p, _p, _sz, _p]),
+    "b200rl_sacc_critic_loss_f32": (_i, [_p, _p, _p, _p, _p, _i64, _p, _p, _i64, _d, _p, _p, _p, _p, _sz, _p]),
+    "b200rl_sacc_critic_bwd_f32": (_i, [_p, _i64, _i64, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "b200rl_sacc_actor_bwd_f32": (_i, [_p, _i64, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p]),
+    "b200rl_sacc_wgrad_f32": (_i, [_i, _i64, _i, _i, _p, _p, _p, _p, _p, _p, _p, _i64, _p]),
+    "b200rl_sacc_soft_update_f32": (_i, [_p, _p, _i64, _d, _p]),
 }
 
 

@@ -1188,3 +1188,249 @@ def sac_update(actor, qf1, qf2, qf1_target, qf2_target, ring, batch, state, gamm
     for n in (actor, qf1, qf2):
         n.params_updated()                    # no python ran inside the replay: the packed operand copies are stale
     return state
+
+
+# ------------------------------------------------------- continuous SAC (cleanrl/sac_continuous_action.py)
+SACC_LOG_STD_MAX = 2
+SACC_LOG_STD_MIN = -5
+SACC_ADAM_EPS = 1e-8        # torch.optim.Adam's default, all three optimisers (sac_continuous_action.py:199-207)
+
+
+def _sacc_dims(env):
+    return int(np.array(env.single_observation_space.shape).prod()), int(np.prod(env.single_action_space.shape))
+
+
+class SoftQNetworkMLP(nn.Module):
+    """sac_continuous_action.py:84-99: fc1 [obs + act -> 256], fc2, fc3 [-> 1], default nn.Linear initialisation.
+    ``forward(x, a)`` runs the fp32 critic kernel on this one network (``net_stride`` 0)."""
+
+    def __init__(self, env):
+        super().__init__()
+        self.obs_dim, self.act_dim = _sacc_dims(env)
+        self.fc1 = nn.Linear(self.obs_dim + self.act_dim, 256)
+        self.fc2 = nn.Linear(256, 256)
+        self.fc3 = nn.Linear(256, 1)
+
+    def flat_params(self):
+        """The parameters as one flat f32 vector (a view when they already live in a flat buffer)."""
+        ps = list(self.parameters())
+        base = ps[0].data
+        n = sum(p.numel() for p in ps)
+        if base.is_contiguous() and all(p.data.data_ptr() == base.data_ptr() + 4 * sum(q.numel() for q in ps[:i])
+                                        for i, p in enumerate(ps)):
+            return torch.as_strided(base, (n,), (1,))
+        return torch.cat([p.data.reshape(-1) for p in ps])
+
+    @torch.no_grad()
+    def forward(self, x, a):
+        B = x.shape[0]
+        q = ops.sacc_critic_fwd(self.flat_params(), 0, x.float().reshape(B, -1).contiguous(),
+                                a.float().reshape(B, -1).contiguous(), B, self.obs_dim, self.act_dim)
+        return q[0].reshape(B, 1)
+
+
+class SACContinuousActor(nn.Module):
+    """sac_continuous_action.py:106-151: fc1, fc2, fc_mean, fc_logstd and the buffers action_scale / action_bias.
+    ``forward(x)`` -> (mean, log_std); ``get_action(x)`` -> (action, log_prob [n, 1], squashed mean), drawing the
+    [n, D] standard normals with ``noise_fn`` (``buf.normal_()`` on the default CUDA generator, what
+    ``Normal.rsample`` consumes)."""
+
+    def __init__(self, env):
+        super().__init__()
+        self.obs_dim, self.act_dim = _sacc_dims(env)
+        self.fc1 = nn.Linear(self.obs_dim, 256)
+        self.fc2 = nn.Linear(256, 256)
+        self.fc_mean = nn.Linear(256, self.act_dim)
+        self.fc_logstd = nn.Linear(256, self.act_dim)
+        high, low = env.single_action_space.high, env.single_action_space.low
+        self.register_buffer("action_scale", torch.tensor((high - low) / 2.0, dtype=torch.float32))
+        self.register_buffer("action_bias", torch.tensor((high + low) / 2.0, dtype=torch.float32))
+        self.noise_fn = _normal_noise
+        self._flat = None
+
+    @property
+    def flat(self):
+        p = next(self.parameters())
+        f = self._flat
+        if f is None or f.flat.device != p.device or p.data_ptr() != f.flat.data_ptr():
+            if p.device.type != "cuda":
+                raise RuntimeError("cleanrl_b200 agents execute on CUDA only (libb200rl kernels); there is no CPU fallback.")
+            self._flat = nets.FlatParams(list(self.parameters()), p.device)
+        return self._flat
+
+    @property
+    def graph_friendly(self):
+        """May the noise draw be captured in a CUDA graph (a device-generator draw)?"""
+        return getattr(self.noise_fn, "graph_safe", False)
+
+    def draw_noise_into(self, buf):
+        if hasattr(self.noise_fn, "inplace"):
+            self.noise_fn.inplace(buf)
+        else:
+            buf.copy_(self.noise_fn(buf.shape[0], buf.shape[1], buf.device))
+
+    def _obs(self, x):
+        return x.float().reshape(x.shape[0], -1).contiguous()
+
+    @torch.no_grad()
+    def forward(self, x):
+        B, D = x.shape[0], self.act_dim
+        ml = torch.empty(B, 2 * D, dtype=torch.float32, device=x.device)
+        ops.sacc_actor_fwd(self.flat.flat, self._obs(x), B, self.obs_dim, D, None, self.action_scale, self.action_bias,
+                           mean_logstd=ml)
+        return ml[:, :D], ml[:, D:]
+
+    @torch.no_grad()
+    def get_action(self, x, eps=None):
+        B, D = x.shape[0], self.act_dim
+        dev = x.device
+        eps = self.noise_fn(B, D, dev) if eps is None else eps
+        action = torch.empty(B, D, dtype=torch.float32, device=dev)
+        log_pi = torch.empty(B, 1, dtype=torch.float32, device=dev)
+        mean = torch.empty(B, D, dtype=torch.float32, device=dev)
+        ops.sacc_actor_fwd(self.flat.flat, self._obs(x), B, self.obs_dim, D, eps.contiguous(), self.action_scale,
+                           self.action_bias, action=action, log_pi=log_pi, mean_out=mean)
+        return action, log_pi, mean
+
+
+class SACContinuousState:
+    """Device-resident part of a continuous-SAC update that is not a network: the flat buffers of the twin critics
+    (one parameter / gradient / Adam buffer, as ``q_optimizer`` covers both) and of the twin targets, the temperature
+    (``alpha`` f32[1], with autotune ``log_alpha`` and its Adam moments), the Adam step counts of the q, actor and
+    temperature optimisers with their device table of step scalars, the logged statistics (``qstats`` =
+    ``ops.SACC_CRITIC_STAT_NAMES``, ``astats`` = ``ops.SACC_ACTOR_STAT_NAMES``) and the scratch of each batch size.
+    With ``use_graph`` every update is replayed as one CUDA graph per (batch size, with actor steps, with target
+    update)."""
+
+    use_graph = True
+
+    def __init__(self, actor, qf1, qf2, qf1_target, qf2_target, device, autotune=True, alpha=0.2, policy_frequency=2):
+        f32 = torch.float32
+        self.device, self.autotune, self.pf = device, bool(autotune), int(policy_frequency)
+        self.actor, self.obs_dim, self.act_dim = actor, actor.obs_dim, actor.act_dim
+        self.net_numel = ops.sacc_param_count(self.obs_dim, self.act_dim, True)
+        self.q = nets.FlatParams(list(qf1.parameters()) + list(qf2.parameters()), device)
+        self.qt = nets.FlatParams(list(qf1_target.parameters()) + list(qf2_target.parameters()), device)
+        actor.flat
+        # -torch.prod(torch.Tensor(envs.single_action_space.shape)).item()  (sac_continuous_action.py:204)
+        self.target_entropy = -torch.prod(torch.Tensor((self.act_dim,))).item()
+        self.log_alpha = torch.zeros(1, dtype=f32, device=device)
+        self.alpha = torch.full((1,), 1.0 if autotune else float(alpha), dtype=f32, device=device)
+        self.exp_avg = torch.zeros(1, dtype=f32, device=device)
+        self.exp_avg_sq = torch.zeros(1, dtype=f32, device=device)
+        self.qstats = torch.zeros(4, dtype=f32, device=device)
+        self.astats = torch.zeros(4, dtype=f32, device=device)
+        self.astats[2] = self.alpha[0]          # losses/alpha before the first temperature step
+        self.steps = {"q": 0, "actor": 0, "alpha": 0}
+        self._bufs, self._graphs, self._pool = {}, {}, None
+
+    def buffers(self, B):
+        b = self._bufs.get(B)
+        if b is None:
+            f32, dev, D, K = torch.float32, self.device, self.act_dim, self.obs_dim + self.act_dim
+            z = lambda *s: torch.zeros(*s, dtype=f32, device=dev)   # noqa: E731
+            b = {"rows": torch.zeros(B, dtype=torch.int64, device=dev), "dyn": z(2 + 4 * self.pf),
+                 "x": z(B, K), "h1": z(2, B, 256), "h2": z(2, B, 256), "dz1": z(2, B, 256), "dz2": z(2, B, 256),
+                 "q": z(2, B), "qn": z(2, B), "dq": z(2, B), "y": z(B), "pi_next": z(B, D), "logpi_next": z(B),
+                 "eps_next": z(B, D), "eps_actor": z(self.pf, B, D), "eps_alpha": z(self.pf, B, D),
+                 "xa": z(B, self.obs_dim), "h1a": z(B, 256), "h2a": z(B, 256), "head": z(B, 2 * D), "pi": z(B, D),
+                 "logpi": z(B), "qpi": z(2, B), "dact": z(2, B, D), "dhead": z(B, 2 * D), "dz1a": z(B, 256),
+                 "dz2a": z(B, 256), "logpi_alpha": z(B), "ws": ops.sacc_workspace(B, dev)}
+            self._bufs[B] = b
+        return b
+
+    def step_table(self, actor_steps, q_lr, policy_lr):
+        """Advance the optimisers' step counts and return their ``adam_step_scalars``: q, then per actor step the
+        actor's and the temperature's (whose lr is q_lr, sac_continuous_action.py:207)."""
+        self.steps["q"] += 1
+        t = list(ops.adam_step_scalars(self.steps["q"], q_lr))
+        for _ in range(self.pf):
+            if actor_steps:
+                self.steps["actor"] += 1
+                t += ops.adam_step_scalars(self.steps["actor"], policy_lr)
+                if self.autotune:
+                    self.steps["alpha"] += 1
+                    t += ops.adam_step_scalars(self.steps["alpha"], q_lr)
+                else:
+                    t += (1.0, 0.0)
+            else:
+                t += (1.0, 0.0, 1.0, 0.0)
+        return t
+
+
+def _sacc_update_body(st, obs, next_obs, actions, rewards, dones, rows, buf, actor_steps, target_update, gamma, tau):
+    """sac_continuous_action.py:255-304 on device buffers; every (step, lr) scalar comes from ``buf["dyn"]``."""
+    actor, B, od, D, S = st.actor, rows.numel(), st.obs_dim, st.act_dim, st.net_numel
+    af, q, dyn, ws = actor.flat, st.q, buf["dyn"], buf["ws"]
+    scale, bias = actor.action_scale, actor.action_bias
+    # 1. soft-Q target on next_obs (the actor's sample, both targets) and the critic loss, backward and q optimiser
+    actor.draw_noise_into(buf["eps_next"])
+    ops.sacc_actor_fwd(af.flat, next_obs, B, od, D, buf["eps_next"], scale, bias, rows=rows, action=buf["pi_next"],
+                       log_pi=buf["logpi_next"])
+    ops.sacc_critic_fwd(st.qt.flat, S, next_obs, buf["pi_next"], B, od, D, obs_rows=rows, q=buf["qn"])
+    ops.sacc_critic_fwd(q.flat, S, obs, actions, B, od, D, obs_rows=rows, act_rows=rows, q=buf["q"], keep_x=buf["x"],
+                        keep_h1=buf["h1"], keep_h2=buf["h2"])
+    ops.sacc_critic_loss(buf["qn"], buf["logpi_next"], buf["q"], rewards, dones, st.alpha, gamma, rows=rows, y=buf["y"],
+                         dq=buf["dq"], stats=st.qstats, workspace=ws)
+    ops.sacc_critic_bwd(q.flat, S, B, od, D, buf["h1"], buf["h2"], dq=buf["dq"], dz1=buf["dz1"], dz2=buf["dz2"])
+    ops.sacc_wgrad(True, B, od, D, buf["x"], buf["h1"], buf["h2"], buf["dz1"], buf["dz2"], buf["dq"], q.grad, S)
+    ops.clip_adam_dyn(q.flat, q.grad, q.exp_avg, q.exp_avg_sq, dyn[0:2], eps=SACC_ADAM_EPS, max_norm=None)
+    # 2. policy_frequency actor steps, each followed by the temperature step on a fresh sample
+    for k in range(st.pf if actor_steps else 0):
+        eps = buf["eps_actor"][k]
+        actor.draw_noise_into(eps)
+        ops.sacc_actor_fwd(af.flat, obs, B, od, D, eps, scale, bias, rows=rows, action=buf["pi"], log_pi=buf["logpi"],
+                           keep_x=buf["xa"], keep_h1=buf["h1a"], keep_h2=buf["h2a"], keep_head=buf["head"])
+        ops.sacc_critic_fwd(q.flat, S, obs, buf["pi"], B, od, D, obs_rows=rows, q=buf["qpi"], keep_h1=buf["h1"],
+                            keep_h2=buf["h2"])
+        ops.sacc_critic_bwd(q.flat, S, B, od, D, buf["h1"], buf["h2"], q=buf["qpi"], dact=buf["dact"])
+        ops.sacc_actor_bwd(af.flat, B, od, D, buf["head"], eps, scale, buf["dact"], buf["qpi"], buf["logpi"], st.alpha,
+                           buf["h1a"], buf["h2a"], buf["dhead"], buf["dz1a"], buf["dz2a"], st.astats, ws)
+        ops.sacc_wgrad(False, B, od, D, buf["xa"], buf["h1a"], buf["h2a"], buf["dz1a"], buf["dz2a"], buf["dhead"], af.grad)
+        ops.clip_adam_dyn(af.flat, af.grad, af.exp_avg, af.exp_avg_sq, dyn[2 + 4 * k:4 + 4 * k], eps=SACC_ADAM_EPS,
+                          max_norm=None)
+        if st.autotune:
+            e2 = buf["eps_alpha"][k]
+            actor.draw_noise_into(e2)
+            ops.sacc_actor_fwd(af.flat, obs, B, od, D, e2, scale, bias, rows=rows, log_pi=buf["logpi_alpha"],
+                               temperature=dict(alpha=st.alpha, log_alpha=st.log_alpha, exp_avg=st.exp_avg,
+                                                exp_avg_sq=st.exp_avg_sq, step_scalars=dyn[4 + 4 * k:6 + 4 * k],
+                                                target_entropy=st.target_entropy, stats=st.astats),
+                               workspace=ws)
+    # 3. soft target update of both targets (one flat buffer)
+    if target_update:
+        ops.sacc_soft_update(q.flat, st.qt.flat, 2 * S, tau)
+
+
+@torch.no_grad()
+def sac_continuous_update(state, ring, batch, global_step, args, graph=None):
+    """One update of sac_continuous_action.py:255-304 on a ``DeviceReplayRing`` batch: the critic step; on steps where
+    ``global_step % policy_frequency == 0`` the ``policy_frequency`` actor and temperature steps on the same batch; the
+    soft target update when ``global_step % target_network_frequency == 0``.  Nothing is read back to the host.  With
+    ``graph`` (default ``state.use_graph``) the update replays one captured CUDA graph per (batch size, actor steps,
+    target update) with the batch rows copied into a fixed slot."""
+    st = state
+    B = int(batch["rows"].numel())
+    buf = st.buffers(B)
+    actor_steps = global_step % args.policy_frequency == 0
+    target_update = global_step % args.target_network_frequency == 0
+    buf["dyn"].copy_(torch.tensor(st.step_table(actor_steps, args.q_lr, args.policy_lr), dtype=torch.float32),
+                     non_blocking=True)
+    views = (ring.frames, ring.next_frames, ring.action_rows, ring.reward_rows, ring.done_rows)
+    use_graph = st.use_graph if graph is None else graph
+    if not (use_graph and st.actor.graph_friendly):
+        _sacc_update_body(st, *views, batch["rows"], buf, actor_steps, target_update, args.gamma, args.tau)
+        return st
+    buf["rows"].copy_(batch["rows"])
+    key = (B, actor_steps, target_update, views[0].data_ptr(), float(args.gamma), float(args.tau))
+    g = st._graphs.get(key)
+    if g is None:
+        ops._workspace(st.device, "adam", ops._lib.load().b200rl_clip_adam_workspace_bytes(st.q.flat.numel()))
+        g = torch.cuda.CUDAGraph()
+        if st._pool is None:
+            st._pool = torch.cuda.graph_pool_handle()
+        with torch.cuda.graph(g, pool=st._pool):
+            _sacc_update_body(st, *views, buf["rows"], buf, actor_steps, target_update, args.gamma, args.tau)
+        st._graphs[key] = g
+    g.replay()
+    return st

@@ -265,6 +265,29 @@ def sac_atari_args(exp_name="sac_atari"):
     return _make("Args", common + algo + extra)
 
 
+def sac_continuous_action_args(exp_name="sac_continuous_action"):
+    """cleanrl/sac_continuous_action.py:19-66."""
+    common = list(_override(_COMMON, exp_name=exp_name))
+    algo = [
+        ("env_id", str, "Hopper-v4", "the environment id of the task"),
+        ("total_timesteps", int, 1000000, "total timesteps of the experiments"),
+        ("num_envs", int, 1, "the number of parallel game environments"),
+        ("buffer_size", int, int(1e6), "the replay memory buffer size"),
+        ("gamma", float, 0.99, "the discount factor gamma"),
+        ("tau", float, 0.005, "target smoothing coefficient (default: 0.005)"),
+        ("batch_size", int, 256, "the batch size of sample from the reply memory"),
+        ("learning_starts", int, 5e3, "timestep to start learning"),
+        ("policy_lr", float, 3e-4, "the learning rate of the policy network optimizer"),
+        ("q_lr", float, 1e-3, "the learning rate of the Q network network optimizer"),
+        ("policy_frequency", int, 2, "the frequency of training policy (delayed)"),
+        ("target_network_frequency", int, 1, "the frequency of updates for the target nerworks"),
+        ("alpha", float, 0.2, "Entropy regularization coefficient."),
+        ("autotune", bool, True, "automatic tuning of the entropy coefficient"),
+    ]
+    extra = [r for r in _EXTRA if r[0] == "synthetic_env"]
+    return _make("Args", common + algo + extra)
+
+
 def parse(cls, argv=None):
     return tyro.cli(cls, args=argv)
 

@@ -1167,3 +1167,122 @@ def sac_actor_loss(logits, q1, q2, alpha, target_entropy=0.0, log_alpha=None, ex
         ws.numel(), _stream())
     _lib.check(rc, "sac_actor_loss")
     return stats, dlogits
+
+
+# ------------------------------------------------------------------------ continuous SAC (sac_continuous_action.py)
+SACC_CRITIC_STAT_NAMES = SAC_CRITIC_STAT_NAMES
+SACC_ACTOR_STAT_NAMES = SAC_ACTOR_STAT_NAMES
+_F32 = torch.float32
+
+
+def _o(t, name):
+    return _ptr(t, _F32, name, allow_none=True)
+
+
+def _rows(t, name="rows"):
+    if t is None:
+        return None
+    return _ptr(_contig(t, name), torch.int64, name)
+
+
+def _ld(t):
+    if t.dim() != 2 or t.stride(1) != 1:
+        raise ValueError("sac_continuous: row-major [n, d] tensor with unit column stride expected")
+    return t.stride(0)
+
+
+def sacc_param_count(obs_dim, act_dim, critic):
+    n = _lib.load().b200rl_sacc_param_count(int(obs_dim), int(act_dim), int(bool(critic)))
+    if n < 0:
+        raise ValueError(f"sac_continuous: obs_dim={obs_dim}, act_dim={act_dim} outside the kernels' limits "
+                         "(1 <= act_dim <= 32, obs_dim + act_dim <= 1024)")
+    return n
+
+
+def sacc_workspace(B, device):
+    """Zeroed scratch of the row-mean kernels of a batch of B rows (one buffer serves all of them on one stream)."""
+    return torch.zeros(max(int(_lib.load().b200rl_sacc_workspace_bytes(int(B))), 16), dtype=torch.uint8, device=device)
+
+
+def sacc_critic_fwd(params, net_stride, obs, act, B, obs_dim, act_dim, obs_rows=None, act_rows=None, q=None, keep_x=None,
+                    keep_h1=None, keep_h2=None):
+    """q [2, B] of the twin critics on [obs[obs_rows] | act[act_rows]] (sac_continuous_action.py:94-99)."""
+    q = torch.empty(2, B, dtype=_F32, device=params.device) if q is None else q
+    rc = _lib.load().b200rl_sacc_critic_fwd_f32(
+        _ptr(params, _F32, "params"), int(net_stride), _ptr(obs, _F32, "obs"), _ld(obs), _rows(obs_rows, "obs_rows"),
+        _ptr(act, _F32, "act"), _ld(act), _rows(act_rows, "act_rows"), int(B), int(obs_dim), int(act_dim),
+        _ptr(q, _F32, "q"), _o(keep_x, "keep_x"), _o(keep_h1, "keep_h1"), _o(keep_h2, "keep_h2"), _stream())
+    _lib.check(rc, "sacc_critic_fwd")
+    return q
+
+
+def sacc_actor_fwd(params, obs, B, obs_dim, act_dim, eps, scale, bias, rows=None, action=None, log_pi=None,
+                   mean_out=None, mean_logstd=None, keep_x=None, keep_h1=None, keep_h2=None, keep_head=None,
+                   temperature=None, workspace=None):
+    """Actor.get_action (sac_continuous_action.py:139-151) with noise ``eps`` [B, D].  ``temperature``: a dict(alpha,
+    log_alpha, exp_avg, exp_avg_sq, step_scalars, target_entropy, stats) to take the autotune step on these log_pi
+    (sac_continuous_action.py:289-297)."""
+    t = temperature or {}
+    rc = _lib.load().b200rl_sacc_actor_fwd_f32(
+        _ptr(params, _F32, "params"), _ptr(obs, _F32, "obs"), _ld(obs), _rows(rows), int(B), int(obs_dim), int(act_dim),
+        _o(eps, "eps"), _ptr(scale, _F32, "scale"), _ptr(bias, _F32, "bias"), _o(action, "action"), _o(log_pi, "log_pi"),
+        _o(mean_out, "mean_out"), _o(mean_logstd, "mean_logstd"), _o(keep_x, "keep_x"), _o(keep_h1, "keep_h1"),
+        _o(keep_h2, "keep_h2"), _o(keep_head, "keep_head"), int(bool(temperature)), float(t.get("target_entropy", 0.0)),
+        _o(t.get("alpha"), "alpha"), _o(t.get("log_alpha"), "log_alpha"), _o(t.get("exp_avg"), "exp_avg"),
+        _o(t.get("exp_avg_sq"), "exp_avg_sq"), _o(t.get("step_scalars"), "step_scalars"), 0.9, 0.999, 1e-8,
+        _o(t.get("stats"), "stats"), workspace.data_ptr() if workspace is not None else None,
+        workspace.numel() if workspace is not None else 0, _stream())
+    _lib.check(rc, "sacc_actor_fwd")
+
+
+def sacc_critic_loss(q_next, next_logpi, q, rewards, dones, alpha, gamma, rows=None, y=None, dq=None, stats=None,
+                     workspace=None):
+    """Soft-Q target and both MSE losses with dq [2, B] (sac_continuous_action.py:257-268).  ``rewards`` / ``dones``
+    are 1-D (strided) views read at ``rows``."""
+    B = q.shape[1]
+    dev = q.device
+    dq = torch.empty(2, B, dtype=_F32, device=dev) if dq is None else dq
+    stats = torch.zeros(4, dtype=_F32, device=dev) if stats is None else stats
+    ws = sacc_workspace(B, dev) if workspace is None else workspace
+    if rewards.stride() != dones.stride():
+        raise ValueError("sacc_critic_loss: rewards and dones need the same stride")
+    rc = _lib.load().b200rl_sacc_critic_loss_f32(
+        _ptr(q_next, _F32, "q_next"), _ptr(next_logpi, _F32, "next_logpi"), _ptr(q, _F32, "q"),
+        _ptr(rewards, _F32, "rewards"), _ptr(dones, _F32, "dones"), rewards.stride(0), _rows(rows), _ptr(alpha, _F32, "alpha"),
+        int(B), float(gamma), _o(y, "y"), _ptr(dq, _F32, "dq"), _ptr(stats, _F32, "stats"), ws.data_ptr(), ws.numel(),
+        _stream())
+    _lib.check(rc, "sacc_critic_loss")
+    return stats, dq
+
+
+def sacc_critic_bwd(params, net_stride, B, obs_dim, act_dim, h1, h2, dq=None, q=None, dz1=None, dz2=None, dact=None):
+    rc = _lib.load().b200rl_sacc_critic_bwd_f32(
+        _ptr(params, _F32, "params"), int(net_stride), int(B), int(obs_dim), int(act_dim), _o(dq, "dq"), _o(q, "q"),
+        _ptr(h1, _F32, "h1"), _ptr(h2, _F32, "h2"), _o(dz1, "dz1"), _o(dz2, "dz2"), _o(dact, "dact"), _stream())
+    _lib.check(rc, "sacc_critic_bwd")
+
+
+def sacc_actor_bwd(params, B, obs_dim, act_dim, head, eps, scale, dact, q, log_pi, alpha, h1, h2, dhead, dz1, dz2, stats,
+                   workspace):
+    rc = _lib.load().b200rl_sacc_actor_bwd_f32(
+        _ptr(params, _F32, "params"), int(B), int(obs_dim), int(act_dim), _ptr(head, _F32, "head"), _ptr(eps, _F32, "eps"),
+        _ptr(scale, _F32, "scale"), _ptr(dact, _F32, "dact"), _ptr(q, _F32, "q"), _ptr(log_pi, _F32, "log_pi"),
+        _ptr(alpha, _F32, "alpha"), _ptr(h1, _F32, "h1"), _ptr(h2, _F32, "h2"), _ptr(dhead, _F32, "dhead"),
+        _ptr(dz1, _F32, "dz1"), _ptr(dz2, _F32, "dz2"), _ptr(stats, _F32, "stats"), workspace.data_ptr(), workspace.numel(),
+        _stream())
+    _lib.check(rc, "sacc_actor_bwd")
+
+
+def sacc_wgrad(critic, B, obs_dim, act_dim, x, h1, h2, dz1, dz2, dout, grad, net_stride=0):
+    rc = _lib.load().b200rl_sacc_wgrad_f32(
+        int(bool(critic)), int(B), int(obs_dim), int(act_dim), _ptr(x, _F32, "x"), _ptr(h1, _F32, "h1"),
+        _ptr(h2, _F32, "h2"), _ptr(dz1, _F32, "dz1"), _ptr(dz2, _F32, "dz2"), _ptr(dout, _F32, "dout"),
+        _ptr(grad, _F32, "grad"), int(net_stride), _stream())
+    _lib.check(rc, "sacc_wgrad")
+
+
+def sacc_soft_update(src, dst, n, tau):
+    """dst[:n] = tau * src[:n] + (1 - tau) * dst[:n] (sac_continuous_action.py:300-304)."""
+    rc = _lib.load().b200rl_sacc_soft_update_f32(_ptr(src, _F32, "src"), _ptr(dst, _F32, "dst"), int(n), float(tau),
+                                                 _stream())
+    _lib.check(rc, "sacc_soft_update")

@@ -63,6 +63,16 @@ class Box:
         self.high = np.full(shape, high, dtype=dtype)
         self.shape = tuple(shape)
         self.dtype = np.dtype(dtype)
+        self._rng = np.random.default_rng(0)
+
+    def seed(self, seed=None):
+        self._rng = np.random.default_rng(seed)
+
+    def sample(self):
+        """Uniform in [low, high] from the space's own generator (bounded spaces only)."""
+        if not (np.all(np.isfinite(self.low)) and np.all(np.isfinite(self.high))):
+            raise ValueError("Box.sample: only bounded boxes can be sampled")
+        return self._rng.uniform(self.low, self.high).astype(self.dtype)
 
     def __repr__(self):
         return f"Box({self.shape}, {self.dtype})"

@@ -567,6 +567,67 @@ int b200rl_sac_actor_loss_f32(const float* logits, int64_t ld, const float* q1, 
                               double beta1, double beta2, double eps, float* dlogits, int64_t ld_d, float* stats,
                               void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---------------------------------------------- continuous soft actor-critic ---
+ * cleanrl/sac_continuous_action.py, fp32: SoftQNetwork [obs | act] -> 256 -> 256 -> 1 and Actor obs -> 256 -> 256 ->
+ * fc_mean / fc_logstd (D each) with the tanh-Gaussian head.  Shapes: 1 <= B <= 8192, 1 <= act_dim (D) <= 32,
+ * obs_dim + act_dim <= 1024; any other shape is B200RL_ERR_INVALID_ARGUMENT.  Parameters are flat f32 in nn.Module order
+ * (fc1.weight, fc1.bias, fc2.weight, fc2.bias, then fc3 or fc_mean, fc_mean.bias, fc_logstd, fc_logstd.bias); the twin
+ * critics are two such blocks net_stride floats apart (critic forward only: 0 = one network, q[0] alone).  Twin
+ * outputs are [2, B] (net-major); kept activations are [2, B, 256] for the critics and [B, 256] for the actor.  Every reduction runs in a fixed order: bitwise repeatable.
+ * Kernels with a row mean take workspace of b200rl_sacc_workspace_bytes(B) bytes, 16-byte aligned, zeroed once; one
+ * buffer may serve all of them on one stream.  Temperature, Adam moments and step scalars live in device memory.
+ *
+ * b200rl_sacc_param_count: floats in one critic (critic != 0) or the actor; -1 for a shape outside the limits.
+ * b200rl_sacc_critic_fwd_f32: q [2, B] of both critics on x = [obs[obs_rows] | act[act_rows]] (either rows vector
+ *   (int64) may be NULL for rows 0..B-1); keep_x [B, K] and keep_h1 / keep_h2 (post-ReLU) may be NULL.
+ * b200rl_sacc_actor_fwd_f32: Actor.get_action on obs[rows] with noise eps [B, D]: action [B, D], log_pi [B], squashed
+ *   mean [B, D], mean_logstd [B, 2D] = Actor.forward's (mean, log_std), the kept x / h1 / h2 and raw head [B, 2D]
+ *   (mean | raw log_std); each may be NULL.  With temperature != 0 it also takes the autotune step on these log_pi:
+ *   alpha_loss = mean(-exp(log_alpha) (log_pi + target_entropy)), one Adam step of log_alpha (beta1, beta2, adam_eps,
+ *   step_scalars f32 [2] as b200rl_adam_step_scalars), alpha = exp(log_alpha); stats[1..3] = alpha_loss, alpha, log_alpha.
+ * min is torch.min's: NaN if either operand is NaN.
+ * b200rl_sacc_critic_loss_f32: y = r + ((1 - d) gamma) (min(q_next[0], q_next[1]) - alpha next_logpi) with r / d read
+ *   through rows (NULL: 0..B-1); dq [2, B] = 2 (q - y) / B; y may be NULL; stats[0..3] = mean q1, mean q2, qf1_loss,
+ *   qf2_loss.
+ * b200rl_sacc_critic_bwd_f32: data gradients through both critics.  Critic step: dq given, writes dz1 / dz2 [2, B, 256]
+ *   (pre-activation gradients of fc1 / fc2).  Actor step: dq NULL, q [2, B] given; the gradient of -mean(min(q1, q2))
+ *   (half to each at a tie, as autograd's min) is carried to the action columns only: dact [2, B, D], one per critic.
+ * b200rl_sacc_actor_bwd_f32: actor_loss = mean(alpha log_pi - min(q[0], q[1])) back through the tanh-Gaussian head (raw
+ *   head and eps of the forward, dact of the critics) to dhead [B, 2D] = (d mean, d raw log_std), then dz2 / dz1
+ *   [B, 256]; stats[0] = actor_loss.
+ * b200rl_sacc_wgrad_f32: weight and bias gradients of all three layers of both critics (critic != 0: dz1 / dz2 [2, B,
+ *   256], dout = dq [2, B], x [B, K], h1 / h2 [2, B, 256]) or of the actor (dout = dhead [B, 2D]) into grad (flat layout,
+ *   overwritten), summed over rows in row order, no atomics.
+ * b200rl_sacc_soft_update_f32: dst = tau * src + (1 - tau) * dst, two products and one sum each rounded.
+ */
+int64_t b200rl_sacc_param_count(int obs_dim, int act_dim, int critic);
+size_t b200rl_sacc_workspace_bytes(int64_t B);
+int b200rl_sacc_critic_fwd_f32(const float* params, int64_t net_stride, const float* obs, int64_t ld_obs,
+                               const int64_t* obs_rows, const float* act, int64_t ld_act, const int64_t* act_rows,
+                               int64_t B, int obs_dim, int act_dim, float* q, float* keep_x, float* keep_h1,
+                               float* keep_h2, void* stream);
+int b200rl_sacc_actor_fwd_f32(const float* params, const float* obs, int64_t ld_obs, const int64_t* rows, int64_t B,
+                              int obs_dim, int act_dim, const float* eps, const float* scale, const float* bias,
+                              float* action, float* log_pi, float* mean_out, float* mean_logstd, float* keep_x,
+                              float* keep_h1, float* keep_h2, float* keep_head, int temperature, double target_entropy,
+                              float* alpha, float* log_alpha, float* exp_avg, float* exp_avg_sq,
+                              const float* step_scalars, double beta1, double beta2, double adam_eps, float* stats,
+                              void* workspace, size_t workspace_bytes, void* stream);
+int b200rl_sacc_critic_loss_f32(const float* q_next, const float* next_logpi, const float* q, const float* rewards,
+                                const float* dones, int64_t ld_rd, const int64_t* rows, const float* alpha, int64_t B, double gamma,
+                                float* y, float* dq, float* stats, void* workspace, size_t workspace_bytes, void* stream);
+int b200rl_sacc_critic_bwd_f32(const float* params, int64_t net_stride, int64_t B, int obs_dim, int act_dim,
+                               const float* dq, const float* q, const float* h1, const float* h2, float* dz1, float* dz2,
+                               float* dact, void* stream);
+int b200rl_sacc_actor_bwd_f32(const float* params, int64_t B, int obs_dim, int act_dim, const float* head,
+                              const float* eps, const float* scale, const float* dact, const float* q,
+                              const float* log_pi, const float* alpha, const float* h1, const float* h2, float* dhead,
+                              float* dz1, float* dz2, float* stats, void* workspace, size_t workspace_bytes, void* stream);
+int b200rl_sacc_wgrad_f32(int critic, int64_t B, int obs_dim, int act_dim, const float* x, const float* h1,
+                          const float* h2, const float* dz1, const float* dz2, const float* dout, float* grad,
+                          int64_t net_stride, void* stream);
+int b200rl_sacc_soft_update_f32(const float* src, float* dst, int64_t n, double tau, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
