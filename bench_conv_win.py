@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Per-launch times of the convolutions and the fc layer of the bf16 NatureCNN (conv1 forward on the uint8 rollout, the
-fused conv2 -> conv3 forward (conv23_fwd), the conv3 data gradient, conv21_bwd: the conv2 data gradient fused with
-the conv1 weight gradient, and the fc Linear(3136, 512) forward, data gradient and weight gradient) at the two batch
-sizes of a PPO iteration: n = 1024 (a rollout step) and n = 32 768 (a minibatch).
+fused conv2 -> conv3 forward (conv23_fwd), the conv3 data gradient, the conv3 and conv2 weight gradients, conv21_bwd:
+the conv2 data gradient fused with the conv1 weight gradient, and the fc Linear(3136, 512) forward, data gradient and
+weight gradient) at the two batch sizes of a PPO iteration: n = 1024 (a rollout step) and n = 32 768 (a minibatch).
 
     python bench_conv_win.py [--reps R] [--sizes 1024,32768]
 
@@ -21,7 +21,8 @@ import torch
 sys.path.insert(0, str(Path(__file__).resolve().parent))
 from cleanrl_b200 import _lib, build, ops  # noqa: E402
 
-KERNELS = ("conv1_fwd", "conv23_fwd", "conv3_dgrad", "conv21_bwd", "fc_fwd", "fc_dgrad", "fc_wgrad")
+KERNELS = ("conv1_fwd", "conv23_fwd", "conv3_wgrad", "conv3_dgrad", "conv2_wgrad", "conv21_bwd", "fc_fwd", "fc_dgrad",
+           "fc_wgrad")
 # a library built before conv2 and conv3 forward were fused reports them as two launches (A/B runs against it)
 OLD_NAMES = {"conv23_fwd": ("conv2_fwd", "conv3_fwd")}
 

@@ -25,9 +25,11 @@
 //       the epilogue; ReLU masks are exchanged between forward and backward as bits.
 //   tc_conv23_fwd                conv2 -> conv3 forward in one persistent kernel, one image per tile: conv2's epilogue
 //       writes act2 into a shared-memory operand image that conv3's MMAs read (and to HBM for the backward).
-//   tc_wgrad_win                 conv weight gradients: dW^T[(tap,c), co] = sum_r X[r+shift_tap, c] * dY[r, co]; the same
+//   tc_wgrad_rows / tc_wgrad_win conv weight gradients: dW^T[(tap,c), co] = sum_r X[r+shift_tap, c] * dY[r, co]; the same
 //       row images are read as MN-major operands (rows = reduction index), taps again by row shifts; the bias
-//       gradient (column sums of dY) is accumulated by the four dY warps from the staged tiles.
+//       gradient (column sums of dY) is accumulated by the four dY warps from the staged tiles.  tc_wgrad_rows (conv2,
+//       conv3) puts dY^T on the M side and a whole kernel row of taps on N; tc_wgrad_win (conv1 on bf16 frames) takes
+//       image-aligned steps through the minibatch gather.
 //   tc_gemm_tma<BN,STAGES>       fc forward / data-gradient: both operands are TMA boxes of row-major matrices.
 //   tc_wgrad_tma                 fc weight gradient (MN-major views of TMA-loaded dhid / act3 row boxes).
 //   tc_heads_*                   the A+1 head outputs in fp32 on CUDA cores (A+1 <= kMaxHeads).
@@ -176,35 +178,47 @@ static WPlan conv1_wgrad_plan(int64_t n, bool u8) {          // the uint8 kernel
 static WPlan conv2_wgrad_plan(int64_t n) { return wgrad_plan(n * 100, kC2Ctas, 128); }
 static WPlan conv3_wgrad_plan(int64_t n) { return wgrad_plan(n * 81, kC3Ctas, 128); }
 
-// scratch of launch_wgrad_win (and of the uint8 conv1 weight gradient, nslots = 4): dW partials ws[splits][nslots*64][64]
-// in the big region, bias partials wsb[splits][64] in the small one
+// scratch of the window weight gradients (launch_wgrad_win, launch_wgrad_rows and the uint8 conv1 weight gradient):
+// dW partials ws[splits][nslots*64][64] in the big region, bias partials wsb[splits][64] in the small one
 static size_t wgrad_win_bytes(int splits, int nslots) { return (size_t)splits * nslots * 64 * 64 * sizeof(float); }
 static size_t wgrad_win_bias_bytes(int splits) { return (size_t)splits * 64 * sizeof(float); }
+static int check_splits(int64_t M, int64_t rows_per_cta, int ctas, const char* what) {
+    if (rows_per_cta % 128 != 0) return fail(B200RL_ERR_INVALID_ARGUMENT, "%s: rows per CTA must be a multiple of 128", what);
+    if (ctas < 1 || (int64_t)(ctas - 1) * rows_per_cta >= M)
+        return fail(B200RL_ERR_INVALID_ARGUMENT, "%s: every row split must own at least one row", what);
+    return B200RL_OK;
+}
+// conv1 on bf16 frames: image-aligned steps (3-D TMA for X, cp.async for the 64-byte dY rows), one CTA per row split
 static int launch_wgrad_win(const WGradWinParams& p, int ctas, cudaStream_t s, const char* what) {
     const size_t smem = (size_t)kWgradWinStages * ((size_t)p.WRX * 128 * p.cpr + 128 * 128) + 4096 + 1024;
     static SmemAttrCache attr;
-    if (int rc0 = attr.ensure(tc_wgrad_win, smem, what)) return rc0;
+    int rc;
+    if ((rc = attr.ensure(tc_wgrad_win, smem, what))) return rc;
+    if ((rc = check_splits(p.M, p.rows_per_cta, ctas, what))) return rc;
+    if (p.nslots != 4) return fail(B200RL_ERR_INVALID_ARGUMENT, "%s: the wgmma warpgroups take 2 output tiles of 2 slots", what);
+    if ((128 << p.tpi_shift) < p.G) return fail(B200RL_ERR_INVALID_ARGUMENT, "%s: steps per image too small", what);
+    CUtensorMap tmX;
+    memset(&tmX, 0, sizeof(tmX));
+    if ((rc = make_tmap_3d(&tmX, p.X, p.n_images, p.G, (int64_t)p.cpr * 64, p.WRX, what))) return rc;
+    tc_wgrad_win<<<ctas, kWgradWinThreads, smem, s>>>(tmX, p);
+    return check_launch(what);
+}
+// conv2 / conv3 on the linear grid: X [M, 64 CPR] and dY [M, 64] (bf16), one CTA per split of plan `pl`
+template <int CPR, int KROWS, int TPR, int WP, int NCW>
+static int launch_wgrad_rows(const bf16* X, const bf16* Y, int64_t M, const WPlan& pl, float* ws, float* wsb, cudaStream_t s,
+                             const char* what) {
+    using C = WgradRowsCfg<CPR, KROWS, TPR, WP, NCW>;
+    static SmemAttrCache attr;
+    int rc;
+    if ((rc = attr.ensure(tc_wgrad_rows<CPR, KROWS, TPR, WP, NCW>, C::kSmem, what))) return rc;
+    if ((rc = check_splits(M, pl.rows_per_cta, pl.splits, what))) return rc;
     CUtensorMap tmX, tmY;
     memset(&tmX, 0, sizeof(tmX)); memset(&tmY, 0, sizeof(tmY));
-    // TMA when rows are contiguous, dY rows are exactly 128 bytes and every CTA owns whole 128-row steps
-    // all-TMA when dY rows are exactly 128 bytes; image-aligned steps (3-D TMA for X, cp.async for dY) otherwise
-    const int use_tma = p.tpi_shift ? 0 : 1;
-    if (p.rows_per_cta % 128 != 0) return fail(B200RL_ERR_INVALID_ARGUMENT, "%s: rows per CTA must be a multiple of 128", what);
-    if (ctas < 1 || (int64_t)(ctas - 1) * p.rows_per_cta >= p.M)
-        return fail(B200RL_ERR_INVALID_ARGUMENT, "%s: every row split must own at least one row", what);
-    int rc;
-    if (use_tma) {
-        if (p.rows || p.ldy != 64 || p.ncolsY != 64)
-            return fail(B200RL_ERR_INVALID_ARGUMENT, "%s: linear-grid mode needs contiguous rows and 64-channel dY", what);
-        if ((rc = make_tmap_2d(&tmX, p.X, p.M, (int64_t)p.cpr * 64, p.WRX, what))) return rc;
-        if ((rc = make_tmap_2d(&tmY, p.Y, p.M, 64, 128, what))) return rc;
-    } else {
-        if ((128 << p.tpi_shift) < p.G) return fail(B200RL_ERR_INVALID_ARGUMENT, "%s: steps per image too small", what);
-        if ((rc = make_tmap_3d(&tmX, p.X, p.n_images, p.G, (int64_t)p.cpr * 64, p.WRX, what))) return rc;
-    }
-    // x = the output-tile group, y = the row split: the CTAs that share a split's rows are launched next to each other
-    const dim3 grid((unsigned)ceil_div(p.nslots / 2, kWgradWinTilesPerCta), ctas);
-    tc_wgrad_win<<<grid, kWgradWinThreads, smem, s>>>(tmX, tmY, p, use_tma);
+    if ((rc = make_tmap_2d(&tmX, X, M, (int64_t)CPR * 64, C::kWRX, what))) return rc;
+    if ((rc = make_tmap_2d(&tmY, Y, M, 64, 128, what))) return rc;
+    WGradRowsParams p;
+    p.M = M; p.rows_per_cta = pl.rows_per_cta; p.ws = ws; p.wsb = wsb;
+    tc_wgrad_rows<CPR, KROWS, TPR, WP, NCW><<<pl.splits, C::kThreads, C::kSmem, s>>>(tmX, tmY, p);
     return check_launch(what);
 }
 
@@ -275,27 +289,21 @@ static int trunk_bwd(const NatureLayout& L, const NatureActs& Q, const bf16* P, 
         { ProfScope ps(s, "fc_dgrad", 2.0 * n * 512 * 3136, (double)n * ((3136 + 512) * 2 + 392) + 512.0 * 3136 * 2);
           if ((rc = launch_gemm_tma<128, 3>(p, s, "naturecnn/fc_dgrad"))) return rc; }
     }
-    WGradWinParams gw;
     WinParams wp;
     FoldWin fw;
     // ---- conv3: dW from act2 windows x dact3 (9x9 grid), then dact2 = full correlation of padded dact3 with W3
     {
-        wgw_defaults(gw);
-        gw.X = act + Q.act2; gw.M = n * 81; gw.n = (int)n; gw.G = 81; gw.cpr = 1; gw.nslots = 10; gw.WRX = round8(128 + 20);
-        for (int t = 0; t < 9; ++t) gw.shift[t] = (t / 3) * 9 + (t % 3);
-        const int st[10] = {0, 1, 2, 3, 4, 5, 6, 7, 7, 8};      // slot 8 duplicates tap 7 so that tap 8 has a partner
-        for (int k = 0; k < 10; ++k) { gw.slot_tap[k] = st[k]; gw.slot_cc[k] = 0; }
-        gw.Y = act + Q.dact3a; gw.ldy = 64; gw.ncolsY = 64;
+        // 3 kernel rows of 3 taps (shifts 9 ky + kx) on one 64-channel chunk; one wgmma warpgroup per kernel row
         const WPlan pl = conv3_wgrad_plan(n);
-        gw.rows_per_cta = pl.rows_per_cta; gw.ws = wsbig; gw.wsb = wssmall;
         { ProfScope ps(s, "conv3_wgrad", 2.0 * n * 49 * 64 * 576, (double)n * (5184 + 5184) * 2);
-          if ((rc = launch_wgrad_win(gw, pl.splits, s, "naturecnn/conv3_wgrad"))) return rc; }
+          if ((rc = launch_wgrad_rows<1, 3, 3, 9, 3>(act + Q.act2, act + Q.dact3a, n * 81, pl, wsbig, wssmall, s,
+                                                      "naturecnn/conv3_wgrad"))) return rc; }
         memset(&fw, 0, sizeof(fw));
-        fw.layer = 3; fw.S = pl.splits; fw.nslots = 10; fw.Cout = 64; fw.scale = 1.f; fw.bscale = 1.f;
-        for (int k = 0; k < 10; ++k) { fw.slot_tap[k] = st[k]; fw.slot_skip[k] = (k == 8); }
+        fw.layer = 3; fw.S = pl.splits; fw.nslots = 9; fw.Cout = 64; fw.scale = 1.f; fw.bscale = 1.f;
+        for (int k = 0; k < 9; ++k) fw.slot_tap[k] = k;
         { ProfScope ps(s, "wgrad_fold_bias", 0, 0);
           fw.wsb = wssmall; fw.db = grads + L.c3b;
-          tc_fold_win<<<(unsigned)ceil_div(640 * 64 + 64, 32), 256, 0, s>>>(wsbig, fw, grads + L.c3w);
+          tc_fold_win<<<(unsigned)ceil_div(576 * 64 + 64, 32), 256, 0, s>>>(wsbig, fw, grads + L.c3w);
           if ((rc = check_launch("naturecnn/conv3_fold"))) return rc; }
         win_defaults(wp);
         wp.A = act + Q.dact3b; wp.n = (int)n; wp.G = 121; wp.Wp = 11; wp.M = n * 121; wp.ntaps = 9;
@@ -309,15 +317,12 @@ static int trunk_bwd(const NatureLayout& L, const NatureActs& Q, const bf16* P, 
     // ---- conv2: dW from act1 cell windows x dact2 (10x10 grid); dact1 = one N=128 GEMM over the 4 stride-parity
     //      classes (the 4 channel groups of a cell)
     {
-        wgw_defaults(gw);
-        gw.X = act + Q.act1; gw.M = n * 100; gw.n = (int)n; gw.G = 100; gw.cpr = 2; gw.nslots = 8; gw.WRX = round8(128 + 11);
-        gw.shift[0] = 0; gw.shift[1] = 1; gw.shift[2] = 10; gw.shift[3] = 11;
-        for (int k = 0; k < 8; ++k) { gw.slot_tap[k] = k >> 1; gw.slot_cc[k] = k & 1; }
-        gw.Y = act + Q.dact2a; gw.ldy = 64; gw.ncolsY = 64;
+        // 2 kernel rows of 2 taps (shifts 10 a + b) on each of the 2 channel chunks of a cell; one wgmma warpgroup per
+        // kernel row, both chunks
         const WPlan pl = conv2_wgrad_plan(n);
-        gw.rows_per_cta = pl.rows_per_cta; gw.ws = wsbig; gw.wsb = wssmall;
         { ProfScope ps(s, "conv2_wgrad", 2.0 * n * 81 * 64 * 512, (double)n * (12800 + 6400) * 2);
-          if ((rc = launch_wgrad_win(gw, pl.splits, s, "naturecnn/conv2_wgrad"))) return rc; }
+          if ((rc = launch_wgrad_rows<2, 2, 2, 10, 2>(act + Q.act1, act + Q.dact2a, n * 100, pl, wsbig, wssmall, s,
+                                                       "naturecnn/conv2_wgrad"))) return rc; }
         memset(&fw, 0, sizeof(fw));
         fw.layer = 2; fw.S = pl.splits; fw.nslots = 8; fw.Cout = 64; fw.scale = 1.f; fw.bscale = 1.f;
         for (int k = 0; k < 8; ++k) { fw.slot_tap[k] = k >> 1; fw.slot_cc[k] = k & 1; }
@@ -340,6 +345,8 @@ static int trunk_bwd(const NatureLayout& L, const NatureActs& Q, const bf16* P, 
 // scratch of trunk_bwd: the fc, conv3 and conv2 weight-gradient partials (big part); the fc bias column sums and the
 // conv bias partials (small part)
 static size_t trunk_big_bytes(int64_t n) {
+    // conv3 writes 9 slots; 10 stay reserved so that the workspace size reported to callers (and allocated by them, at
+    // small n this term is the largest) is the one earlier releases reported
     return std::max({wgrad_tma_bytes(n, 512, 3136), wgrad_win_bytes(conv3_wgrad_plan(n).splits, 10),
                      wgrad_win_bytes(conv2_wgrad_plan(n).splits, 8)});
 }

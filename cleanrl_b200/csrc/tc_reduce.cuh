@@ -34,8 +34,8 @@ __device__ __forceinline__ float zlane_sum(const float* __restrict__ part, int64
 // fold for the window weight gradients: ws[S][nslots*64][64] -> torch layout dst[co][c][ky][kx].
 //   layer 1: slot = tap (a,b); row channel q = c*16 + sy*4 + sx; ky = 4a+sy, kx = 4b+sx; 32 outputs, Cin 4, 8x8
 //   layer 2: slot = (tap (a,b), cc); q = cc*64 + row = (py*2+px)*32 + c; ky = 2a+py, kx = 2b+px; Cin 32, 4x4
-//   layer 3: slot -> tap (ky,kx) via slot_tap (a duplicate slot is skipped); q = c; Cin 64, 3x3
-struct FoldWin { int layer, S, nslots, Cout; int slot_tap[16], slot_cc[16], slot_skip[16]; float scale;
+//   layer 3: slot -> tap (ky,kx) via slot_tap; q = c; Cin 64, 3x3
+struct FoldWin { int layer, S, nslots, Cout; int slot_tap[16], slot_cc[16]; float scale;
                  float bscale;     // scale of the bias gradient (1, or 1 / kDact1Scale when dY was stored scaled)
                  const float* wsb; float* db; };
 static __global__ void __launch_bounds__(256) tc_fold_win(const float* __restrict__ ws, const FoldWin f, float* __restrict__ dst) {
@@ -51,9 +51,8 @@ static __global__ void __launch_bounds__(256) tc_fold_win(const float* __restric
     }
     const int xi = idx / f.Cout, co = idx - xi * f.Cout;
     const int slot = xi >> 6, row = xi & 63;
-    const bool valid = !f.slot_skip[slot];
-    float s = zlane_sum(ws, (int64_t)KX * 64, f.S, (int64_t)xi * 64 + co, valid, red);
-    if (!valid || threadIdx.x >= 32) return;
+    float s = zlane_sum(ws, (int64_t)KX * 64, f.S, (int64_t)xi * 64 + co, true, red);
+    if (threadIdx.x >= 32) return;
     s *= f.scale;
     const int tap = f.slot_tap[slot];
     int64_t o;

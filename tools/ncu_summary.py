@@ -65,7 +65,9 @@ def main():
         elif short.startswith("tc_conv_win<64, 2"): layer = "conv2_fwd"
         elif short.startswith("tc_conv_win<64, 1"): layer = "conv3_fwd" if k % 2 == 0 else "conv3_dgrad"
         elif short.startswith("tc_conv_win<128"): layer = "conv2_dgrad"
-        elif short.startswith("tc_wgrad_win"): layer = ["conv3_wgrad", "conv2_wgrad", "conv1_wgrad"][k % (2 if u8 else 3)]
+        elif short.startswith("tc_wgrad_rows<1"): layer = "conv3_wgrad"
+        elif short.startswith("tc_wgrad_rows<2"): layer = "conv2_wgrad"
+        elif short.startswith("tc_wgrad_win"): layer = "conv1_wgrad"
         elif short.startswith("tc_gemm_tma<256"): layer = "fc_fwd" if k % 2 == 0 else "fc_dgrad"
         elif short.startswith("tc_wgrad_tma"): layer = "fc_wgrad"
         e = {"id": int(r[col["ID"]]), "kernel": short, "layer": layer, "grid": grid,
