@@ -554,14 +554,14 @@ extern "C" int b200rl_naturecnn_bf16_backward(const void* obs, const void* obs_a
     const bool u8 = obs_format == B200RL_OBS_S2D_U8;
     const WPlan pl = conv1_wgrad_plan(n, u8);
     if (u8) {
-        // conv2 data gradient (fp16 x kDact1Scale) + uint8 channel-major frames -> fp16 wgmma operands in registers
-        // (tc_conv1_u8.cuh); 1 CTA per SM
+        // conv2 data gradient (fp16 x kDact1Scale) + the row-major uint8 frames expanded to an fp16 wgmma operand in
+        // shared memory (tc_conv1_u8.cuh); 1 CTA per SM.  obs_aux (the channel-major copy) is not read.
         Conv21BwdU8Params cw;
         memset(&cw, 0, sizeof(cw));
         cw.rows = rows; cw.n = (int)n; cw.rows_per_cta = pl.rows_per_cta; cw.ws = wsbig; cw.wsb = wssmall;
         cw.w2dg = P + L.w2dg; cw.m1 = reinterpret_cast<const uint32_t*>(act + Q.m1);
-        { ProfScope ps(s, "conv21_bwd", 2.0 * 2.0 * n * 400 * 32 * 256, (double)n * (7744 * 2 + 1600 + 28672 + 14112 * 2));
-          if ((rc = launch_conv21_bwd_u8(cw, obs_aux, rows ? (int64_t)1 << 24 : n, act + Q.dact2b, act + Q.dact1, pl.splits, s,
+        { ProfScope ps(s, "conv21_bwd", 2.0 * 2.0 * n * 400 * 32 * 256, (double)n * (7744 * 2 + 1600 + 28224 + 14112 * 2));
+          if ((rc = launch_conv21_bwd_u8(cw, obs, rows ? (int64_t)1 << 24 : n, act + Q.dact2b, act + Q.dact1, pl.splits, s,
                                          "naturecnn/conv21_bwd_u8"))) return rc; }
     } else {
         WGradWinParams gw;

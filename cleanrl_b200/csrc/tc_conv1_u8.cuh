@@ -1,9 +1,9 @@
 // conv1 straight from the uint8 rollout (no 16-bit copy of the frames anywhere).
 //
-// The rollout keeps every frame ONCE as uint8 space-to-depth(4) pixels, 28 224 B per frame (the algorithmic
-// minimum; reference: a 14.8 GB fp32 buffer, ppo_atari_envpool.py:203):
-//     frames    u8 [img][441 grid rows][64 ch]   row-major    -> forward  (K-major operand rows)
-//     frames_t  u8 [img][64 ch][448 grid rows]   channel-major -> weight gradient (lanes = channels, K = rows)
+// The rollout keeps every frame as uint8 space-to-depth(4) pixels, 28 224 B per frame (the algorithmic minimum;
+// reference: a 14.8 GB fp32 buffer, ppo_atari_envpool.py:203):
+//     frames    u8 [img][441 grid rows][64 ch]   row-major    -> forward and weight gradient
+//     frames_t  u8 [img][64 ch][448 grid rows]   channel-major (still written by tc_frames_to_s2d_u8; no kernel reads it)
 //
 // Forward  tc_conv1_i8: integer tensor cores (wgmma u8 x s8 -> s32, accumulators in registers).  The
 //   pixels are EXACT (0..255 are integers); the fp32 master weights are split per output channel into two signed
@@ -16,12 +16,12 @@
 //   shifted by whole 64-byte rows of a SWIZZLE_64B image.
 //
 // Weight gradient  tc_conv21_bwd_u8 (which first computes dY, the conv2 data gradient, into shared memory):
-//   dW[tap, c, co] = sum_p X[p + off_tap, c] * dY[p, co].  The pixels go
-//   uint8 (shared memory, channel-major TMA box) -> fp16 pairs in REGISTERS (one PRMT per two pixels builds
-//   1024 + x; the offset is removed once per CTA through the bias partial), and are consumed as the A operand straight
-//   from registers (wgmma with A in registers); dY rows are a SWIZZLE_64B shared-memory image used as an MN-major B
-//   operand, read at two row offsets (0 and -21) so that one A fragment serves all four taps.  No 16-bit image of the
-//   frames ever exists in shared or global memory.
+//   dW[tap, c, co] = sum_p X[p + off_tap, c] * dY[p, co].  The row-major pixels go
+//   uint8 (shared memory, TMA boxes of pair rows) -> fp16 1024 + x (one PRMT per two pixels, by a warpgroup of their
+//   own, into a SWIZZLE_128B shared-memory image one step ahead of the MMAs; the offset is removed once per CTA through
+//   the bias partial), and are consumed as the MN-major B operand (N = 128: both pixel streams X[k], X[k + 1] through
+//   LBO = one row); the A operand is the dY image, read at two row offsets (0 and -21) so that one MMA serves all four
+//   taps.  Both operands come from shared memory, so the MMAs of one step run while the next step is expanded.
 #pragma once
 #include "tc_base.cuh"
 #include <cuda_fp16.h>
@@ -286,27 +286,29 @@ __global__ void __launch_bounds__(kConv1I8Threads, 1) tc_conv1_i8(const __grid_c
 // conv2 data gradient (warpgroup 1), per image: d(act1) = the full correlation of the zero-padded 11x11 d(act2) grid
 //   with the four stride-parity classes of W2 (one N = 128 GEMM, K = 4 taps x 64 channels), exactly as the window
 //   convolution tc_conv_win runs it: a TMA window of 140 rows of the image's d(act2) rows (128 GEMM rows + the largest tap
-//   shift of 12 rows), resident weights, m64n128k16 MMAs in the same tap and K order.  The epilogue (act1 > 0 mask, x
+//   shift of 12 rows) and, with it, one bulk copy of the image's act1 > 0 mask bits (1600 B; read from HBM by the
+//   epilogue itself, they stalled it), resident weights, m64n128k16 MMAs in the same tap and K order.  The epilogue (act1 > 0 mask, x
 //   kDact1Scale, saturating fp16) writes the image as the dY operand of the weight gradient straight into shared memory,
 //   and one TMA store per 128 rows copies it to d(act1) in HBM.
 // conv1 weight gradient (warpgroups 2 and 3): dW[tap, c, co] = sum_p X[p + off_tap, c] * dY[p, co] over the grid
 //   positions p of an image, off = {0, 1, 21, 22} (taps (dy, dx) of the 2x2 window on the 21-wide grid).  Written over
 //   k = p + s_b with s_b = {0, 21}:
-//       D_b[(h, c), co] = sum_k X[k + h, c] * dY[k - s_b, co],    tap = 2 b + h.
-//   A  (registers, 64 rows x 16 K per wgmma): warpgroup h holds channel c of the pixel stream X[k + h] as fp16 fragments;
-//       one fragment per K-step serves both tap groups b.
-//   B  (shared memory, MN-major SWIZZLE_64B): the dY rows of the step, rows [k0, k0 + 128) for b = 0 and rows
-//       [k0 - 21, k0 + 107) for b = 1, as ONE N = 64 operand: MN atom 0 (columns 0-31) starts at row k0 - 21 for b = 1,
-//       atom 1 (columns 32-63) 21 rows later for b = 0.  A dY image is [24-row zero halo | 512 rows] of 64 B: rows of
-//       positions that are not conv2 outputs (x = 20 or y = 20) and rows 441..511 stay zero, so the b = 1 operand of an
-//       image's first step and the padding rows of its last step read zeros.  Two dY images alternate, so the data
-//       gradient of image j + 1 runs under the weight gradient of image j.
-//   X  : channel-major frames [img][64 ch][448 rows] u8, staged in blocks of 128 positions (SWIZZLE_128B boxes of 64 full
-//        lines).  The h = 1 stream needs one pixel of the next block.
+//       D[(b, co), (h, c)] = sum_k dY[k - s_b, co] * X16[k + h, c],    tap = 2 b + h,
+//   one m64n128k16 per 16 positions, both operands in shared memory:
+//   A  (M = 64, MN-major SWIZZLE_64B): the dY rows of the step, rows [k0 - 21, k0 + 107) for b = 1 (MN atom 0, co 0-31)
+//       and rows [k0, k0 + 128) for b = 0 (atom 1, 21 rows = LBO later).  A dY image is [24-row zero halo | 512 rows] of
+//       64 B: rows of positions that are not conv2 outputs (x = 20 or y = 20) and rows 441..511 stay zero, so the b = 1
+//       operand of an image's first step and the padding rows of its last step read zeros.  Two dY images alternate, so
+//       the data gradient of image j + 1 runs under the weight gradient of image j.
+//   B  (N = 128, MN-major SWIZZLE_128B): X16, an fp16 image of the step's pixels, one 128-byte row (64 channels) per
+//       position k0 .. k0 + 128.  The h = 1 atom is the same rows one position on: LBO = 128 B.
+//   X  : the row-major frames [img][441][64] u8 that conv1 forward reads, as pair rows of 128 B: per step two TMA boxes
+//        of 33 pair rows (positions k0 + 64 hb .. k0 + 64 hb + 65).  Position 441 of an image is the first pixel of the
+//        next one (the second half of pair row 220) and pair rows >= 221 are zero-filled: both meet zero dY rows.
 //   dY : d(act1) on the 21x21 grid, fp16 [img][441][32] scaled by 2^12 (saturating conversion).
-//   The wgmma warps read their channel rows with 16-byte loads and expand uint8 -> fp16 with PRMTs (bytes (x, 0x64) =
-//   fp16 1024 + x; the offset is taken out again through the bias partial).  After publishing an image, warpgroup 1
-//   accumulates the bias gradient (column sums of dY) from it.  Partial tiles go to ws[cta][256][64] / wsb[cta][64]
+//   Warpgroup 3 expands the bytes to X16 with PRMTs (bytes (x, 0x64) = fp16 1024 + x; the offset is taken out again
+//   through the bias partial) one step ahead of the MMAs, which warpgroup 2 issues.  After publishing an image, warpgroup
+//   1 accumulates the bias gradient (column sums of dY) from it.  Partial tiles go to ws[cta][256][64] / wsb[cta][64]
 //   (first 32 columns used; row = tap * 64 + c) and are folded in fixed order by tc_fold_win.
 // Every output is bit-identical to the conv2 data gradient on tc_conv_win followed by a conv1 weight gradient that reads
 // d(act1) back: the same bf16 / fp16 products, the same fp32 accumulation order, the same CTA row ranges.
@@ -319,14 +321,21 @@ struct Conv21BwdU8Params {
     float* ws;
     float* wsb;
 };
-// X blocks (8 KB: 64 channels x 128 positions) in flight; with the resident conv2 weights (64 KB), two d(act2) windows and
-// two dY images, six blocks fill the 227 KB of shared memory
-constexpr int kC1WXStages = 6, kC21WinStages = 2;
-constexpr int kC1WBlock = 64 * 128, kC1WYBytes = 128 * 64, kC1WYPadRows = 24, kC1WYPad = kC1WYPadRows * 64;
+// u8 blocks of 33 pair rows (half a step and the h = 1 halo) in flight, and two fp16 pixel images of 129 rows (136: the
+// 1 KB swizzle period); with the resident conv2 weights (64 KB), two d(act2) windows and two dY images they fill the 227 KB
+// of shared memory
+constexpr int kC1WXStages = 4, kC21WinStages = 2;
+constexpr int kC1WXRows = 33, kC1WXBytes = kC1WXRows * 128, kC1WF16Bytes = 136 * 128;
+constexpr int kC1WYBytes = 128 * 64, kC1WYPadRows = 24, kC1WYPad = kC1WYPadRows * 64;
 constexpr int kC1WShift = 21;                     // grid rows between the two tap groups
 constexpr int kC21WinRows = 140, kC21WinBytes = 18 * 1024;      // 128 rows + the largest tap shift (12), 1 KB aligned
 constexpr int kC21W2Bytes = 4 * 128 * 128;                       // 4 taps x 128 output columns x 64 channels (bf16)
 constexpr int kC21ImgBytes = kC1WYPad + 4 * kC1WYBytes;          // zero halo + 512 rows of 64 B
+constexpr int kC21MaskBytes = 100 * 16;                           // act1 > 0 bits of one image: 100 cells x 4 words
+constexpr size_t kC21Smem = (size_t)kC21W2Bytes + (size_t)kC21WinStages * (kC21WinBytes + kC21MaskBytes) + 2 * (size_t)kC21ImgBytes +
+                            2 * (size_t)kC1WF16Bytes + (size_t)kC1WXStages * kC1WXBytes + 1024;
+static_assert(kC21Smem + 4608 <= 227 * 1024, "conv21_bwd: shared memory exceeds 227 KB");
+static_assert((kC21W2Bytes + kC21WinStages * kC21WinBytes + 2 * kC21ImgBytes) % 1024 == 0, "the fp16 images need 1 KB alignment");
 constexpr float kDact1Scale = 4096.0f;
 
 __device__ __forceinline__ uint32_t prmt(uint32_t a, uint32_t b, uint32_t sel) {
@@ -337,23 +346,22 @@ __device__ __forceinline__ uint32_t prmt(uint32_t a, uint32_t b, uint32_t sel) {
 // uint8 x -> fp16 1024 + x: 0..255 stay exact; sum_k (1024 + x) dY = dW + 1024 sum_k dY, and sum_k dY is the bias partial
 // the same CTA computes anyway, so the drain subtracts 1024 x it (fp32; the offset costs < 1e-5 relative accuracy).
 constexpr float kU8Bias = 1024.0f;
-
-
-// fp16 pair (1024 + x[pos], 1024 + x[pos + 1]) from the 20-byte window w[0..4], pos = 4 (j + up) + b: the lane-dependent
-// word choice is one select per word on a per-thread constant (an indexed array would go to local memory, and a chain of
-// comparisons compiles to branches), and `sel` = b | (b + 1) << 4 picks the two bytes
-__device__ __forceinline__ uint32_t pair_f16_biased(const uint32_t (&w)[5], int j, bool up, uint32_t sel) {
-    const uint32_t lo = up ? w[j + 1] : w[j];
-    const uint32_t hi = up ? w[j + 2] : w[j + 1];
-    return prmt(prmt(lo, hi, sel), 0x64646464u, 0x5140u);
+// 16 pixels -> two 16-byte chunks of fp16 1024 + x (pixels 0-7, 8-15): one PRMT per two pixels
+__device__ __forceinline__ void u8x16_to_f16_biased(const uint4& v, uint4& lo, uint4& hi) {
+    constexpr uint32_t k64 = 0x64646464u;
+    lo = make_uint4(prmt(v.x, k64, 0x5140u), prmt(v.x, k64, 0x7362u), prmt(v.y, k64, 0x5140u), prmt(v.y, k64, 0x7362u));
+    hi = make_uint4(prmt(v.z, k64, 0x5140u), prmt(v.z, k64, 0x7362u), prmt(v.w, k64, 0x5140u), prmt(v.w, k64, 0x7362u));
 }
 // 16 bytes at a shared-memory address.  The staging pointers come from the 1 KB-aligned dynamic shared memory through an
-// integer cast, so plain dereferences compile to generic 64-bit loads; these are LDS.128 with 32-bit addresses.  volatile
-// + memory: the loads stay between the mbarrier wait that publishes the block and the arrive that releases it.
+// integer cast, so plain dereferences compile to generic 64-bit loads; these are LDS.128 / STS.128 with 32-bit addresses.
+// volatile + memory: the accesses stay between the mbarrier wait that publishes a buffer and the arrive that releases it.
 __device__ __forceinline__ uint4 lds128(uint32_t addr) {
     uint4 v;
     asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
     return v;
+}
+__device__ __forceinline__ void sts128(uint32_t addr, const uint4& v) {
+    asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
 // fp32 pair -> fp16x2, saturating to +-65504 (d(act1) x kDact1Scale never becomes inf)
 __device__ __forceinline__ uint32_t pack_f16x2_sat(float lo, float hi) {
@@ -371,34 +379,39 @@ __device__ __forceinline__ void tma_store_3d(const void* tmap, uint32_t smem_src
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
 template <int N> __device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+// bulk copy global -> shared (16-byte aligned, a multiple of 16 bytes); completion is signalled on `bar` (complete_tx)
+__device__ __forceinline__ void bulk_load(uint32_t smem_dst, const void* src, uint32_t bytes, uint64_t* bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(smem_dst), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
+}
 
-// Per-warpgroup register budgets (setmaxnreg): the kernel launches at 128 registers per thread (512 threads, 1 CTA per
-// SM); the producer warpgroup gives registers back to the weight-gradient warpgroups, whose fragment build then keeps more
-// shared-memory loads in flight.  The data-gradient warpgroup (64 accumulators) keeps the 128 it launched with.
-constexpr int kC1WRegsProducer = 40, kC21RegsDgrad = 128, kC1WRegsMma = 168;
-static_assert(128 * kC1WRegsProducer + 128 * kC21RegsDgrad + 256 * kC1WRegsMma <= 65536, "register budgets exceed the SM");
-
-// 512 threads: warp 0 = X producer, warp 1 = d(act2) window producer (warps 2-3 idle: warpgroup alignment), warpgroup 1 =
-// conv2 data gradient + bias sums, warpgroups 2 and 3 = wgmma for the pixel streams h = 0 and h = 1
+// 512 threads: warp 0 = pixel producer, warp 1 = d(act2) window producer (warps 2-3 idle: warpgroup alignment), warpgroup
+// 1 = conv2 data gradient + bias sums, warpgroup 2 = weight-gradient wgmma, warpgroup 3 = uint8 -> fp16 pixel expansion.
+// Every warpgroup keeps the 128 registers per thread the launch gives it (the wgmma warpgroups hold 64 accumulators each).
 constexpr int kC1WThreads = 512;
 __global__ void __launch_bounds__(kC1WThreads, 1) tc_conv21_bwd_u8(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmWin,
                                                                  const __grid_constant__ CUtensorMap tmY, const Conv21BwdU8Params p) {
     constexpr int XS = kC1WXStages, WS = kC21WinStages;
     extern __shared__ uint8_t smem_raw[];
-    __shared__ uint64_t xfull[XS], xempty[XS], wfull[WS], wempty[WS], yfull[2], yempty[2];
+    __shared__ uint64_t xfull[XS], xempty[XS], wfull[WS], wempty[WS], yfull[2], yempty[2], ffull[2], fempty[2];
     __shared__ float sRed[32 * 32], sBias[32];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* sW2 = smem;                                       // conv2 data-gradient weights, 4 taps x 16 KB
     uint8_t* sWin = sW2 + kC21W2Bytes;                         // WS d(act2) windows
-    uint8_t* sX = sWin + (size_t)WS * kC21WinBytes;            // XS blocks of 8 KB
-    uint8_t* sImg = sX + (size_t)XS * kC1WBlock;               // 2 dY images (512-B aligned: the SWIZZLE_64B pattern)
+    uint8_t* sImg = sWin + (size_t)WS * kC21WinBytes;          // 2 dY images (512-B aligned: the SWIZZLE_64B pattern)
+    uint8_t* sF = sImg + 2 * (size_t)kC21ImgBytes;             // 2 fp16 pixel images (1 KB aligned: SWIZZLE_128B)
+    uint8_t* sX = sF + 2 * (size_t)kC1WF16Bytes;               // XS u8 blocks of 33 pair rows (unswizzled)
+    uint8_t* sM = sX + (size_t)XS * kC1WXBytes;                // WS images of act1 mask bits, one per d(act2) window
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     if (tid == 0) {
-        // X block k is read by all eight wgmma warps as step k's main block and by the four h = 1 warps as step k - 1's halo;
-        // a window is released by the four data-gradient warps, a dY image by the eight wgmma warps
-        for (int s = 0; s < XS; ++s) { mbar_init(&xfull[s], 1); mbar_init(&xempty[s], 12); }
+        // a u8 block is released by the four expansion warps, a window by the four data-gradient warps, an fp16 image and
+        // a dY image by the four wgmma warps once the MMAs that read them have completed
+        for (int s = 0; s < XS; ++s) { mbar_init(&xfull[s], 1); mbar_init(&xempty[s], 4); }
         for (int s = 0; s < WS; ++s) { mbar_init(&wfull[s], 1); mbar_init(&wempty[s], 4); }
-        for (int s = 0; s < 2; ++s) { mbar_init(&yfull[s], 1); mbar_init(&yempty[s], 8); }
+        for (int s = 0; s < 2; ++s) {
+            mbar_init(&yfull[s], 1); mbar_init(&yempty[s], 4);
+            mbar_init(&ffull[s], 4); mbar_init(&fempty[s], 4);
+        }
         fence_barrier_init();
         tma_prefetch_desc(&tmX);
         tma_prefetch_desc(&tmWin);
@@ -411,42 +424,44 @@ __global__ void __launch_bounds__(kC1WThreads, 1) tc_conv21_bwd_u8(const __grid_
     for (int idx = tid; idx < 2 * kC21ImgBytes / 16; idx += blockDim.x) reinterpret_cast<int4*>(sImg)[idx] = make_int4(0, 0, 0, 0);
     fence_proxy_async_smem();
     __syncthreads();
+    // every CTA owns at least one whole image (launch_conv21_bwd_u8 checks it): nsteps >= 4
     const int64_t M = (int64_t)p.n * 512;
     const int64_t m_begin = (int64_t)blockIdx.x * p.rows_per_cta;
     int64_t m_end = m_begin + p.rows_per_cta;
     if (m_end > M) m_end = M;
-    const int nsteps = m_end > m_begin ? (int)((m_end - m_begin) >> 7) : 0;
+    const int nsteps = (int)((m_end - m_begin) >> 7);
     const int nimg = nsteps >> 2;
-    const int64_t g0 = m_begin >> 7;                       // first global step (4 steps per image)
     const int img0 = (int)(m_begin >> 9);
 
     if (warp < 4) {
-        setmaxnreg_dec<kC1WRegsProducer>();
-        if (warp == 0 && lane == 0 && nsteps > 0) {
-            // =================== TMA producer 1: X block k (k = 0 .. nsteps, the last one only feeds the one-pixel halo)
-            auto image_of = [&](int64_t g) -> int {
-                int64_t img = g >> 2;
-                if (img >= p.n) img = p.n - 1;             // the halo block after the very last step: any mapped block will do
-                return p.rows ? (int)__ldg(p.rows + img) : (int)img;
-            };
-            // the gather index is fetched one IMAGE (four steps) ahead
-            int z = image_of(g0), z_next = image_of(g0 + 4);        // g0 is image-aligned (whole images per CTA)
-            for (int k = 0; k <= nsteps; ++k) {
-                const int64_t g = g0 + k;
-                if (k > 0 && (g & 3) == 0) { z = z_next; z_next = image_of(g + 4); }
-                const int xs = k % XS;
-                if (k >= XS) mbar_wait(&xempty[xs], ((k / XS) - 1) & 1);
-                mbar_arrive_expect_tx(&xfull[xs], (uint32_t)kC1WBlock);
-                tma_load_3d(smem_u32(sX + (size_t)xs * kC1WBlock), &tmX, (int)(g & 3) * 128, 0, z, &xfull[xs]);
+        if (warp == 0 && lane == 0) {
+            // =================== TMA producer 1: the pixels of step k (image-aligned: step k & 3 of its image) as two
+            // blocks of 33 pair rows, positions 128 (k & 3) + 64 hb .. + 65 (rows >= 221 are zero-filled)
+            auto image_of = [&](int j) -> int { return p.rows ? (int)__ldg(p.rows + img0 + j) : img0 + j; };
+            int z = 0, z_next = image_of(0);                   // the gather index is fetched one image ahead
+            for (int k = 0; k < nsteps; ++k) {
+                if ((k & 3) == 0) {
+                    z = z_next;
+                    if ((k >> 2) + 1 < nimg) z_next = image_of((k >> 2) + 1);
+                }
+#pragma unroll
+                for (int hb = 0; hb < 2; ++hb) {
+                    const int j = 2 * k + hb, xs = j % XS;
+                    if (j >= XS) mbar_wait(&xempty[xs], ((j / XS) - 1) & 1);
+                    mbar_arrive_expect_tx(&xfull[xs], (uint32_t)kC1WXBytes);
+                    tma_load_3d(smem_u32(sX + (size_t)xs * kC1WXBytes), &tmX, 0, (k & 3) * 64 + hb * 32, z, &xfull[xs]);
+                }
             }
         } else if (warp == 1 && lane == 0) {
             // =================== TMA producer 2: the d(act2) window of image j (rows 121 i .. 121 i + 139 of the padded
-            // 11x11 grids; rows past the last image are zero-filled)
+            // 11x11 grids; rows past the last image are zero-filled) and the image's act1 mask bits, which the epilogue
+            // would otherwise wait for from HBM
             for (int j = 0; j < nimg; ++j) {
                 const int s = j % WS;
                 if (j >= WS) mbar_wait(&wempty[s], ((j / WS) - 1) & 1);
-                mbar_arrive_expect_tx(&wfull[s], (uint32_t)(kC21WinRows * 128));
+                mbar_arrive_expect_tx(&wfull[s], (uint32_t)(kC21WinRows * 128 + kC21MaskBytes));
                 tma_load_2d(smem_u32(sWin + (size_t)s * kC21WinBytes), &tmWin, 0, (img0 + j) * 121, &wfull[s]);
+                bulk_load(smem_u32(sM + (size_t)s * kC21MaskBytes), p.m1 + (int64_t)(img0 + j) * 100 * 4, (uint32_t)kC21MaskBytes, &wfull[s]);
             }
         }
     } else if (warp < 8) {
@@ -460,6 +475,7 @@ __global__ void __launch_bounds__(kC1WThreads, 1) tc_conv21_bwd_u8(const __grid_
         for (int j = 0; j < nimg; ++j) {
             const int i = img0 + j, buf = j & 1, s = j % WS;
             const uint32_t img = smem_u32(sImg + (size_t)buf * kC21ImgBytes) + kC1WYPad;     // row 0 of the image
+            const uint32_t masks = smem_u32(sM + (size_t)s * kC21MaskBytes);
             mbar_wait(&wfull[s], (j / WS) & 1);
             // image j - 2 has left dY image `buf`: the weight gradient consumed it and its TMA store has read it
             if (j >= 2) mbar_wait(&yempty[buf], ((j >> 1) - 1) & 1);
@@ -480,7 +496,7 @@ __global__ void __launch_bounds__(kC1WThreads, 1) tc_conv21_bwd_u8(const __grid_
                     for (int kk = 0; kk < 4; ++kk) WgmmaBf16<128, 0, 0>::mma(d, a + 2 * kk, b + 2 * kk, (t | kk) != 0 ? 1u : 0u);
                 }
                 wgmma_commit();
-                // this thread's rows r and r + 8 of the 11x11 grid: cell (Y, X), its mask words, requested under the MMAs
+                // this thread's rows r and r + 8 of the 11x11 grid: cell (Y, X) and its mask words
                 int pos[2];
                 uint4 mb[2];
 #pragma unroll
@@ -490,14 +506,10 @@ __global__ void __launch_bounds__(kC1WThreads, 1) tc_conv21_bwd_u8(const __grid_
                     const bool valid = Y < 10 && X < 10;
                     pos[hr] = valid ? 2 * Y * 21 + 2 * X : -1;
                     mb[hr] = make_uint4(0u, 0u, 0u, 0u);
-                    if (valid) {
-                        const int4 t = ldg16(p.m1 + ((int64_t)i * 100 + Y * 10 + X) * 4);
-                        mb[hr] = make_uint4((uint32_t)t.x, (uint32_t)t.y, (uint32_t)t.z, (uint32_t)t.w);
-                    }
+                    if (valid) mb[hr] = lds128(masks + (uint32_t)(Y * 10 + X) * 16u);
                 }
                 wgmma_wait<0>();
                 wgmma_fence_operands(d);
-                if (h2 == 1 && lane == 0) mbar_arrive(&wempty[s]);
                 // epilogue on the accumulator fragment: column 8 jj + 2 qd (+1) = channel 8 (jj & 3) + 2 qd of class
                 // g = jj >> 2 = (py, px), stored at grid position (2 Y + py, 2 X + px) of the dY image
 #pragma unroll
@@ -514,6 +526,9 @@ __global__ void __launch_bounds__(kC1WThreads, 1) tc_conv21_bwd_u8(const __grid_
                         sts32(img + img64_off(q, c >> 3) + (uint32_t)((c & 7) * 2), pack_f16x2_sat(f0, f1));
                     }
                 }
+                // the window and the mask bits of this image have been read
+                __syncwarp();
+                if (h2 == 1 && lane == 0) mbar_arrive(&wempty[s]);
             }
             // publish: the wgmma operand reads and the TMA store are async-proxy reads of what this warpgroup just wrote
             fence_proxy_async_smem();
@@ -553,96 +568,119 @@ __global__ void __launch_bounds__(kC1WThreads, 1) tc_conv21_bwd_u8(const __grid_
             // b = 1 operand (shifted by 21, zero outside the image) sum to the same value as the rows of the b = 0 operand
             sBias[wt] = t * kU8Bias;
         }
-        named_bar(2, 384);                                  // sBias is ready for the wgmma warpgroups' drain
-    } else {
-        setmaxnreg_inc<kC1WRegsMma>();
-        // ======================= wgmma warpgroup h: A = fp16 fragments of the pixel stream X[k + h] built in registers,
-        // B = the step's dY rows at offsets -21 (b = 1, columns 0-31) and 0 (b = 0, columns 32-63) as one N = 64 operand;
-        // 8 K-steps of 16 positions per step.  Every accumulator column sees the same MMAs in the same K order as with two
-        // N = 32 MMAs per K-step, but a wgmma with A in registers holds the issuing warp for about as long as the MMA
-        // runs, and one m64n64k16 takes far less of that time than two m64n32k16.
-        //   d[4 j + e], j < 4: b = 1, channels 8 j + 2 qd (+1);  d[16 + 4 j + e]: b = 0, the same channels
-        const int h = (warp - 8) >> 2, wt = tid & 127, qd = lane & 3;
-        const int c0 = ((wt >> 5) << 4) + (lane >> 2);     // fragment rows c0 and c0 + 8 = channels
-        // this thread's pixel pairs start at byte 2 qd + h and 8 + 2 qd + h of each 16-position chunk: words (qd >> 1) [+ 2]
-        const bool up = qd >= 2;
-        const uint32_t pb = (uint32_t)((2 * qd + h) & 3), psel = pb | ((pb + 1) << 4);
-        float d[32];
+        named_bar(2, 256);                                  // sBias is ready for the wgmma warpgroup's drain
+    } else if (warp < 12) {
+        // ======================= wgmma warpgroup: 8 K-steps of 16 positions per step, m64n128k16 with A = the dY rows of
+        // both tap groups, B = X16 of both pixel streams.  Every dW element gets the products of the same steps and K16
+        // groups as with the pixels on the A side, and scale-d 0 only on the first MMA.
+        //   d[4 j + e]: (b, co) = row 16 (wt >> 5) + lane / 4 (+ 8 for e >= 2), (h, c) = column 8 j + 2 qd (+ 1 for odd e)
+        const int wt = tid & 127, qd = lane & 3;
+        float d[64];
 #pragma unroll
-        for (int e = 0; e < 32; ++e) d[e] = 0.f;
-        for (int it = 0; it < nsteps; ++it) {
-            const int xm = it % XS, xh = (it + 1) % XS, buf = (it >> 2) & 1;
-            mbar_wait(&xfull[xm], (it / XS) & 1);
-            if (h == 1) mbar_wait(&xfull[xh], ((it + 1) / XS) & 1);
-            uint32_t a[8][4];
-#pragma unroll
-            for (int r = 0; r < 2; ++r) {
-                const int c = c0 + 8 * r;
-                const uint32_t bm = smem_u32(sX + (size_t)xm * kC1WBlock + c * 128);
-                const uint32_t bh = smem_u32(sX + (size_t)xh * kC1WBlock + c * 128);
-                const uint32_t sw = (uint32_t)(c & 7);
-                uint4 cur = lds128(bm + ((0u ^ sw) << 4));
-#pragma unroll
-                for (int kk = 0; kk < 8; ++kk) {
-                    uint4 nxt = make_uint4(0, 0, 0, 0);
-                    if (h == 1) nxt = lds128((kk < 7 ? bm : bh) + ((((uint32_t)(kk + 1) & 7u) ^ sw) << 4));
-                    const uint32_t w[5] = {cur.x, cur.y, cur.z, cur.w, nxt.x};
-                    a[kk][r] = pair_f16_biased(w, 0, up, psel);             // K 2 qd, 2 qd + 1
-                    a[kk][2 + r] = pair_f16_biased(w, 2, up, psel);         // K 8 + 2 qd, 9 + 2 qd
-                    if (kk < 7) cur = h == 1 ? nxt : lds128(bm + ((((uint32_t)(kk + 1)) ^ sw) << 4));
-                }
-            }
-            // the pixels are in registers: release the X blocks (block 0 has no halo reader, so its h = 1 readers arrive twice)
-            __syncwarp();
-            if (lane == 0) {
-                mbar_arrive(&xempty[xm]);
-                if (h == 1) { mbar_arrive(&xempty[xh]); if (it == 0) mbar_arrive(&xempty[xm]); }
-            }
+        for (int e = 0; e < 64; ++e) d[e] = 0.f;
+        auto step = [&](int it) {                            // one batch of 8 MMAs on the images of step it, one commit group
+            const int fs = it & 1, buf = (it >> 2) & 1;
             if ((it & 3) == 0) mbar_wait(&yfull[buf], (it >> 3) & 1);
-            wgmma_fence();                                   // the A fragments were just written by ordinary instructions
+            mbar_wait(&ffull[fs], (it >> 1) & 1);
+            wgmma_fence();
             const uint32_t ystep = smem_u32(sImg + (size_t)buf * kC21ImgBytes) + (uint32_t)(kC1WYPad + (it & 3) * kC1WYBytes);
-            const uint64_t yd = desc_mnmajor_sw64(ystep - kC1WShift * 64, kC1WShift * 64);
+            const uint64_t ad = desc_mnmajor_sw64(ystep - kC1WShift * 64, kC1WShift * 64);
+            const uint64_t bd = desc_mnmajor(smem_u32(sF + (size_t)fs * kC1WF16Bytes), 128);
+            // K-step kk: 16 dY rows (1 KB, + 64 in the address field) and 16 X16 rows (2 KB, + 128)
 #pragma unroll
-            for (int kk = 0; kk < 8; ++kk) wgmma_f16_rs_n64_tb(d, a[kk], yd + 64 * kk, (it | kk) != 0 ? 1u : 0u);
+            for (int kk = 0; kk < 8; ++kk) WgmmaF16N128<1, 1>::mma(d, ad + 64 * kk, bd + 128 * kk, (it | kk) != 0 ? 1u : 0u);
             wgmma_commit();
-            wgmma_wait<0>();
-            if ((it & 3) == 3 && lane == 0) mbar_arrive(&yempty[buf]);
+        };
+        // Step it-1's fp16 image (and, after an image's last step, its dY image) is released once step it's batch has been
+        // issued and step it-1's MMAs have completed (wgmma_wait<1>), so the tensor pipe does not drain between steps.  The
+        // last step is peeled: its MMAs, the final wait and the accumulator stores then share one basic block.
+        for (int it = 0; it + 1 < nsteps; ++it) {
+            step(it);
+            wgmma_wait<1>();
+            if (it > 0 && lane == 0) {
+                mbar_arrive(&fempty[(it - 1) & 1]);
+                if (((it - 1) & 3) == 3) mbar_arrive(&yempty[((it - 1) >> 2) & 1]);
+            }
         }
+        step(nsteps - 1);
+        wgmma_wait<0>();
         wgmma_fence_operands(d);
-        named_bar(2, 384);
+        named_bar(2, 256);
+        // accumulator element ((b, co), (h, c)) -> ws[cta][(2 b + h) * 64 + c][co], the layout of the channels on M; rows
+        // 0-31 of the tile are b = 1, rows 32-63 b = 0
+        const int m = ((wt >> 5) << 4) + (lane >> 2), b = m < 32 ? 1 : 0, co = m & 31;
+        const float bias0 = sBias[co], bias8 = sBias[co + 8];
         float* wsc = p.ws + (int64_t)blockIdx.x * 256 * 64;
 #pragma unroll
-        for (int b = 0; b < 2; ++b) {
+        for (int j = 0; j < 16; ++j) {
+            const int h = j >> 3, c = 8 * (j & 7) + 2 * qd;
+            float* q = wsc + (int64_t)((2 * b + h) * 64 + c) * 64 + co;
+            q[0] = d[4 * j] - bias0;
+            q[64] = d[4 * j + 1] - bias0;
+            q[8] = d[4 * j + 2] - bias8;
+            q[64 + 8] = d[4 * j + 3] - bias8;
+        }
+    } else {
+        // ======================= pixel expansion, one step ahead of the MMAs: X16 row r = position k0 + r, r = 0 .. 128,
+        // from block hb = r / 64 (row 128, the h = 1 halo, is position 64 of the second block).  Thread wt expands the
+        // 16-byte chunks t = wt + 128 i (position t / 4 of the block, channels 16 (t & 3) ..) into chunks 2 (t & 3) and
+        // 2 (t & 3) + 1 of the row; 8 consecutive threads read 128 contiguous bytes and write two whole rows.
+        const int wt = tid & 127;
+        for (int it = 0; it < nsteps; ++it) {
+            const int fs = it & 1;
+            const uint32_t img = smem_u32(sF + (size_t)fs * kC1WF16Bytes);
+            if (it >= 2) mbar_wait(&fempty[fs], ((it >> 1) - 1) & 1);
 #pragma unroll
-            for (int r = 0; r < 2; ++r) {
-                float* dst = wsc + (int64_t)((2 * b + h) * 64 + c0 + 8 * r) * 64;
+            for (int hb = 0; hb < 2; ++hb) {
+                const int j = 2 * it + hb, xs = j % XS;
+                const uint32_t blk = smem_u32(sX + (size_t)xs * kC1WXBytes);
+                const int nch = (64 + hb) * 4;               // 16-byte chunks used from this block
+                mbar_wait(&xfull[xs], (j / XS) & 1);
+                uint4 v[3];
 #pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    const int co = 8 * j + 2 * qd, e = (b == 0 ? 16 : 0) + 4 * j + 2 * r;
-                    *reinterpret_cast<float2*>(dst + co) = make_float2(d[e] - sBias[co], d[e + 1] - sBias[co + 1]);
+                for (int i = 0; i < 2 + hb; ++i)
+                    if (wt + 128 * i < nch) v[i] = lds128(blk + (uint32_t)(wt + 128 * i) * 16u);
+#pragma unroll
+                for (int i = 0; i < 2 + hb; ++i) {
+                    const int t = wt + 128 * i;
+                    if (t < nch) {
+                        const int r = 64 * hb + (t >> 2), c = t & 3;
+                        uint4 lo, hi;
+                        u8x16_to_f16_biased(v[i], lo, hi);
+                        sts128(img + (uint32_t)(r * 128 + (((2 * c) ^ (r & 7)) << 4)), lo);
+                        sts128(img + (uint32_t)(r * 128 + (((2 * c + 1) ^ (r & 7)) << 4)), hi);
+                    }
                 }
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&xempty[xs]);
             }
+            // publish: the wgmma operand reads are async-proxy reads of what this warp just wrote
+            fence_proxy_async_smem();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&ffull[fs]);
         }
     }
 }
 
-// dact2b: d(act2) on the zero-padded 11x11 grids [n,121,64] bf16; dact1: fp16 x kDact1Scale [n,441,32] (written here)
-static int launch_conv21_bwd_u8(const Conv21BwdU8Params& p, const void* frames_cm, int64_t n_images, const bf16* dact2b, void* dact1_f16,
+// dact2b: d(act2) on the zero-padded 11x11 grids [n,121,64] bf16; dact1: fp16 x kDact1Scale [n,441,32] (written here);
+// frames_rm: the row-major uint8 frames [n_images][441][64] (conv1 forward's input)
+static int launch_conv21_bwd_u8(const Conv21BwdU8Params& p, const void* frames_rm, int64_t n_images, const bf16* dact2b, void* dact1_f16,
                                 int ctas, cudaStream_t s, const char* what) {
-    const size_t smem = (size_t)kC21W2Bytes + (size_t)kC21WinStages * kC21WinBytes + (size_t)kC1WXStages * kC1WBlock + 2 * (size_t)kC21ImgBytes + 1024;
     int rc;
     if (p.rows_per_cta % 512 != 0) return fail(B200RL_ERR_INVALID_ARGUMENT, "%s: a CTA must own whole images (512 grid rows)", what);
+    if (ctas < 1 || (int64_t)(ctas - 1) * p.rows_per_cta >= (int64_t)p.n * 512)
+        return fail(B200RL_ERR_INVALID_ARGUMENT, "%s: every CTA must own at least one image", what);
     CUtensorMap tmX, tmWin, tmY;
     memset(&tmX, 0, sizeof(tmX)); memset(&tmWin, 0, sizeof(tmWin)); memset(&tmY, 0, sizeof(tmY));
-    // frames [img][64 ch][448 positions] u8: box = [64 ch][128 positions], SWIZZLE_128B; d(act2) rows [n * 121][64 ch] bf16:
-    // box = 140 rows, SWIZZLE_128B; dY [img][441 rows][32 co] fp16 = 64-byte rows: box [128 rows][64 B], SWIZZLE_64B (stores;
-    // rows >= 441 of a box are not written)
-    if ((rc = make_tmap_3d_u8(&tmX, frames_cm, n_images, 64, 448, 448, 64, 128, what))) return rc;
+    // frames as pair rows [img][221][128 B]: box = 33 pair rows, unswizzled; d(act2) rows [n * 121][64 ch] bf16: box = 140
+    // rows, SWIZZLE_128B; dY [img][441 rows][32 co] fp16 = 64-byte rows: box [128 rows][64 B], SWIZZLE_64B (stores; rows
+    // >= 441 of a box are not written)
+    if ((rc = make_tmap_pairs_u8(&tmX, frames_rm, n_images, kC1WXRows, false, what))) return rc;
     if ((rc = make_tmap_2d(&tmWin, dact2b, (int64_t)p.n * 121, 64, kC21WinRows, what))) return rc;
     if ((rc = make_tmap_3d_u8(&tmY, dact1_f16, p.n, 441, 64, 64, 128, 64, what))) return rc;
     static SmemAttrCache attr;
-    if ((rc = attr.ensure(tc_conv21_bwd_u8, smem, what))) return rc;
-    tc_conv21_bwd_u8<<<ctas, kC1WThreads, smem, s>>>(tmX, tmWin, tmY, p);
+    if ((rc = attr.ensure(tc_conv21_bwd_u8, kC21Smem, what))) return rc;
+    tc_conv21_bwd_u8<<<ctas, kC1WThreads, kC21Smem, s>>>(tmX, tmWin, tmY, p);
     return check_launch(what);
 }
 
@@ -658,7 +696,7 @@ static int launch_conv1_i8(const Conv1U8Params& p, const void* frames_rm, cudaSt
     memset(&tmW, 0, sizeof(tmW));
     // the row-major image [441][64 B] viewed as 221 pair rows of 128 B (image stride 28 224 B = 220.5 rows: the second
     // half of row 220 belongs to the next image and only ever feeds invalid positions); SWIZZLE_128B boxes of 144 rows
-    int rc = make_tmap_pairs_u8(&tmA, frames_rm, p.n_images, what);
+    int rc = make_tmap_pairs_u8(&tmA, frames_rm, p.n_images, 144, true, what);
     if (rc) return rc;
     // the limbs [64 rows][4 taps x 64 B]: one SWIZZLE_64B box [64 rows][64 B] per tap
     if ((rc = make_tmap_3d_u8(&tmW, p.limbs, 1, 64, 256, 256, 64, 64, what))) return rc;

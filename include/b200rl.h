@@ -306,9 +306,10 @@ enum { B200RL_OBS_U8_NCHW = 0, B200RL_OBS_S2D_BF16 = 1, B200RL_OBS_S2D_U8 = 2 };
 int b200rl_frames_to_s2d_bf16(const uint8_t* obs, const int64_t* rows, int64_t n, void* out_s2d, void* stream);
 /* B200RL_OBS_S2D_U8: the rollout keeps each frame as uint8 space-to-depth(4) pixels (28 224 B, the algorithmic minimum;
  * reference: fp32, 112 896 B, ppo_atari_envpool.py:203) in TWO orientations written once per env step:
- *   out_rm u8 [n, 441 grid rows, 64 channels]  -> `obs` of forward: conv1 on the integer tensor cores (kind::i8)
- *   out_cm u8 [n, 64 channels, 448 grid rows]  -> `obs_aux` of backward: conv1 weight gradient (pixels converted
- *                                                  uint8 -> fp16 in registers, fed to the MMA from tensor memory)
+ *   out_rm u8 [n, 441 grid rows, 64 channels]  -> `obs` of forward and backward: conv1 on the integer tensor cores
+ *                                                  (kind::i8) and the conv1 weight gradient (pixels expanded
+ *                                                  uint8 -> fp16 in shared memory)
+ *   out_cm u8 [n, 64 channels, 448 grid rows]  -> `obs_aux` of backward: required, no longer read
  * channel = c*16 + sy*4 + sx of source pixel (4Y+sy, 4X+sx), grid row = Y*21 + X; rows 441..447 of out_cm are zero. */
 int b200rl_frames_to_s2d_u8(const uint8_t* obs, const int64_t* rows, int64_t n, uint8_t* out_rm, uint8_t* out_cm, void* stream);
 /* Frame-stack delta upload (csrc/frame_stack.cu).  The Atari observation the reference uploads whole every step
