@@ -1229,24 +1229,9 @@ class SoftQNetworkMLP(nn.Module):
         return q[0].reshape(B, 1)
 
 
-class SACContinuousActor(nn.Module):
-    """sac_continuous_action.py:106-151: fc1, fc2, fc_mean, fc_logstd and the buffers action_scale / action_bias.
-    ``forward(x)`` -> (mean, log_std); ``get_action(x)`` -> (action, log_prob [n, 1], squashed mean), drawing the
-    [n, D] standard normals with ``noise_fn`` (``buf.normal_()`` on the default CUDA generator, what
-    ``Normal.rsample`` consumes)."""
-
-    def __init__(self, env):
-        super().__init__()
-        self.obs_dim, self.act_dim = _sacc_dims(env)
-        self.fc1 = nn.Linear(self.obs_dim, 256)
-        self.fc2 = nn.Linear(256, 256)
-        self.fc_mean = nn.Linear(256, self.act_dim)
-        self.fc_logstd = nn.Linear(256, self.act_dim)
-        high, low = env.single_action_space.high, env.single_action_space.low
-        self.register_buffer("action_scale", torch.tensor((high - low) / 2.0, dtype=torch.float32))
-        self.register_buffer("action_bias", torch.tensor((high + low) / 2.0, dtype=torch.float32))
-        self.noise_fn = _normal_noise
-        self._flat = None
+class _FlatActor(nn.Module):
+    """An actor whose parameters the kernels read from one ``nets.FlatParams`` buffer (``flat``, built on first use on
+    the parameters' CUDA device), with the action noise drawn by ``noise_fn``."""
 
     @property
     def flat(self):
@@ -1271,6 +1256,26 @@ class SACContinuousActor(nn.Module):
 
     def _obs(self, x):
         return x.float().reshape(x.shape[0], -1).contiguous()
+
+
+class SACContinuousActor(_FlatActor):
+    """sac_continuous_action.py:106-151: fc1, fc2, fc_mean, fc_logstd and the buffers action_scale / action_bias.
+    ``forward(x)`` -> (mean, log_std); ``get_action(x)`` -> (action, log_prob [n, 1], squashed mean), drawing the
+    [n, D] standard normals with ``noise_fn`` (``buf.normal_()`` on the default CUDA generator, what
+    ``Normal.rsample`` consumes)."""
+
+    def __init__(self, env):
+        super().__init__()
+        self.obs_dim, self.act_dim = _sacc_dims(env)
+        self.fc1 = nn.Linear(self.obs_dim, 256)
+        self.fc2 = nn.Linear(256, 256)
+        self.fc_mean = nn.Linear(256, self.act_dim)
+        self.fc_logstd = nn.Linear(256, self.act_dim)
+        high, low = env.single_action_space.high, env.single_action_space.low
+        self.register_buffer("action_scale", torch.tensor((high - low) / 2.0, dtype=torch.float32))
+        self.register_buffer("action_bias", torch.tensor((high + low) / 2.0, dtype=torch.float32))
+        self.noise_fn = _normal_noise
+        self._flat = None
 
     @torch.no_grad()
     def forward(self, x):
@@ -1423,6 +1428,14 @@ def sac_continuous_update(state, ring, batch, global_step, args, graph=None):
         return st
     buf["rows"].copy_(batch["rows"])
     key = (B, actor_steps, target_update, views[0].data_ptr(), float(args.gamma), float(args.tau))
+    _replay_update_graph(st, key, lambda: _sacc_update_body(st, *views, buf["rows"], buf, actor_steps, target_update,
+                                                            args.gamma, args.tau))
+    return st
+
+
+def _replay_update_graph(st, key, body):
+    """Replay the update graph ``st`` captured under ``key``, capturing ``body()`` first if there is none (the graphs
+    share one memory pool; the Adam workspace of the largest flat buffer, ``st.q``, is sized before any capture)."""
     g = st._graphs.get(key)
     if g is None:
         ops._workspace(st.device, "adam", ops._lib.load().b200rl_clip_adam_workspace_bytes(st.q.flat.numel()))
@@ -1430,7 +1443,155 @@ def sac_continuous_update(state, ring, batch, global_step, args, graph=None):
         if st._pool is None:
             st._pool = torch.cuda.graph_pool_handle()
         with torch.cuda.graph(g, pool=st._pool):
-            _sacc_update_body(st, *views, buf["rows"], buf, actor_steps, target_update, args.gamma, args.tau)
+            body()
         st._graphs[key] = g
     g.replay()
+
+
+# ---------------------------------------------------------- TD3 (cleanrl/td3_continuous_action.py)
+class TD3Actor(_FlatActor):
+    """td3_continuous_action.py:106-132: fc1, fc2, fc_mu and the buffers action_scale / action_bias, default nn.Linear
+    initialisation.  ``forward(x)`` = tanh(fc_mu(...)) * action_scale + action_bias on the deterministic-head kernel.
+    ``noise_fn`` draws the [B, D] standard normals of the target policy smoothing (``randn_like(actions)`` on the
+    default CUDA generator)."""
+
+    def __init__(self, env):
+        super().__init__()
+        self.obs_dim, self.act_dim = _sacc_dims(env)
+        self.fc1 = nn.Linear(self.obs_dim, 256)
+        self.fc2 = nn.Linear(256, 256)
+        self.fc_mu = nn.Linear(256, self.act_dim)
+        high, low = env.single_action_space.high, env.single_action_space.low
+        self.register_buffer("action_scale", torch.tensor((high - low) / 2.0, dtype=torch.float32))
+        self.register_buffer("action_bias", torch.tensor((high + low) / 2.0, dtype=torch.float32))
+        self.noise_fn = _normal_noise
+        self._flat = None
+
+    @torch.no_grad()
+    def forward(self, x):
+        B = x.shape[0]
+        mu = torch.empty(B, self.act_dim, dtype=torch.float32, device=x.device)
+        ops.td3_actor_fwd(self.flat.flat, self._obs(x), B, self.obs_dim, self.act_dim, self.action_scale,
+                          self.action_bias, mu=mu)
+        return mu
+
+
+def _exploration_noise(std):
+    """td3_continuous_action.py:203: ``torch.normal(0, std)``, one [D] draw that every env adds to its action."""
+    return torch.normal(0, std)
+
+
+class TD3State:
+    """Device-resident part of a TD3 update that is not a network: the flat buffers of the twin critics (one parameter
+    / gradient / Adam buffer, as ``q_optimizer`` covers both), of the twin targets and of the actor target, the Adam
+    step counts of the q and actor optimisers with their device table of step scalars (``dyn``: q, then actor), the
+    logged statistics (``qstats`` = ``ops.SACC_CRITIC_STAT_NAMES``, ``astats[0]`` = the latest actor_loss) and the
+    scratch of each batch size.  With ``use_graph`` every update is replayed as one CUDA graph per (batch size, actor
+    step, gamma, tau, policy_noise, noise_clip, bounds).  ``low`` / ``high``: the scalar bounds the smoothed target
+    action is clamped to (the reference's ``single_action_space.low[0]`` / ``high[0]``; default: the actor's first
+    dimension, action_bias -/+ action_scale)."""
+
+    use_graph = True
+
+    def __init__(self, actor, qf1, qf2, qf1_target, qf2_target, target_actor, device, low=None, high=None):
+        f32 = torch.float32
+        self.device = device
+        b0, s0 = float(actor.action_bias[0]), float(actor.action_scale[0])
+        self.low = float(b0 - s0 if low is None else low)
+        self.high = float(b0 + s0 if high is None else high)
+        self.actor, self.target_actor, self.obs_dim, self.act_dim = actor, target_actor, actor.obs_dim, actor.act_dim
+        self.net_numel = ops.sacc_param_count(self.obs_dim, self.act_dim, True)
+        self.q = nets.FlatParams(list(qf1.parameters()) + list(qf2.parameters()), device)
+        self.qt = nets.FlatParams(list(qf1_target.parameters()) + list(qf2_target.parameters()), device)
+        actor.flat
+        target_actor.flat
+        self.qstats = torch.zeros(4, dtype=f32, device=device)
+        self.astats = torch.zeros(1, dtype=f32, device=device)
+        self.steps = {"q": 0, "actor": 0}
+        self._bufs, self._graphs, self._pool = {}, {}, None
+
+    def buffers(self, B):
+        b = self._bufs.get(B)
+        if b is None:
+            f32, dev, D, K = torch.float32, self.device, self.act_dim, self.obs_dim + self.act_dim
+            z = lambda *s: torch.zeros(*s, dtype=f32, device=dev)   # noqa: E731
+            b = {"rows": torch.zeros(B, dtype=torch.int64, device=dev), "dyn": z(4),
+                 "x": z(B, K), "h1": z(2, B, 256), "h2": z(2, B, 256), "dz1": z(2, B, 256), "dz2": z(2, B, 256),
+                 "q": z(2, B), "qn": z(2, B), "dq": z(2, B), "y": z(B), "eps_next": z(B, D), "a_next": z(B, D),
+                 "xa": z(B, self.obs_dim), "h1a": z(B, 256), "h2a": z(B, 256), "ya": z(B, D), "pi": z(B, D),
+                 "qpi": z(1, B), "dact": z(B, D), "dhead": z(B, D), "dz1a": z(B, 256), "dz2a": z(B, 256),
+                 "ws": ops.sacc_workspace(B, dev)}
+            self._bufs[B] = b
+        return b
+
+    def step_table(self, actor_step, lr):
+        """Advance the optimisers' step counts and return their ``adam_step_scalars``: q, then the actor's (both at
+        ``learning_rate``, td3_continuous_action.py:180-181)."""
+        self.steps["q"] += 1
+        t = list(ops.adam_step_scalars(self.steps["q"], lr))
+        if actor_step:
+            self.steps["actor"] += 1
+            t += ops.adam_step_scalars(self.steps["actor"], lr)
+        else:
+            t += (1.0, 0.0)
+        return t
+
+
+def _td3_update_body(st, obs, next_obs, actions, rewards, dones, rows, buf, actor_step, gamma, tau, smoothing):
+    """td3_continuous_action.py:231-267 on device buffers; the (step, lr) scalars come from ``buf["dyn"]``."""
+    actor, ta, B, od, D, S = st.actor, st.target_actor, rows.numel(), st.obs_dim, st.act_dim, st.net_numel
+    af, q, dyn, ws = actor.flat, st.q, buf["dyn"], buf["ws"]
+    # 1. smoothed target action, the twin targets, the critic loss, its backward and the q optimiser
+    actor.draw_noise_into(buf["eps_next"])
+    ops.td3_actor_fwd(ta.flat.flat, next_obs, B, od, D, ta.action_scale, ta.action_bias, rows=rows,
+                      smoothing=dict(smoothing, eps=buf["eps_next"], out=buf["a_next"]))
+    ops.sacc_critic_fwd(st.qt.flat, S, next_obs, buf["a_next"], B, od, D, obs_rows=rows, q=buf["qn"])
+    ops.sacc_critic_fwd(q.flat, S, obs, actions, B, od, D, obs_rows=rows, act_rows=rows, q=buf["q"], keep_x=buf["x"],
+                        keep_h1=buf["h1"], keep_h2=buf["h2"])
+    ops.sacc_critic_loss(buf["qn"], None, buf["q"], rewards, dones, None, gamma, rows=rows, y=buf["y"], dq=buf["dq"],
+                         stats=st.qstats, workspace=ws)
+    ops.sacc_critic_bwd(q.flat, S, B, od, D, buf["h1"], buf["h2"], dq=buf["dq"], dz1=buf["dz1"], dz2=buf["dz2"])
+    ops.sacc_wgrad(True, B, od, D, buf["x"], buf["h1"], buf["h2"], buf["dz1"], buf["dz2"], buf["dq"], q.grad, S)
+    ops.clip_adam_dyn(q.flat, q.grad, q.exp_avg, q.exp_avg_sq, dyn[0:2], eps=SACC_ADAM_EPS, max_norm=None)
+    if not actor_step:
+        return
+    # 2. the delayed actor step on -qf1(obs, actor(obs)).mean(), then the soft update of all three targets
+    ops.td3_actor_fwd(af.flat, obs, B, od, D, actor.action_scale, actor.action_bias, rows=rows, mu=buf["pi"],
+                      keep_y=buf["ya"], keep_x=buf["xa"], keep_h1=buf["h1a"], keep_h2=buf["h2a"])
+    ops.sacc_critic_fwd(q.flat, 0, obs, buf["pi"], B, od, D, obs_rows=rows, q=buf["qpi"], keep_h1=buf["h1"],
+                        keep_h2=buf["h2"])
+    ops.sacc_critic_bwd(q.flat, 0, B, od, D, buf["h1"], buf["h2"], dact=buf["dact"])
+    ops.td3_actor_bwd(af.flat, B, od, D, buf["ya"], actor.action_scale, buf["dact"], buf["qpi"], buf["h1a"],
+                      buf["h2a"], buf["dhead"], buf["dz1a"], buf["dz2a"], st.astats, ws)
+    ops.sacc_wgrad(ops.SACC_TD3_ACTOR, B, od, D, buf["xa"], buf["h1a"], buf["h2a"], buf["dz1a"], buf["dz2a"],
+                   buf["dhead"], af.grad)
+    ops.clip_adam_dyn(af.flat, af.grad, af.exp_avg, af.exp_avg_sq, dyn[2:4], eps=SACC_ADAM_EPS, max_norm=None)
+    ops.sacc_soft_update(af.flat, ta.flat.flat, af.numel, tau)
+    ops.sacc_soft_update(q.flat, st.qt.flat, 2 * S, tau)
+
+
+@torch.no_grad()
+def td3_update(state, ring, batch, global_step, args, graph=None):
+    """One update of td3_continuous_action.py:230-267 on a ``DeviceReplayRing`` batch: the critic step; on steps where
+    ``global_step % policy_frequency == 0`` the actor step and the soft update of the actor target and both critic
+    targets.  Nothing is read back to the host.  With ``graph`` (default ``state.use_graph``) the
+    update replays one captured CUDA graph per (batch size, actor step, gamma, tau, policy_noise, noise_clip, bounds)
+    with the batch rows copied into a fixed slot and the smoothing draw captured in it."""
+    st = state
+    B = int(batch["rows"].numel())
+    buf = st.buffers(B)
+    actor_step = global_step % args.policy_frequency == 0
+    buf["dyn"].copy_(torch.tensor(st.step_table(actor_step, args.learning_rate), dtype=torch.float32),
+                     non_blocking=True)
+    smoothing = dict(policy_noise=float(args.policy_noise), noise_clip=float(args.noise_clip),
+                     low=st.low, high=st.high)
+    views = (ring.frames, ring.next_frames, ring.action_rows, ring.reward_rows, ring.done_rows)
+    use_graph = st.use_graph if graph is None else graph
+    if not (use_graph and st.actor.graph_friendly):
+        _td3_update_body(st, *views, batch["rows"], buf, actor_step, args.gamma, args.tau, smoothing)
+        return st
+    buf["rows"].copy_(batch["rows"])
+    key = (B, actor_step, views[0].data_ptr(), float(args.gamma), float(args.tau)) + tuple(smoothing.values())
+    _replay_update_graph(st, key, lambda: _td3_update_body(st, *views, buf["rows"], buf, actor_step, args.gamma,
+                                                           args.tau, smoothing))
     return st

@@ -3,6 +3,9 @@
 //   critic  SoftQNetwork  [obs | act] (K = obs_dim + act_dim) -> 256 -> ReLU -> 256 -> ReLU -> 1
 //   actor   Actor         obs -> 256 -> ReLU -> 256 -> ReLU -> fc_mean (D) and fc_logstd (D), tanh-Gaussian head
 //
+// The twin delayed DDPG of cleanrl/td3_continuous_action.py uses the same critics and trunk with a deterministic head:
+//   actor   Actor         obs -> 256 -> ReLU -> 256 -> ReLU -> fc_mu (D), tanh(z) * scale + bias
+//
 // Flat parameter layout: each network's parameters in nn.Module order (fc1.weight [256, in], fc1.bias, fc2.weight, fc2.bias,
 // head weight(s) and bias(es)); the twin critics are two such blocks ``net_stride`` floats apart (q_optimizer's one flat
 // buffer, and the two targets' one flat buffer).
@@ -143,6 +146,37 @@ __device__ __forceinline__ float log_std_of(float raw) {
     return __fadd_rn(-5.f, __fmul_rn(3.5f, __fadd_rn(tanhf(raw), 1.f)));
 }
 
+// The actor's trunk for the CTA's rows: [obs[rows]] gathered into shared memory, h1 = relu(fc1), h2 = relu(fc2), each
+// kept when asked.  ``sm`` holds [kRows][K + 512] floats; returns h2 there.
+__device__ __forceinline__ const float* actor_trunk(const float* p, const MlpOff& o, const float* obs, int64_t ld_obs,
+                                                    const int64_t* rows, int64_t B, int K, float* keep_x, float* keep_h1,
+                                                    float* keep_h2, float* sm, int64_t r0) {
+    float* xs = sm;
+    float* h1 = xs + kRows * K;
+    float* h2 = h1 + kRows * kH;
+    for (int i = threadIdx.x; i < kRows * K; i += kH) {
+        const int r = i / K, k = i - r * K;
+        const int64_t b = r0 + r;
+        float v = 0.f;
+        if (b < B) {
+            v = obs[(rows ? rows[b] : b) * ld_obs + k];
+            if (keep_x) keep_x[b * K + k] = v;
+        }
+        xs[i] = v;
+    }
+    __syncthreads();
+    dense_relu(p + o.w1, p + o.b1, xs, K, h1);
+    __syncthreads();
+    dense_relu(p + o.w2, p + o.b2, h1, kH, h2);
+    __syncthreads();
+    if (keep_h1)
+        for (int r = 0; r < kRows && r0 + r < B; ++r) {
+            keep_h1[(r0 + r) * kH + threadIdx.x] = h1[r * kH + threadIdx.x];
+            keep_h2[(r0 + r) * kH + threadIdx.x] = h2[r * kH + threadIdx.x];
+        }
+    return h2;
+}
+
 struct ActorFwdParams {
     const float* params;
     const float* obs; int64_t ld_obs; const int64_t* rows;
@@ -163,32 +197,10 @@ __global__ void __launch_bounds__(kH) sacc_actor_fwd_kernel(ActorFwdParams P) {
     __shared__ float red[32];
     __shared__ bool is_last;
     const int K = P.obs_dim, D = P.D;
-    float* xs = sm;
-    float* h1 = xs + kRows * K;
-    float* h2 = h1 + kRows * kH;
     const int64_t r0 = (int64_t)blockIdx.x * kRows;
-    for (int i = threadIdx.x; i < kRows * K; i += kH) {
-        const int r = i / K, k = i - r * K;
-        const int64_t b = r0 + r;
-        float v = 0.f;
-        if (b < P.B) {
-            v = P.obs[(P.rows ? P.rows[b] : b) * P.ld_obs + k];
-            if (P.keep_x) P.keep_x[b * K + k] = v;
-        }
-        xs[i] = v;
-    }
-    __syncthreads();
     const MlpOff o(K, D);
     const float* p = P.params;
-    dense_relu(p + o.w1, p + o.b1, xs, K, h1);
-    __syncthreads();
-    dense_relu(p + o.w2, p + o.b2, h1, kH, h2);
-    __syncthreads();
-    if (P.keep_h1)
-        for (int r = 0; r < kRows && r0 + r < P.B; ++r) {
-            P.keep_h1[(r0 + r) * kH + threadIdx.x] = h1[r * kH + threadIdx.x];
-            P.keep_h2[(r0 + r) * kH + threadIdx.x] = h2[r * kH + threadIdx.x];
-        }
+    const float* h2 = actor_trunk(p, o, P.obs, P.ld_obs, P.rows, P.B, K, P.keep_x, P.keep_h1, P.keep_h2, sm, r0);
     // joint [2D, 256] head: outputs 0..D-1 fc_mean, D..2D-1 fc_logstd
     for (int i = threadIdx.x; i < kRows * 2 * D; i += kH) {
         const int r = i / (2 * D), c = i - r * 2 * D;
@@ -254,6 +266,49 @@ __global__ void __launch_bounds__(kH) sacc_actor_fwd_kernel(ActorFwdParams P) {
     }
 }
 
+// ------------------------------------------------------------------------- deterministic actor forward (TD3)
+// torch.clamp: NaN stays NaN.
+__device__ __forceinline__ float clamp_nan(float x, float lo, float hi) { return x < lo ? lo : (x > hi ? hi : x); }
+
+struct Td3ActorFwdParams {
+    const float* params;
+    const float* obs; int64_t ld_obs; const int64_t* rows;
+    int64_t B; int obs_dim, D;
+    const float* scale; const float* bias;
+    float* mu; float* keep_y;                                            // [B, D] each (optional)
+    float* keep_x; float* keep_h1; float* keep_h2;                       // [B, obs], [B, 256] x2 (optional)
+    const float* eps; float policy_noise, noise_clip, lo, hi; float* smoothed;   // target policy smoothing (optional)
+};
+
+__global__ void __launch_bounds__(kH, 1) td3_actor_fwd_kernel(Td3ActorFwdParams P) {
+    extern __shared__ float sm[];
+    const int K = P.obs_dim, D = P.D;
+    const int64_t r0 = (int64_t)blockIdx.x * kRows;
+    const MlpOff o(K, D);
+    const float* p = P.params;
+    const float* h2 = actor_trunk(p, o, P.obs, P.ld_obs, P.rows, P.B, K, P.keep_x, P.keep_h1, P.keep_h2, sm, r0);
+    // fc_mu, then x = tanh(z); x * action_scale + action_bias, each rounded
+    for (int i = threadIdx.x; i < kRows * D; i += kH) {
+        const int r = i / D, c = i - r * D;
+        const int64_t b = r0 + r;
+        if (b >= P.B) continue;
+        const float* w = p + o.w3 + (int64_t)c * kH;
+        float s = 0.f;
+        for (int j = 0; j < kH; ++j) s = fmaf(__ldg(w + j), h2[r * kH + j], s);
+        const float y = tanhf(__fadd_rn(s, __ldg(p + o.b3 + c)));
+        const float sc = P.scale[c];
+        const float mu = __fadd_rn(__fmul_rn(y, sc), P.bias[c]);
+        if (P.keep_y) P.keep_y[b * D + c] = y;
+        if (P.mu) P.mu[b * D + c] = mu;
+        if (P.smoothed) {
+            // clipped_noise = (eps * policy_noise).clamp(-noise_clip, noise_clip) * action_scale;
+            // (mu + clipped_noise).clamp(low[0], high[0])
+            const float n = __fmul_rn(clamp_nan(__fmul_rn(P.eps[b * D + c], P.policy_noise), -P.noise_clip, P.noise_clip), sc);
+            P.smoothed[b * D + c] = clamp_nan(__fadd_rn(mu, n), P.lo, P.hi);
+        }
+    }
+}
+
 // ------------------------------------------------------------------------------------------------ critic loss
 struct CriticLossParams {
     const float* q_next; const float* next_logpi; const float* q;        // [2,B], [B], [2,B]
@@ -269,9 +324,10 @@ __global__ void __launch_bounds__(kLossThreads) sacc_critic_loss_kernel(CriticLo
     float v[4] = {0.f, 0.f, 0.f, 0.f};
     if (i < P.B) {
         const int64_t ri = (P.rows ? P.rows[i] : i) * P.ld_rd;
-        const float alpha = __ldg(P.alpha);
-        // min(qf1_next_target, qf2_next_target) - alpha * next_state_log_pi; r + ((1 - d) * gamma) * that
-        const float m = __fsub_rn(min_nan(P.q_next[i], P.q_next[P.B + i]), __fmul_rn(alpha, P.next_logpi[i]));
+        // min(qf1_next_target, qf2_next_target) - alpha * next_state_log_pi; r + ((1 - d) * gamma) * that.  Without
+        // next_logpi (TD3) the entropy term is absent: the min itself.
+        float m = min_nan(P.q_next[i], P.q_next[P.B + i]);
+        if (P.next_logpi) m = __fsub_rn(m, __fmul_rn(__ldg(P.alpha), P.next_logpi[i]));
         const float y = __fadd_rn(P.rewards[ri], __fmul_rn(__fmul_rn(__fsub_rn(1.f, P.dones[ri]), P.gamma), m));
         const float q1 = P.q[i], q2 = P.q[P.B + i];
         const float d1 = __fsub_rn(q1, y), d2 = __fsub_rn(q2, y);
@@ -291,6 +347,7 @@ __global__ void __launch_bounds__(kLossThreads) sacc_critic_loss_kernel(CriticLo
 // Critic step (dq given): dz2 = relu'(h2) * w3 dq, dz1 = relu'(h1) * W2^T dz2, kept for the weight gradients.
 // Actor step (dq null): dq from actor_loss = mean(alpha log_pi - min(q1, q2)) -- -1/B to the smaller Q, half of it to each
 // at a tie (autograd's binary min) -- and the gradient is carried to the action columns only: dact = W1[:, obs:]^T dz1.
+// Single-network actor step (dq and q null, TD3): actor_loss = -mean(q1), dq = -1/B into the one network.
 struct CriticBwdParams {
     const float* params; int64_t net_stride;
     int64_t B; int obs_dim, D;
@@ -315,6 +372,8 @@ __global__ void __launch_bounds__(kH) sacc_critic_bwd_kernel(CriticBwdParams P) 
             float dq;
             if (P.dq) {
                 dq = P.dq[net * P.B + b];
+            } else if (!P.q) {
+                dq = -P.inv_b;
             } else {
                 const float q1 = P.q[b], q2 = P.q[P.B + b];
                 const float mine = net == 0 ? q1 : q2, other = net == 0 ? q2 : q1;
@@ -404,12 +463,46 @@ __device__ __forceinline__ void tanh_gauss_bwd(float m, float raw, float e, floa
     *draw = __fmul_rn(g_t, __fsub_rn(1.f, __fmul_rn(t, t)));
 }
 
+// From the head gradient dh [kRows][ncols] of the CTA's rows back through the trunk: dz2 = relu'(h2) * W_head^T dh, then
+// dz1 = relu'(h1) * W2^T dz2 (both [B, 256]); head column c < D is row c of w3, c >= D row c - D of w4.
+__device__ __forceinline__ void actor_trunk_bwd(const float* p, const MlpOff& o, int D, int ncols,
+                                                const float (*dh)[2 * kSacMaxD], float (*z2)[kH], const float* h1,
+                                                const float* h2, float* dz1, float* dz2, int64_t B, int64_t r0) {
+    const int j = threadIdx.x;
+    for (int r = 0; r < kRows; ++r) {
+        const int64_t b = r0 + r;
+        float s = 0.f;
+        if (b < B) {
+            for (int c = 0; c < ncols; ++c) {
+                const float w = c < D ? __ldg(p + o.w3 + (int64_t)c * kH + j) : __ldg(p + o.w4 + (int64_t)(c - D) * kH + j);
+                s = fmaf(w, dh[r][c], s);
+            }
+            s = h2[b * kH + j] > 0.f ? s : 0.f;
+            dz2[b * kH + j] = s;
+        }
+        z2[r][j] = s;
+    }
+    __syncthreads();
+    float acc[kRows];
+#pragma unroll
+    for (int r = 0; r < kRows; ++r) acc[r] = 0.f;
+    for (int i = 0; i < kH; ++i) {
+        const float w = __ldg(p + o.w2 + (int64_t)i * kH + j);
+#pragma unroll
+        for (int r = 0; r < kRows; ++r) acc[r] = fmaf(w, z2[r][i], acc[r]);
+    }
+    for (int r = 0; r < kRows; ++r) {
+        const int64_t b = r0 + r;
+        if (b < B) dz1[b * kH + j] = h1[b * kH + j] > 0.f ? acc[r] : 0.f;
+    }
+}
+
 __global__ void __launch_bounds__(kH) sacc_actor_bwd_kernel(ActorBwdParams P) {
     __shared__ float dh[kRows][2 * kSacMaxD];
     __shared__ float z2[kRows][kH];
     __shared__ float red[32];
     __shared__ bool is_last;
-    const int D = P.D, j = threadIdx.x;
+    const int D = P.D;
     const int64_t r0 = (int64_t)blockIdx.x * kRows;
     const float alpha = __ldg(P.alpha);
     const float g = __fmul_rn(P.inv_b, alpha);                  // d actor_loss / d log_pi
@@ -428,34 +521,7 @@ __global__ void __launch_bounds__(kH) sacc_actor_bwd_kernel(ActorBwdParams P) {
         dh[r][D + d] = dr;
     }
     __syncthreads();
-    const MlpOff o(P.obs_dim, D);
-    const float* p = P.params;
-    for (int r = 0; r < kRows; ++r) {
-        const int64_t b = r0 + r;
-        float s = 0.f;
-        if (b < P.B) {
-            for (int c = 0; c < 2 * D; ++c) {
-                const float w = c < D ? __ldg(p + o.w3 + (int64_t)c * kH + j) : __ldg(p + o.w4 + (int64_t)(c - D) * kH + j);
-                s = fmaf(w, dh[r][c], s);
-            }
-            s = P.h2[b * kH + j] > 0.f ? s : 0.f;
-            P.dz2[b * kH + j] = s;
-        }
-        z2[r][j] = s;
-    }
-    __syncthreads();
-    float acc[kRows];
-#pragma unroll
-    for (int r = 0; r < kRows; ++r) acc[r] = 0.f;
-    for (int i = 0; i < kH; ++i) {
-        const float w = __ldg(p + o.w2 + (int64_t)i * kH + j);
-#pragma unroll
-        for (int r = 0; r < kRows; ++r) acc[r] = fmaf(w, z2[r][i], acc[r]);
-    }
-    for (int r = 0; r < kRows; ++r) {
-        const int64_t b = r0 + r;
-        if (b < P.B) P.dz1[b * kH + j] = P.h1[b * kH + j] > 0.f ? acc[r] : 0.f;
-    }
+    actor_trunk_bwd(P.params, MlpOff(P.obs_dim, D), D, 2 * D, dh, z2, P.h1, P.h2, P.dz1, P.dz2, P.B, r0);
     // losses/actor_loss = ((alpha * log_pi) - min_qf_pi).mean()
     float v[1] = {0.f};
     if (threadIdx.x < kRows && r0 + threadIdx.x < P.B) {
@@ -464,6 +530,46 @@ __global__ void __launch_bounds__(kH) sacc_actor_bwd_kernel(ActorBwdParams P) {
     }
     if (!fold<1>(v, P.partials, P.ticket, red, &is_last)) return;
     if (threadIdx.x == 0) P.stats[0] = __fdiv_rn(v[0], (float)P.B);
+}
+
+// ----------------------------------------------------------- deterministic actor loss + data backward (TD3)
+// actor_loss = -mean(qf1(obs, actor(obs))): dact [B, D] is qf1's gradient w.r.t. the action (dq = -1/B).  Through
+// x * action_scale + action_bias and tanh: dz = (dact * scale) * (1 - y^2), autograd's mul backward then tanh_backward;
+// then fc_mu, fc2 and fc1 backward.  The last block writes losses/actor_loss.
+struct Td3ActorBwdParams {
+    const float* params;
+    int64_t B; int obs_dim, D;
+    const float* y; const float* scale; const float* dact; const float* q;    // [B,D], [D], [B,D], [B]
+    const float* h1; const float* h2;
+    float* dhead; float* dz1; float* dz2;                                     // [B,D], [B,256] x2
+    float* stats; float* partials; unsigned int* ticket;
+};
+
+__global__ void __launch_bounds__(kH) td3_actor_bwd_kernel(Td3ActorBwdParams P) {
+    __shared__ float dh[kRows][2 * kSacMaxD];
+    __shared__ float z2[kRows][kH];
+    __shared__ float red[32];
+    __shared__ bool is_last;
+    const int D = P.D;
+    const int64_t r0 = (int64_t)blockIdx.x * kRows;
+    for (int i = threadIdx.x; i < kRows * D; i += kH) {
+        const int r = i / D, d = i - r * D;
+        const int64_t b = r0 + r;
+        float dz = 0.f;
+        if (b < P.B) {
+            const float y = P.y[b * D + d];
+            dz = __fmul_rn(__fmul_rn(P.dact[b * D + d], P.scale[d]), __fsub_rn(1.f, __fmul_rn(y, y)));
+            P.dhead[b * D + d] = dz;
+        }
+        dh[r][d] = dz;
+    }
+    __syncthreads();
+    actor_trunk_bwd(P.params, MlpOff(P.obs_dim, D), D, D, dh, z2, P.h1, P.h2, P.dz1, P.dz2, P.B, r0);
+    // losses/actor_loss = -qf1(...).mean()
+    float v[1] = {0.f};
+    if (threadIdx.x < kRows && r0 + threadIdx.x < P.B) v[0] = P.q[r0 + threadIdx.x];
+    if (!fold<1>(v, P.partials, P.ticket, red, &is_last)) return;
+    if (threadIdx.x == 0) P.stats[0] = -__fdiv_rn(v[0], (float)P.B);
 }
 
 // ------------------------------------------------------------------------------------------- weight gradients
@@ -523,7 +629,7 @@ __global__ void sacc_soft_update_kernel(const float* __restrict__ src, float* __
 }
 
 // The forward kernels stage [kRows][in + 512] floats: up to 49152 B of dynamic shared memory at in = 1024, which with
-// the actor's static arrays exceeds the default 48 KB window.  Opt both kernels in once per device.
+// the actor's static arrays exceeds the default 48 KB window.  Opt the three kernels in once per device.
 static int sacc_opt_in_smem() {
     static bool done[64] = {};
     int dev = 0;
@@ -532,7 +638,8 @@ static int sacc_opt_in_smem() {
     if (done[dev]) return 0;
     const int bytes = kRows * (kSacMaxIn + 2 * kH) * (int)sizeof(float);
     if (cudaFuncSetAttribute(sacc_critic_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) != cudaSuccess ||
-        cudaFuncSetAttribute(sacc_actor_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) != cudaSuccess)
+        cudaFuncSetAttribute(sacc_actor_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) != cudaSuccess ||
+        cudaFuncSetAttribute(td3_actor_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) != cudaSuccess)
         return fail(B200RL_ERR_CUDA, "sac_continuous: cudaFuncSetAttribute(MaxDynamicSharedMemorySize, %d)", bytes);
     done[dev] = true;
     return 0;
@@ -553,11 +660,16 @@ static int sacc_opt_in_smem() {
         for (const void* p_ : ps_) B200RL_REQUIRE(b200rl::aligned(p_, 4), what ": misaligned pointer");               \
     } while (0)
 
+// Network kinds of b200rl_sacc_param_count / b200rl_sacc_wgrad_f32 (include/b200rl.h).
+enum { kSaccActor = 0, kSaccCritic = 1, kTd3Actor = 2 };
+
 extern "C" int64_t b200rl_sacc_param_count(int obs_dim, int act_dim, int critic) {
     if (obs_dim < 1 || act_dim < 1 || act_dim > b200rl::kSacMaxD || obs_dim + act_dim > b200rl::kSacMaxIn) return -1;
-    const int64_t in = critic ? obs_dim + act_dim : obs_dim;
-    const int64_t H = b200rl::kH;
-    return H * in + H + H * H + H + (critic ? H + 1 : 2 * ((int64_t)act_dim * H + act_dim));
+    if (critic < kSaccActor || critic > kTd3Actor) return -1;
+    const int64_t in = critic == kSaccCritic ? obs_dim + act_dim : obs_dim;
+    const int64_t H = b200rl::kH, D = act_dim;
+    const int64_t head = critic == kSaccCritic ? H + 1 : critic == kTd3Actor ? D * H + D : 2 * (D * H + D);
+    return H * in + H + H * H + H + head;
 }
 
 extern "C" size_t b200rl_sacc_workspace_bytes(int64_t B) {
@@ -636,8 +748,8 @@ extern "C" int b200rl_sacc_critic_loss_f32(const float* q_next, const float* nex
                                            void* workspace, size_t workspace_bytes, void* stream) {
     using namespace b200rl;
     B200RL_REQUIRE(B >= 1 && B <= 8192, "sacc_critic_loss: B=%lld outside [1, 8192]", (long long)B);
-    B200RL_REQUIRE(q_next && next_logpi && q && rewards && dones && alpha && dq && stats,
-                   "sacc_critic_loss: null pointer");
+    B200RL_REQUIRE(q_next && q && rewards && dones && dq && stats, "sacc_critic_loss: null pointer");
+    B200RL_REQUIRE(!next_logpi || alpha, "sacc_critic_loss: next_logpi needs alpha");
     B200RL_REQUIRE(ld_rd >= 1, "sacc_critic_loss: bad strides");
     SACC_ALIGNED("sacc_critic_loss", q_next, next_logpi, q, rewards, dones, alpha, y, dq, stats);
     B200RL_REQUIRE(aligned(rows, 8), "sacc_critic_loss: misaligned rows");
@@ -660,15 +772,18 @@ extern "C" int b200rl_sacc_critic_bwd_f32(const float* params, int64_t net_strid
     using namespace b200rl;
     SACC_SHAPES("sacc_critic_bwd", obs_dim + act_dim);
     B200RL_REQUIRE(params && h1 && h2, "sacc_critic_bwd: null pointer");
-    B200RL_REQUIRE(dq ? (dz1 && dz2 && !dact) : (q && dact && !dz1 && !dz2),
-                   "sacc_critic_bwd: give dq with dz1 / dz2 (critic step) or q with dact (actor step)");
+    // single: the one-network actor step (net_stride 0, neither dq nor q)
+    const bool single = !dq && !q && net_stride == 0;
+    B200RL_REQUIRE(dq ? (dz1 && dz2 && !dact) : ((q || single) && dact && !dz1 && !dz2),
+                   "sacc_critic_bwd: give dq with dz1 / dz2 (critic step), q with dact (actor step) or, with "
+                   "net_stride 0, dact alone (single-network actor step)");
     B200RL_REQUIRE(net_stride == 0 || net_stride >= b200rl_sacc_param_count(obs_dim, act_dim, 1),
                    "sacc_critic_bwd: net_stride too small");
     SACC_ALIGNED("sacc_critic_bwd", params, dq, q, h1, h2, dz1, dz2, dact);
     cudaStream_t s = (cudaStream_t)stream;
     ProfScope ps(s, "sacc_critic_bwd", 4.0 * B * kH * (kH + 1 + (dact ? act_dim : 0)), 0);
     CriticBwdParams P{params, net_stride, B, obs_dim, act_dim, dq, q, (float)(1.0 / (double)B), h1, h2, dz1, dz2, dact};
-    sacc_critic_bwd_kernel<<<dim3((unsigned)ceil_div(B, kRows), 2), kH, 0, s>>>(P);
+    sacc_critic_bwd_kernel<<<dim3((unsigned)ceil_div(B, kRows), single ? 1 : 2), kH, 0, s>>>(P);
     return check_launch("sacc_critic_bwd");
 }
 
@@ -699,9 +814,11 @@ extern "C" int b200rl_sacc_wgrad_f32(int critic, int64_t B, int obs_dim, int act
                                      const float* h2, const float* dz1, const float* dz2, const float* dout, float* grad,
                                      int64_t net_stride, void* stream) {
     using namespace b200rl;
-    SACC_SHAPES("sacc_wgrad", critic ? obs_dim + act_dim : obs_dim);
+    B200RL_REQUIRE(critic >= kSaccActor && critic <= kTd3Actor, "sacc_wgrad: network kind %d outside [0, 2]", critic);
+    SACC_SHAPES("sacc_wgrad", critic == kSaccCritic ? obs_dim + act_dim : obs_dim);
     B200RL_REQUIRE(x && h1 && h2 && dz1 && dz2 && dout && grad, "sacc_wgrad: null pointer");
-    B200RL_REQUIRE(!critic || net_stride >= b200rl_sacc_param_count(obs_dim, act_dim, 1), "sacc_wgrad: net_stride too small");
+    B200RL_REQUIRE(critic != kSaccCritic || net_stride >= b200rl_sacc_param_count(obs_dim, act_dim, 1),
+                   "sacc_wgrad: net_stride too small");
     SACC_ALIGNED("sacc_wgrad", x, h1, h2, dz1, dz2, dout, grad);
     WgradParams P{};
     P.B = B;
@@ -711,7 +828,7 @@ extern "C" int b200rl_sacc_wgrad_f32(int critic, int64_t B, int obs_dim, int act
         J = WgradJob{dz, ld_dz, xx, ld_x, N, K, dw, db, (int)ceil_div(K + 1, kWT), t};
         t += (int)ceil_div(N, kWT) * J.tiles_k;
     };
-    if (critic) {
+    if (critic == kSaccCritic) {
         const int K = obs_dim + act_dim;
         const MlpOff o(K, 1);
         for (int n = 0; n < 2; ++n) {
@@ -721,17 +838,68 @@ extern "C" int b200rl_sacc_wgrad_f32(int critic, int64_t B, int obs_dim, int act
             add(dz2 + a, kH, h1 + a, kH, kH, kH, g + o.w2, g + o.b2);
             add(dout + (int64_t)n * B, 1, h2 + a, kH, 1, kH, g + o.w3, g + o.b3);
         }
-    } else {
+    } else if (critic == kSaccActor) {
         const MlpOff o(obs_dim, act_dim);
         add(dz1, kH, x, obs_dim, kH, obs_dim, grad + o.w1, grad + o.b1);
         add(dz2, kH, h1, kH, kH, kH, grad + o.w2, grad + o.b2);
         add(dout, 2 * act_dim, h2, kH, act_dim, kH, grad + o.w3, grad + o.b3);
         add(dout + act_dim, 2 * act_dim, h2, kH, act_dim, kH, grad + o.w4, grad + o.b4);
+    } else {
+        const MlpOff o(obs_dim, act_dim);
+        add(dz1, kH, x, obs_dim, kH, obs_dim, grad + o.w1, grad + o.b1);
+        add(dz2, kH, h1, kH, kH, kH, grad + o.w2, grad + o.b2);
+        add(dout, act_dim, h2, kH, act_dim, kH, grad + o.w3, grad + o.b3);
     }
     cudaStream_t s = (cudaStream_t)stream;
     ProfScope ps(s, "sacc_wgrad", 0, 0);
     sacc_wgrad_kernel<<<(unsigned)t, kH, 0, s>>>(P);
     return check_launch("sacc_wgrad");
+}
+
+extern "C" int b200rl_td3_actor_fwd_f32(const float* params, const float* obs, int64_t ld_obs, const int64_t* rows,
+                                        int64_t B, int obs_dim, int act_dim, const float* scale, const float* bias,
+                                        float* mu, float* keep_y, float* keep_x, float* keep_h1, float* keep_h2,
+                                        const float* eps, double policy_noise, double noise_clip, double low,
+                                        double high, float* smoothed, void* stream) {
+    using namespace b200rl;
+    SACC_SHAPES("td3_actor_fwd", obs_dim);
+    B200RL_REQUIRE(params && obs && scale && bias, "td3_actor_fwd: null pointer");
+    B200RL_REQUIRE((eps == nullptr) == (smoothed == nullptr), "td3_actor_fwd: eps and smoothed go together");
+    B200RL_REQUIRE((keep_h1 == nullptr) == (keep_h2 == nullptr), "td3_actor_fwd: keep_h1 and keep_h2 go together");
+    B200RL_REQUIRE(ld_obs >= obs_dim, "td3_actor_fwd: bad strides");
+    B200RL_REQUIRE(!smoothed || (noise_clip >= 0.0 && low <= high), "td3_actor_fwd: noise_clip < 0 or low > high");
+    SACC_ALIGNED("td3_actor_fwd", params, obs, scale, bias, mu, keep_y, keep_x, keep_h1, keep_h2, eps, smoothed);
+    B200RL_REQUIRE(aligned(rows, 8), "td3_actor_fwd: misaligned rows");
+    cudaStream_t s = (cudaStream_t)stream;
+    ProfScope ps(s, "td3_actor_fwd", 2.0 * B * kH * (obs_dim + kH + act_dim), 0);
+    Td3ActorFwdParams P{params, obs, ld_obs, rows, B, obs_dim, act_dim, scale, bias, mu, keep_y, keep_x, keep_h1,
+                        keep_h2, eps, (float)policy_noise, (float)noise_clip, (float)low, (float)high, smoothed};
+    if (int rc = sacc_opt_in_smem()) return rc;
+    const size_t smem = (size_t)kRows * (obs_dim + 2 * kH) * sizeof(float);
+    td3_actor_fwd_kernel<<<(unsigned)ceil_div(B, kRows), kH, smem, s>>>(P);
+    return check_launch("td3_actor_fwd");
+}
+
+extern "C" int b200rl_td3_actor_bwd_f32(const float* params, int64_t B, int obs_dim, int act_dim, const float* y,
+                                        const float* scale, const float* dact, const float* q, const float* h1,
+                                        const float* h2, float* dhead, float* dz1, float* dz2, float* stats,
+                                        void* workspace, size_t workspace_bytes, void* stream) {
+    using namespace b200rl;
+    SACC_SHAPES("td3_actor_bwd", obs_dim);
+    B200RL_REQUIRE(params && y && scale && dact && q && h1 && h2 && dhead && dz1 && dz2 && stats,
+                   "td3_actor_bwd: null pointer");
+    SACC_ALIGNED("td3_actor_bwd", params, y, scale, dact, q, h1, h2, dhead, dz1, dz2, stats);
+    B200RL_REQUIRE(workspace && aligned(workspace, 16), "td3_actor_bwd: workspace null or misaligned");
+    if (workspace_bytes < b200rl_sacc_workspace_bytes(B))
+        return fail(B200RL_ERR_WORKSPACE, "td3_actor_bwd: workspace %zu < %zu", workspace_bytes,
+                    b200rl_sacc_workspace_bytes(B));
+    cudaStream_t s = (cudaStream_t)stream;
+    ProfScope ps(s, "td3_actor_bwd", 2.0 * B * kH * (kH + act_dim), 0);
+    Td3ActorBwdParams P{params, B, obs_dim, act_dim, y, scale, dact, q, h1, h2, dhead, dz1, dz2, stats,
+                        reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 16),
+                        reinterpret_cast<unsigned int*>(workspace)};
+    td3_actor_bwd_kernel<<<(unsigned)ceil_div(B, kRows), kH, 0, s>>>(P);
+    return check_launch("td3_actor_bwd");
 }
 
 extern "C" int b200rl_sacc_soft_update_f32(const float* src, float* dst, int64_t n, double tau, void* stream) {

@@ -1,5 +1,5 @@
-"""Post-training evaluation with the call surfaces of cleanrl_utils/evals/ppo_eval.py:7-36, dqn_eval.py:9-44 and c51_eval.py
-(SURVEY.md 8f rank 1).
+"""Post-training evaluation with the call surfaces of cleanrl_utils/evals/ppo_eval.py:7-36, dqn_eval.py:9-44, c51_eval.py
+and td3_eval.py (SURVEY.md 8f rank 1).
 
 ``evaluate(model_path, make_env, env_id, eval_episodes, run_name, Model, device, capture_video, gamma)`` rebuilds
 the agent from a ``.cleanrl_model`` file (a plain ``state_dict`` whose keys equal the reference's, so files written
@@ -111,6 +111,40 @@ def evaluate_c51(model_path, make_env, env_id, eval_episodes, run_name, Model, d
             with torch.no_grad():
                 actions, _ = model.get_action(torch.as_tensor(np.asarray(obs)).to(device))
             actions = actions.cpu().numpy()
+        obs, _, _, _, infos = envs.step(actions)
+        for ret in _finished_returns(infos):
+            print(f"eval_episode={len(returns)}, episodic_return={ret}")
+            returns.append(ret)
+    return returns
+
+
+def evaluate_td3(model_path, make_env, env_id, eval_episodes, run_name, Model, device=torch.device("cuda"),
+                 capture_video=True, exploration_noise=0.1, envs=None, max_steps=1000000):
+    """Noisy deterministic rollout of a saved TD3 actor (cleanrl_utils/evals/td3_eval.py): the file holds
+    ``(actor.state_dict(), qf1.state_dict(), qf2.state_dict())``; ``Model = (Actor, QNetwork)``.  Each step adds one
+    ``torch.normal(0, action_scale * exploration_noise)`` draw to the actor's actions (libb200rl kernels) and clips
+    them to the action space on the host; the critics are loaded but not used, as in the reference."""
+    if envs is None:
+        import gymnasium as gym  # type: ignore
+
+        envs = gym.vector.SyncVectorEnv([make_env(env_id, 0, 0, capture_video, run_name)])
+    actor, qf1, qf2 = Model[0](envs).to(device), Model[1](envs).to(device), Model[1](envs).to(device)
+    actor_params, qf1_params, qf2_params = torch.load(model_path, map_location=device)
+    actor.load_state_dict(actor_params)
+    qf1.load_state_dict(qf1_params)
+    qf2.load_state_dict(qf2_params)
+    for m in (actor, qf1, qf2):
+        m.eval()
+
+    returns = []
+    obs, _ = envs.reset()
+    for _ in range(max_steps):
+        if len(returns) >= eval_episodes:
+            break
+        with torch.no_grad():
+            actions = actor(torch.as_tensor(np.asarray(obs, dtype=np.float32)).to(device))
+            actions += torch.normal(0, actor.action_scale * exploration_noise)
+            actions = actions.cpu().numpy().clip(envs.single_action_space.low, envs.single_action_space.high)
         obs, _, _, _, infos = envs.step(actions)
         for ret in _finished_returns(infos):
             print(f"eval_episode={len(returns)}, episodic_return={ret}")

@@ -1191,8 +1191,16 @@ def _ld(t):
     return t.stride(0)
 
 
+SACC_TD3_ACTOR = 2    # network kind of the deterministic TD3 actor (sacc_param_count / sacc_wgrad ``critic``)
+
+
+def _net_kind(critic):
+    """False / True: the tanh-Gaussian actor / a critic; ``SACC_TD3_ACTOR``: the deterministic actor."""
+    return SACC_TD3_ACTOR if critic == SACC_TD3_ACTOR else int(bool(critic))
+
+
 def sacc_param_count(obs_dim, act_dim, critic):
-    n = _lib.load().b200rl_sacc_param_count(int(obs_dim), int(act_dim), int(bool(critic)))
+    n = _lib.load().b200rl_sacc_param_count(int(obs_dim), int(act_dim), _net_kind(critic))
     if n < 0:
         raise ValueError(f"sac_continuous: obs_dim={obs_dim}, act_dim={act_dim} outside the kernels' limits "
                          "(1 <= act_dim <= 32, obs_dim + act_dim <= 1024)")
@@ -1238,7 +1246,8 @@ def sacc_actor_fwd(params, obs, B, obs_dim, act_dim, eps, scale, bias, rows=None
 def sacc_critic_loss(q_next, next_logpi, q, rewards, dones, alpha, gamma, rows=None, y=None, dq=None, stats=None,
                      workspace=None):
     """Soft-Q target and both MSE losses with dq [2, B] (sac_continuous_action.py:257-268).  ``rewards`` / ``dones``
-    are 1-D (strided) views read at ``rows``."""
+    are 1-D (strided) views read at ``rows``.  ``next_logpi`` None: no entropy term (td3_continuous_action.py:241-242);
+    ``alpha`` may then be None."""
     B = q.shape[1]
     dev = q.device
     dq = torch.empty(2, B, dtype=_F32, device=dev) if dq is None else dq
@@ -1247,8 +1256,8 @@ def sacc_critic_loss(q_next, next_logpi, q, rewards, dones, alpha, gamma, rows=N
     if rewards.stride() != dones.stride():
         raise ValueError("sacc_critic_loss: rewards and dones need the same stride")
     rc = _lib.load().b200rl_sacc_critic_loss_f32(
-        _ptr(q_next, _F32, "q_next"), _ptr(next_logpi, _F32, "next_logpi"), _ptr(q, _F32, "q"),
-        _ptr(rewards, _F32, "rewards"), _ptr(dones, _F32, "dones"), rewards.stride(0), _rows(rows), _ptr(alpha, _F32, "alpha"),
+        _ptr(q_next, _F32, "q_next"), _o(next_logpi, "next_logpi"), _ptr(q, _F32, "q"),
+        _ptr(rewards, _F32, "rewards"), _ptr(dones, _F32, "dones"), rewards.stride(0), _rows(rows), _o(alpha, "alpha"),
         int(B), float(gamma), _o(y, "y"), _ptr(dq, _F32, "dq"), _ptr(stats, _F32, "stats"), ws.data_ptr(), ws.numel(),
         _stream())
     _lib.check(rc, "sacc_critic_loss")
@@ -1256,6 +1265,8 @@ def sacc_critic_loss(q_next, next_logpi, q, rewards, dones, alpha, gamma, rows=N
 
 
 def sacc_critic_bwd(params, net_stride, B, obs_dim, act_dim, h1, h2, dq=None, q=None, dz1=None, dz2=None, dact=None):
+    """Critic step (``dq``, ``dz1`` / ``dz2``), twin actor step (``q``, ``dact`` [2, B, D]) or, with ``net_stride`` 0
+    and neither ``dq`` nor ``q``, the single-network actor step of -mean(q) (``dact`` [B, D])."""
     rc = _lib.load().b200rl_sacc_critic_bwd_f32(
         _ptr(params, _F32, "params"), int(net_stride), int(B), int(obs_dim), int(act_dim), _o(dq, "dq"), _o(q, "q"),
         _ptr(h1, _F32, "h1"), _ptr(h2, _F32, "h2"), _o(dz1, "dz1"), _o(dz2, "dz2"), _o(dact, "dact"), _stream())
@@ -1275,7 +1286,7 @@ def sacc_actor_bwd(params, B, obs_dim, act_dim, head, eps, scale, dact, q, log_p
 
 def sacc_wgrad(critic, B, obs_dim, act_dim, x, h1, h2, dz1, dz2, dout, grad, net_stride=0):
     rc = _lib.load().b200rl_sacc_wgrad_f32(
-        int(bool(critic)), int(B), int(obs_dim), int(act_dim), _ptr(x, _F32, "x"), _ptr(h1, _F32, "h1"),
+        _net_kind(critic), int(B), int(obs_dim), int(act_dim), _ptr(x, _F32, "x"), _ptr(h1, _F32, "h1"),
         _ptr(h2, _F32, "h2"), _ptr(dz1, _F32, "dz1"), _ptr(dz2, _F32, "dz2"), _ptr(dout, _F32, "dout"),
         _ptr(grad, _F32, "grad"), int(net_stride), _stream())
     _lib.check(rc, "sacc_wgrad")
@@ -1286,3 +1297,30 @@ def sacc_soft_update(src, dst, n, tau):
     rc = _lib.load().b200rl_sacc_soft_update_f32(_ptr(src, _F32, "src"), _ptr(dst, _F32, "dst"), int(n), float(tau),
                                                  _stream())
     _lib.check(rc, "sacc_soft_update")
+
+
+# ----------------------------------------------------------- TD3 (td3_continuous_action.py), kind SACC_TD3_ACTOR
+def td3_actor_fwd(params, obs, B, obs_dim, act_dim, scale, bias, rows=None, mu=None, keep_y=None, keep_x=None,
+                  keep_h1=None, keep_h2=None, smoothing=None):
+    """Actor.forward (td3_continuous_action.py:128-132) on obs[rows]: ``mu`` [B, D] and the kept tanh ``keep_y``.
+    ``smoothing``: a dict(eps [B, D], policy_noise, noise_clip, low, high, out [B, D]) for the smoothed target action
+    of td3_continuous_action.py:232-238."""
+    sm = smoothing or {}
+    rc = _lib.load().b200rl_td3_actor_fwd_f32(
+        _ptr(params, _F32, "params"), _ptr(obs, _F32, "obs"), _ld(obs), _rows(rows), int(B), int(obs_dim), int(act_dim),
+        _ptr(scale, _F32, "scale"), _ptr(bias, _F32, "bias"), _o(mu, "mu"), _o(keep_y, "keep_y"), _o(keep_x, "keep_x"),
+        _o(keep_h1, "keep_h1"), _o(keep_h2, "keep_h2"), _o(sm.get("eps"), "eps"), float(sm.get("policy_noise", 0.0)),
+        float(sm.get("noise_clip", 0.0)), float(sm.get("low", 0.0)), float(sm.get("high", 0.0)), _o(sm.get("out"), "out"),
+        _stream())
+    _lib.check(rc, "td3_actor_fwd")
+
+
+def td3_actor_bwd(params, B, obs_dim, act_dim, y, scale, dact, q, h1, h2, dhead, dz1, dz2, stats, workspace):
+    """actor_loss = -qf1(obs, actor(obs)).mean() (td3_continuous_action.py:256) back through the deterministic head and
+    the trunk; stats[0] = actor_loss."""
+    rc = _lib.load().b200rl_td3_actor_bwd_f32(
+        _ptr(params, _F32, "params"), int(B), int(obs_dim), int(act_dim), _ptr(y, _F32, "y"), _ptr(scale, _F32, "scale"),
+        _ptr(dact, _F32, "dact"), _ptr(q, _F32, "q"), _ptr(h1, _F32, "h1"), _ptr(h2, _F32, "h2"),
+        _ptr(dhead, _F32, "dhead"), _ptr(dz1, _F32, "dz1"), _ptr(dz2, _F32, "dz2"), _ptr(stats, _F32, "stats"),
+        workspace.data_ptr(), workspace.numel(), _stream())
+    _lib.check(rc, "td3_actor_bwd")

@@ -578,7 +578,9 @@ int b200rl_sac_actor_loss_f32(const float* logits, int64_t ld, const float* q1, 
  * Kernels with a row mean take workspace of b200rl_sacc_workspace_bytes(B) bytes, 16-byte aligned, zeroed once; one
  * buffer may serve all of them on one stream.  Temperature, Adam moments and step scalars live in device memory.
  *
- * b200rl_sacc_param_count: floats in one critic (critic != 0) or the actor; -1 for a shape outside the limits.
+ * Network kinds (``critic``): 0 = the tanh-Gaussian actor, 1 = a critic, 2 = the deterministic TD3 actor (one D-wide
+ *   head fc_mu).
+ * b200rl_sacc_param_count: floats in one network of that kind; -1 for a shape or kind outside the limits.
  * b200rl_sacc_critic_fwd_f32: q [2, B] of both critics on x = [obs[obs_rows] | act[act_rows]] (either rows vector
  *   (int64) may be NULL for rows 0..B-1); keep_x [B, K] and keep_h1 / keep_h2 (post-ReLU) may be NULL.
  * b200rl_sacc_actor_fwd_f32: Actor.get_action on obs[rows] with noise eps [B, D]: action [B, D], log_pi [B], squashed
@@ -589,17 +591,30 @@ int b200rl_sac_actor_loss_f32(const float* logits, int64_t ld, const float* q1, 
  * min is torch.min's: NaN if either operand is NaN.
  * b200rl_sacc_critic_loss_f32: y = r + ((1 - d) gamma) (min(q_next[0], q_next[1]) - alpha next_logpi) with r / d read
  *   through rows (NULL: 0..B-1); dq [2, B] = 2 (q - y) / B; y may be NULL; stats[0..3] = mean q1, mean q2, qf1_loss,
- *   qf2_loss.
+ *   qf2_loss.  next_logpi NULL (TD3): no entropy term, y = r + ((1 - d) gamma) min(q_next[0], q_next[1]); alpha may then
+ *   be NULL.
  * b200rl_sacc_critic_bwd_f32: data gradients through both critics.  Critic step: dq given, writes dz1 / dz2 [2, B, 256]
  *   (pre-activation gradients of fc1 / fc2).  Actor step: dq NULL, q [2, B] given; the gradient of -mean(min(q1, q2))
  *   (half to each at a tie, as autograd's min) is carried to the action columns only: dact [2, B, D], one per critic.
+ *   Single-network actor step (TD3): net_stride 0, dq and q NULL; the gradient of -mean(q) of the one network goes to
+ *   dact [B, D].
  * b200rl_sacc_actor_bwd_f32: actor_loss = mean(alpha log_pi - min(q[0], q[1])) back through the tanh-Gaussian head (raw
  *   head and eps of the forward, dact of the critics) to dhead [B, 2D] = (d mean, d raw log_std), then dz2 / dz1
  *   [B, 256]; stats[0] = actor_loss.
- * b200rl_sacc_wgrad_f32: weight and bias gradients of all three layers of both critics (critic != 0: dz1 / dz2 [2, B,
- *   256], dout = dq [2, B], x [B, K], h1 / h2 [2, B, 256]) or of the actor (dout = dhead [B, 2D]) into grad (flat layout,
- *   overwritten), summed over rows in row order, no atomics.
+ * b200rl_sacc_wgrad_f32: weight and bias gradients of all three layers of both critics (critic 1: dz1 / dz2 [2, B,
+ *   256], dout = dq [2, B], x [B, K], h1 / h2 [2, B, 256]), of the actor (critic 0: dout = dhead [B, 2D]) or of the TD3
+ *   actor (critic 2: dout = dhead [B, D]) into grad (flat layout, overwritten), summed over rows in row order, no
+ *   atomics.
  * b200rl_sacc_soft_update_f32: dst = tau * src + (1 - tau) * dst, two products and one sum each rounded.
+ *
+ * cleanrl/td3_continuous_action.py's deterministic Actor (kind 2) on the same trunk, critics and limits:
+ * b200rl_td3_actor_fwd_f32: Actor.forward on obs[rows]: mu [B, D] = tanh(z) scale + bias (two roundings), keep_y [B, D]
+ *   = tanh(z), the kept x / h1 / h2; each may be NULL.  With eps [B, D] it also writes the smoothed target action
+ *   smoothed [B, D] = (mu + (eps policy_noise).clamp(-noise_clip, noise_clip) scale).clamp(low, high) in that rounding
+ *   order (eps and smoothed go together; low / high are scalars: the reference clamps to low[0] / high[0]).
+ * b200rl_td3_actor_bwd_f32: actor_loss = -mean(q) (q [B] of qf1 on the actor's action, dact [B, D] its gradient from
+ *   the single-network critic backward) back through the head: dhead [B, D] = (dact scale) (1 - y^2), then dz2 / dz1
+ *   [B, 256]; stats[0] = actor_loss.  Workspace as above.
  */
 int64_t b200rl_sacc_param_count(int obs_dim, int act_dim, int critic);
 size_t b200rl_sacc_workspace_bytes(int64_t B);
@@ -628,6 +643,14 @@ int b200rl_sacc_wgrad_f32(int critic, int64_t B, int obs_dim, int act_dim, const
                           const float* h2, const float* dz1, const float* dz2, const float* dout, float* grad,
                           int64_t net_stride, void* stream);
 int b200rl_sacc_soft_update_f32(const float* src, float* dst, int64_t n, double tau, void* stream);
+int b200rl_td3_actor_fwd_f32(const float* params, const float* obs, int64_t ld_obs, const int64_t* rows, int64_t B,
+                             int obs_dim, int act_dim, const float* scale, const float* bias, float* mu, float* keep_y,
+                             float* keep_x, float* keep_h1, float* keep_h2, const float* eps, double policy_noise,
+                             double noise_clip, double low, double high, float* smoothed, void* stream);
+int b200rl_td3_actor_bwd_f32(const float* params, int64_t B, int obs_dim, int act_dim, const float* y,
+                             const float* scale, const float* dact, const float* q, const float* h1, const float* h2,
+                             float* dhead, float* dz1, float* dz2, float* stats, void* workspace,
+                             size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }
