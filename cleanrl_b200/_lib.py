@@ -134,6 +134,8 @@ SIGNATURES = {
     "b200rl_td3_actor_fwd_f32": (_i, [_p, _p, _i64, _p, _i64, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _d, _d, _d, _d, _p,
                                       _p]),
     "b200rl_td3_actor_bwd_f32": (_i, [_p, _i64, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p]),
+    "b200rl_ddpg_critic_loss_bwd_f32": (_i, [_p, _i64, _i, _i, _p, _p, _p, _p, _i64, _p, _d, _p, _p, _p, _p, _p, _p,
+                                             _p, _p, _sz, _p]),
 }
 
 

@@ -1595,3 +1595,112 @@ def td3_update(state, ring, batch, global_step, args, graph=None):
     _replay_update_graph(st, key, lambda: _td3_update_body(st, *views, buf["rows"], buf, actor_step, args.gamma,
                                                            args.tau, smoothing))
     return st
+
+
+# ---------------------------------------------------------- DDPG (cleanrl/ddpg_continuous_action.py)
+class DDPGActor(TD3Actor):
+    """ddpg_continuous_action.py:96-116: TD3's modules, initialisation and state_dict keys, with action_scale /
+    action_bias taken from ``env.action_space`` -- the vector env's batched space, so [1, D] under gymnasium's
+    ``SyncVectorEnv`` and [D] where ``action_space`` is unbatched.  The kernels read D contiguous floats either way."""
+
+    def __init__(self, env):
+        super().__init__(env)
+        high, low = env.action_space.high, env.action_space.low
+        self.action_scale = torch.tensor((high - low) / 2.0, dtype=torch.float32)
+        self.action_bias = torch.tensor((high + low) / 2.0, dtype=torch.float32)
+
+
+class DDPGState:
+    """Device-resident part of a DDPG update that is not a network: the flat buffers of qf1 and of qf1_target (one
+    network each), the actor target's (on the module), the Adam step counts of the q and actor optimisers with their
+    device table of step scalars (``dyn``: q, then actor), the logged statistics (``qstats`` =
+    ``ops.DDPG_CRITIC_STAT_NAMES``, ``astats[0]`` = the latest actor_loss) and the scratch of each batch size.  The
+    update draws no random numbers; with ``use_graph`` it is replayed as one CUDA graph per (batch size, actor step,
+    ring, gamma, tau)."""
+
+    use_graph = True
+
+    def __init__(self, actor, qf1, qf1_target, target_actor, device):
+        f32 = torch.float32
+        self.device = device
+        self.actor, self.target_actor, self.obs_dim, self.act_dim = actor, target_actor, actor.obs_dim, actor.act_dim
+        self.net_numel = ops.sacc_param_count(self.obs_dim, self.act_dim, True)
+        self.q = nets.FlatParams(list(qf1.parameters()), device)
+        self.qt = nets.FlatParams(list(qf1_target.parameters()), device)
+        actor.flat
+        target_actor.flat
+        self.qstats = torch.zeros(2, dtype=f32, device=device)
+        self.astats = torch.zeros(1, dtype=f32, device=device)
+        self.steps = {"q": 0, "actor": 0}
+        self._bufs, self._graphs, self._pool = {}, {}, None
+
+    def buffers(self, B):
+        b = self._bufs.get(B)
+        if b is None:
+            f32, dev, D, K = torch.float32, self.device, self.act_dim, self.obs_dim + self.act_dim
+            z = lambda *s: torch.zeros(*s, dtype=f32, device=dev)   # noqa: E731
+            b = {"rows": torch.zeros(B, dtype=torch.int64, device=dev), "dyn": z(4),
+                 "x": z(B, K), "h1": z(1, B, 256), "h2": z(1, B, 256), "dz1": z(1, B, 256), "dz2": z(1, B, 256),
+                 "q": z(1, B), "qn": z(1, B), "dq": z(B), "y": z(B), "a_next": z(B, D),
+                 "xa": z(B, self.obs_dim), "h1a": z(B, 256), "h2a": z(B, 256), "ya": z(B, D), "pi": z(B, D),
+                 "qpi": z(1, B), "dact": z(B, D), "dhead": z(B, D), "dz1a": z(B, 256), "dz2a": z(B, 256),
+                 "ws": ops.sacc_workspace(B, dev)}
+            self._bufs[B] = b
+        return b
+
+    step_table = TD3State.step_table      # both optimisers at learning_rate (ddpg_continuous_action.py:158-159)
+
+
+def _ddpg_update_body(st, obs, next_obs, actions, rewards, dones, rows, buf, actor_step, gamma, tau):
+    """ddpg_continuous_action.py:214-245 on device buffers; the (step, lr) scalars come from ``buf["dyn"]``."""
+    actor, ta, B, od, D, S = st.actor, st.target_actor, rows.numel(), st.obs_dim, st.act_dim, st.net_numel
+    af, q, dyn, ws = actor.flat, st.q, buf["dyn"], buf["ws"]
+    # 1. target action (no smoothing), qf1_target, qf1, the fused loss + data backward, the weight gradient, q_optimizer
+    ops.td3_actor_fwd(ta.flat.flat, next_obs, B, od, D, ta.action_scale, ta.action_bias, rows=rows, mu=buf["a_next"])
+    ops.sacc_critic_fwd(st.qt.flat, 0, next_obs, buf["a_next"], B, od, D, obs_rows=rows, q=buf["qn"])
+    ops.sacc_critic_fwd(q.flat, 0, obs, actions, B, od, D, obs_rows=rows, act_rows=rows, q=buf["q"], keep_x=buf["x"],
+                        keep_h1=buf["h1"], keep_h2=buf["h2"])
+    ops.ddpg_critic_loss_bwd(q.flat, B, od, D, buf["qn"], buf["q"], rewards, dones, gamma, buf["h1"], buf["h2"],
+                             rows=rows, y=buf["y"], dq=buf["dq"], dz1=buf["dz1"], dz2=buf["dz2"], stats=st.qstats,
+                             workspace=ws)
+    ops.sacc_wgrad(True, B, od, D, buf["x"], buf["h1"], buf["h2"], buf["dz1"], buf["dz2"], buf["dq"], q.grad, 0)
+    ops.clip_adam_dyn(q.flat, q.grad, q.exp_avg, q.exp_avg_sq, dyn[0:2], eps=SACC_ADAM_EPS, max_norm=None)
+    if not actor_step:
+        return
+    # 2. the actor step on -qf1(obs, actor(obs)).mean() with the critic just updated (TD3's), then both soft updates
+    ops.td3_actor_fwd(af.flat, obs, B, od, D, actor.action_scale, actor.action_bias, rows=rows, mu=buf["pi"],
+                      keep_y=buf["ya"], keep_x=buf["xa"], keep_h1=buf["h1a"], keep_h2=buf["h2a"])
+    ops.sacc_critic_fwd(q.flat, 0, obs, buf["pi"], B, od, D, obs_rows=rows, q=buf["qpi"], keep_h1=buf["h1"],
+                        keep_h2=buf["h2"])
+    ops.sacc_critic_bwd(q.flat, 0, B, od, D, buf["h1"], buf["h2"], dact=buf["dact"])
+    ops.td3_actor_bwd(af.flat, B, od, D, buf["ya"], actor.action_scale, buf["dact"], buf["qpi"], buf["h1a"],
+                      buf["h2a"], buf["dhead"], buf["dz1a"], buf["dz2a"], st.astats, ws)
+    ops.sacc_wgrad(ops.SACC_TD3_ACTOR, B, od, D, buf["xa"], buf["h1a"], buf["h2a"], buf["dz1a"], buf["dz2a"],
+                   buf["dhead"], af.grad)
+    ops.clip_adam_dyn(af.flat, af.grad, af.exp_avg, af.exp_avg_sq, dyn[2:4], eps=SACC_ADAM_EPS, max_norm=None)
+    ops.sacc_soft_update(af.flat, ta.flat.flat, af.numel, tau)
+    ops.sacc_soft_update(q.flat, st.qt.flat, S, tau)
+
+
+@torch.no_grad()
+def ddpg_update(state, ring, batch, global_step, args, graph=None):
+    """One update of ddpg_continuous_action.py:214-245 on a ``DeviceReplayRing`` batch: the critic step; on steps where
+    ``global_step % policy_frequency == 0`` the actor step and the soft update of the actor target and qf1_target.
+    Nothing is read back to the host and nothing is drawn.  With ``graph`` (default ``state.use_graph``) the update
+    replays one captured CUDA graph per (batch size, actor step, ring, gamma, tau) with the batch rows copied into a
+    fixed slot."""
+    st = state
+    B = int(batch["rows"].numel())
+    buf = st.buffers(B)
+    actor_step = global_step % args.policy_frequency == 0
+    buf["dyn"].copy_(torch.tensor(st.step_table(actor_step, args.learning_rate), dtype=torch.float32),
+                     non_blocking=True)
+    views = (ring.frames, ring.next_frames, ring.action_rows, ring.reward_rows, ring.done_rows)
+    if not (st.use_graph if graph is None else graph):
+        _ddpg_update_body(st, *views, batch["rows"], buf, actor_step, args.gamma, args.tau)
+        return st
+    buf["rows"].copy_(batch["rows"])
+    key = (B, actor_step, views[0].data_ptr(), float(args.gamma), float(args.tau))
+    _replay_update_graph(st, key, lambda: _ddpg_update_body(st, *views, buf["rows"], buf, actor_step, args.gamma,
+                                                            args.tau))
+    return st

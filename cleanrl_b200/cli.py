@@ -315,6 +315,30 @@ def td3_continuous_action_args(exp_name="td3_continuous_action"):
     return _make("Args", common + algo + extra)
 
 
+def ddpg_continuous_action_args(exp_name="ddpg_continuous_action"):
+    """cleanrl/ddpg_continuous_action.py:19-64 (one env: no num_envs; env_id keeps the reference's help text)."""
+    common = list(_override(_COMMON, exp_name=exp_name))
+    common += [
+        ("save_model", bool, False, "whether to save model into the `runs/{run_name}` folder"),
+        ("upload_model", bool, False, "whether to upload the saved model to huggingface"),
+        ("hf_entity", str, "", "the user or org name of the model repository from the Hugging Face Hub"),
+    ]
+    algo = [
+        ("env_id", str, "Hopper-v4", "the environment id of the Atari game"),
+        ("total_timesteps", int, 1000000, "total timesteps of the experiments"),
+        ("learning_rate", float, 3e-4, "the learning rate of the optimizer"),
+        ("buffer_size", int, int(1e6), "the replay memory buffer size"),
+        ("gamma", float, 0.99, "the discount factor gamma"),
+        ("tau", float, 0.005, "target smoothing coefficient (default: 0.005)"),
+        ("batch_size", int, 256, "the batch size of sample from the reply memory"),
+        ("exploration_noise", float, 0.1, "the scale of exploration noise"),
+        ("learning_starts", int, 25e3, "timestep to start learning"),
+        ("policy_frequency", int, 2, "the frequency of training policy (delayed)"),
+    ]
+    extra = [r for r in _EXTRA if r[0] == "synthetic_env"]
+    return _make("Args", common + algo + extra)
+
+
 def parse(cls, argv=None):
     return tyro.cli(cls, args=argv)
 

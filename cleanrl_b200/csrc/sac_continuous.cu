@@ -5,6 +5,7 @@
 //
 // The twin delayed DDPG of cleanrl/td3_continuous_action.py uses the same critics and trunk with a deterministic head:
 //   actor   Actor         obs -> 256 -> ReLU -> 256 -> ReLU -> fc_mu (D), tanh(z) * scale + bias
+// and cleanrl/ddpg_continuous_action.py the same actor with one critic (net_stride 0) instead of two.
 //
 // Flat parameter layout: each network's parameters in nn.Module order (fc1.weight [256, in], fc1.bias, fc2.weight, fc2.bias,
 // head weight(s) and bias(es)); the twin critics are two such blocks ``net_stride`` floats apart (q_optimizer's one flat
@@ -356,33 +357,19 @@ struct CriticBwdParams {
     float* dz1; float* dz2; float* dact;                  // [2,B,256] x2, [2,B,D]
 };
 
-__global__ void __launch_bounds__(kH) sacc_critic_bwd_kernel(CriticBwdParams P) {
-    __shared__ float z2[kRows][kH];
-    __shared__ float z1[kRows][kH];
-    const int net = blockIdx.y, j = threadIdx.x;
-    const int K = P.obs_dim + P.D;
-    const int64_t r0 = (int64_t)blockIdx.x * kRows;
-    const float* p = P.params + net * P.net_stride;
-    const MlpOff o(K, 1);
+// From dq of the CTA's rows (dq[r], row r0 + r) back through one critic's trunk: dz2 = relu'(h2) * w3 dq, then
+// dz1 = relu'(h1) * W2^T dz2, into z2 / z1 in shared memory and, when dz1 is given, into dz1 / dz2 [B, 256].  h1, h2,
+// dz1 and dz2 point at the network's own [B, 256] block.  The twin critic backward and the one-critic DDPG step share it.
+__device__ __forceinline__ void critic_trunk_bwd(const float* p, const MlpOff& o, const float (&dq)[kRows],
+                                                 const float* h1, const float* h2, float* dz1, float* dz2,
+                                                 float (*z2)[kH], float (*z1)[kH], int64_t B, int64_t r0) {
+    const int j = threadIdx.x;
     const float w3 = __ldg(p + o.w3 + j);
+#pragma unroll
     for (int r = 0; r < kRows; ++r) {
         const int64_t b = r0 + r;
         float g = 0.f;
-        if (b < P.B) {
-            float dq;
-            if (P.dq) {
-                dq = P.dq[net * P.B + b];
-            } else if (!P.q) {
-                dq = -P.inv_b;
-            } else {
-                const float q1 = P.q[b], q2 = P.q[P.B + b];
-                const float mine = net == 0 ? q1 : q2, other = net == 0 ? q2 : q1;
-                const float gm = -P.inv_b;
-                dq = mine == other ? __fmul_rn(gm, 0.5f) : (mine > other ? 0.f : gm);   // minimum's backward
-            }
-            const float h = P.h2[((int64_t)net * P.B + b) * kH + j];
-            g = h > 0.f ? __fmul_rn(dq, w3) : 0.f;
-        }
+        if (b < B) g = h2[b * kH + j] > 0.f ? __fmul_rn(dq[r], w3) : 0.f;
         z2[r][j] = g;
     }
     __syncthreads();
@@ -394,16 +381,48 @@ __global__ void __launch_bounds__(kH) sacc_critic_bwd_kernel(CriticBwdParams P) 
 #pragma unroll
         for (int r = 0; r < kRows; ++r) acc[r] = fmaf(w, z2[r][i], acc[r]);
     }
+#pragma unroll
     for (int r = 0; r < kRows; ++r) {
         const int64_t b = r0 + r;
         float g = 0.f;
-        if (b < P.B) {
-            const int64_t at = ((int64_t)net * P.B + b) * kH + j;
-            g = P.h1[at] > 0.f ? acc[r] : 0.f;
-            if (P.dz1) { P.dz1[at] = g; P.dz2[at] = z2[r][j]; }
+        if (b < B) {
+            g = h1[b * kH + j] > 0.f ? acc[r] : 0.f;
+            if (dz1) { dz1[b * kH + j] = g; dz2[b * kH + j] = z2[r][j]; }
         }
         z1[r][j] = g;
     }
+}
+
+__global__ void __launch_bounds__(kH) sacc_critic_bwd_kernel(CriticBwdParams P) {
+    __shared__ float z2[kRows][kH];
+    __shared__ float z1[kRows][kH];
+    const int net = blockIdx.y;
+    const int K = P.obs_dim + P.D;
+    const int64_t r0 = (int64_t)blockIdx.x * kRows;
+    const float* p = P.params + net * P.net_stride;
+    const MlpOff o(K, 1);
+    float dq[kRows];
+#pragma unroll
+    for (int r = 0; r < kRows; ++r) {
+        const int64_t b = r0 + r;
+        float d = 0.f;
+        if (b < P.B) {
+            if (P.dq) {
+                d = P.dq[net * P.B + b];
+            } else if (!P.q) {
+                d = -P.inv_b;
+            } else {
+                const float q1 = P.q[b], q2 = P.q[P.B + b];
+                const float mine = net == 0 ? q1 : q2, other = net == 0 ? q2 : q1;
+                const float gm = -P.inv_b;
+                d = mine == other ? __fmul_rn(gm, 0.5f) : (mine > other ? 0.f : gm);   // minimum's backward
+            }
+        }
+        dq[r] = d;
+    }
+    const int64_t at = (int64_t)net * P.B * kH;
+    critic_trunk_bwd(p, o, dq, P.h1 + at, P.h2 + at, P.dz1 ? P.dz1 + at : nullptr, P.dz1 ? P.dz2 + at : nullptr, z2,
+                     z1, P.B, r0);
     if (!P.dact) return;
     __syncthreads();
     for (int i = threadIdx.x; i < kRows * P.D; i += kH) {
@@ -414,6 +433,58 @@ __global__ void __launch_bounds__(kH) sacc_critic_bwd_kernel(CriticBwdParams P) 
         float s = 0.f;
         for (int k = 0; k < kH; ++k) s = fmaf(__ldg(w + (int64_t)k * K), z1[r][k], s);
         P.dact[((int64_t)net * P.B + b) * P.D + c] = s;
+    }
+}
+
+// ------------------------------------------------------------ one-critic loss + critic data backward (DDPG)
+// y = r + ((1 - d) gamma) q_next and dq = (2 / B)(q - y) for the CTA's rows (threads 0..kRows-1, in the twin loss's
+// rounding order), then the critic trunk backward of critic_trunk_bwd on the one network.  The last block writes
+// stats[0..1] = mean q (losses/qf1_values) and qf1_loss.
+struct DdpgLossBwdParams {
+    const float* params;
+    int64_t B; int obs_dim, D;
+    const float* q_next; const float* q;                                   // [B] each
+    const float* rewards; const float* dones; int64_t ld_rd; const int64_t* rows;
+    float gamma, two_over_b;
+    const float* h1; const float* h2;                                      // [B, 256] each
+    float* y; float* dq; float* dz1; float* dz2;                           // [B], [B], [B, 256] x2
+    float* stats; float* partials; unsigned int* ticket;
+};
+
+__global__ void __launch_bounds__(kH) ddpg_critic_loss_bwd_kernel(DdpgLossBwdParams P) {
+    __shared__ float z2[kRows][kH];
+    __shared__ float z1[kRows][kH];
+    __shared__ float dqs[kRows];
+    __shared__ float red[32];
+    __shared__ bool is_last;
+    const int64_t r0 = (int64_t)blockIdx.x * kRows;
+    float v[2] = {0.f, 0.f};
+    if (threadIdx.x < kRows) {
+        const int64_t b = r0 + threadIdx.x;
+        float d = 0.f;
+        if (b < P.B) {
+            const int64_t ri = (P.rows ? P.rows[b] : b) * P.ld_rd;
+            const float y = __fadd_rn(P.rewards[ri], __fmul_rn(__fmul_rn(__fsub_rn(1.f, P.dones[ri]), P.gamma), P.q_next[b]));
+            const float q = P.q[b];
+            const float e = __fsub_rn(q, y);
+            v[0] = q;
+            v[1] = __fmul_rn(e, e);
+            if (P.y) P.y[b] = y;
+            d = __fmul_rn(P.two_over_b, e);                             // F.mse_loss backward: (2 / B) (input - target)
+            P.dq[b] = d;
+        }
+        dqs[threadIdx.x] = d;
+    }
+    __syncthreads();
+    float dq[kRows];
+#pragma unroll
+    for (int r = 0; r < kRows; ++r) dq[r] = dqs[r];
+    critic_trunk_bwd(P.params, MlpOff(P.obs_dim + P.D, 1), dq, P.h1, P.h2, P.dz1, P.dz2, z2, z1, P.B, r0);
+    if (!fold<2>(v, P.partials, P.ticket, red, &is_last)) return;
+    if (threadIdx.x == 0) {
+        const float b = (float)P.B;
+        P.stats[0] = __fdiv_rn(v[0], b);                                // losses/qf1_values
+        P.stats[1] = __fdiv_rn(v[1], b);                                // losses/qf1_loss
     }
 }
 
@@ -787,6 +858,33 @@ extern "C" int b200rl_sacc_critic_bwd_f32(const float* params, int64_t net_strid
     return check_launch("sacc_critic_bwd");
 }
 
+extern "C" int b200rl_ddpg_critic_loss_bwd_f32(const float* params, int64_t B, int obs_dim, int act_dim,
+                                               const float* q_next, const float* q, const float* rewards,
+                                               const float* dones, int64_t ld_rd, const int64_t* rows, double gamma,
+                                               const float* h1, const float* h2, float* y, float* dq, float* dz1,
+                                               float* dz2, float* stats, void* workspace, size_t workspace_bytes,
+                                               void* stream) {
+    using namespace b200rl;
+    SACC_SHAPES("ddpg_critic_loss_bwd", obs_dim + act_dim);
+    B200RL_REQUIRE(params && q_next && q && rewards && dones && h1 && h2 && dq && dz1 && dz2 && stats,
+                   "ddpg_critic_loss_bwd: null pointer");
+    B200RL_REQUIRE(ld_rd >= 1, "ddpg_critic_loss_bwd: bad strides");
+    SACC_ALIGNED("ddpg_critic_loss_bwd", params, q_next, q, rewards, dones, h1, h2, y, dq, dz1, dz2, stats);
+    B200RL_REQUIRE(aligned(rows, 8), "ddpg_critic_loss_bwd: misaligned rows");
+    B200RL_REQUIRE(workspace && aligned(workspace, 16), "ddpg_critic_loss_bwd: workspace null or misaligned");
+    if (workspace_bytes < b200rl_sacc_workspace_bytes(B))
+        return fail(B200RL_ERR_WORKSPACE, "ddpg_critic_loss_bwd: workspace %zu < %zu", workspace_bytes,
+                    b200rl_sacc_workspace_bytes(B));
+    cudaStream_t s = (cudaStream_t)stream;
+    ProfScope ps(s, "ddpg_critic_loss_bwd", 20.0 * B + 2.0 * B * kH * (kH + 1), 0);
+    DdpgLossBwdParams P{params, B, obs_dim, act_dim, q_next, q, rewards, dones, ld_rd, rows, (float)gamma,
+                        (float)(2.0 / (double)B), h1, h2, y, dq, dz1, dz2, stats,
+                        reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 16),
+                        reinterpret_cast<unsigned int*>(workspace)};
+    ddpg_critic_loss_bwd_kernel<<<(unsigned)ceil_div(B, kRows), kH, 0, s>>>(P);
+    return check_launch("ddpg_critic_loss_bwd");
+}
+
 extern "C" int b200rl_sacc_actor_bwd_f32(const float* params, int64_t B, int obs_dim, int act_dim, const float* head,
                                          const float* eps, const float* scale, const float* dact, const float* q,
                                          const float* log_pi, const float* alpha, const float* h1, const float* h2,
@@ -817,8 +915,8 @@ extern "C" int b200rl_sacc_wgrad_f32(int critic, int64_t B, int obs_dim, int act
     B200RL_REQUIRE(critic >= kSaccActor && critic <= kTd3Actor, "sacc_wgrad: network kind %d outside [0, 2]", critic);
     SACC_SHAPES("sacc_wgrad", critic == kSaccCritic ? obs_dim + act_dim : obs_dim);
     B200RL_REQUIRE(x && h1 && h2 && dz1 && dz2 && dout && grad, "sacc_wgrad: null pointer");
-    B200RL_REQUIRE(critic != kSaccCritic || net_stride >= b200rl_sacc_param_count(obs_dim, act_dim, 1),
-                   "sacc_wgrad: net_stride too small");
+    B200RL_REQUIRE(critic != kSaccCritic || net_stride == 0 ||
+                   net_stride >= b200rl_sacc_param_count(obs_dim, act_dim, 1), "sacc_wgrad: net_stride too small");
     SACC_ALIGNED("sacc_wgrad", x, h1, h2, dz1, dz2, dout, grad);
     WgradParams P{};
     P.B = B;
@@ -831,7 +929,7 @@ extern "C" int b200rl_sacc_wgrad_f32(int critic, int64_t B, int obs_dim, int act
     if (critic == kSaccCritic) {
         const int K = obs_dim + act_dim;
         const MlpOff o(K, 1);
-        for (int n = 0; n < 2; ++n) {
+        for (int n = 0; n < (net_stride ? 2 : 1); ++n) {              // net_stride 0: one critic (DDPG)
             float* g = grad + n * net_stride;
             const int64_t a = (int64_t)n * B * kH;
             add(dz1 + a, kH, x, K, kH, K, g + o.w1, g + o.b1);

@@ -1,5 +1,5 @@
-"""Post-training evaluation with the call surfaces of cleanrl_utils/evals/ppo_eval.py:7-36, dqn_eval.py:9-44, c51_eval.py
-and td3_eval.py (SURVEY.md 8f rank 1).
+"""Post-training evaluation with the call surfaces of cleanrl_utils/evals/ppo_eval.py:7-36, dqn_eval.py:9-44, c51_eval.py,
+td3_eval.py and ddpg_eval.py (SURVEY.md 8f rank 1).
 
 ``evaluate(model_path, make_env, env_id, eval_episodes, run_name, Model, device, capture_video, gamma)`` rebuilds
 the agent from a ``.cleanrl_model`` file (a plain ``state_dict`` whose keys equal the reference's, so files written
@@ -118,24 +118,10 @@ def evaluate_c51(model_path, make_env, env_id, eval_episodes, run_name, Model, d
     return returns
 
 
-def evaluate_td3(model_path, make_env, env_id, eval_episodes, run_name, Model, device=torch.device("cuda"),
-                 capture_video=True, exploration_noise=0.1, envs=None, max_steps=1000000):
-    """Noisy deterministic rollout of a saved TD3 actor (cleanrl_utils/evals/td3_eval.py): the file holds
-    ``(actor.state_dict(), qf1.state_dict(), qf2.state_dict())``; ``Model = (Actor, QNetwork)``.  Each step adds one
+def _noisy_actor_returns(actor, envs, eval_episodes, exploration_noise, device, max_steps):
+    """The rollout of cleanrl_utils/evals/td3_eval.py and ddpg_eval.py: reset without a seed, then each step adds one
     ``torch.normal(0, action_scale * exploration_noise)`` draw to the actor's actions (libb200rl kernels) and clips
-    them to the action space on the host; the critics are loaded but not used, as in the reference."""
-    if envs is None:
-        import gymnasium as gym  # type: ignore
-
-        envs = gym.vector.SyncVectorEnv([make_env(env_id, 0, 0, capture_video, run_name)])
-    actor, qf1, qf2 = Model[0](envs).to(device), Model[1](envs).to(device), Model[1](envs).to(device)
-    actor_params, qf1_params, qf2_params = torch.load(model_path, map_location=device)
-    actor.load_state_dict(actor_params)
-    qf1.load_state_dict(qf1_params)
-    qf2.load_state_dict(qf2_params)
-    for m in (actor, qf1, qf2):
-        m.eval()
-
+    them to the single action space on the host, until ``eval_episodes`` returns are in."""
     returns = []
     obs, _ = envs.reset()
     for _ in range(max_steps):
@@ -150,3 +136,39 @@ def evaluate_td3(model_path, make_env, env_id, eval_episodes, run_name, Model, d
             print(f"eval_episode={len(returns)}, episodic_return={ret}")
             returns.append(ret)
     return returns
+
+
+def _load_actor_and_critics(model_path, envs, Model, n_critics, device):
+    """Rebuild ``Model[0]`` (the actor) and ``n_critics`` ``Model[1]`` critics from a file holding their state_dicts in
+    that order; the critics are loaded but not used, as in the reference."""
+    nets_ = [Model[0](envs).to(device)] + [Model[1](envs).to(device) for _ in range(n_critics)]
+    for m, sd in zip(nets_, torch.load(model_path, map_location=device)):
+        m.load_state_dict(sd)
+        m.eval()
+    return nets_[0]
+
+
+def _gymnasium_env(make_env, env_id, capture_video, run_name):
+    import gymnasium as gym  # type: ignore
+
+    return gym.vector.SyncVectorEnv([make_env(env_id, 0, 0, capture_video, run_name)])
+
+
+def evaluate_td3(model_path, make_env, env_id, eval_episodes, run_name, Model, device=torch.device("cuda"),
+                 capture_video=True, exploration_noise=0.1, envs=None, max_steps=1000000):
+    """Noisy deterministic rollout of a saved TD3 actor (cleanrl_utils/evals/td3_eval.py): the file holds
+    ``(actor.state_dict(), qf1.state_dict(), qf2.state_dict())``; ``Model = (Actor, QNetwork)``.  Each step adds one
+    ``torch.normal(0, action_scale * exploration_noise)`` draw to the actor's actions (libb200rl kernels) and clips
+    them to the action space on the host; the critics are loaded but not used, as in the reference."""
+    envs = envs if envs is not None else _gymnasium_env(make_env, env_id, capture_video, run_name)
+    actor = _load_actor_and_critics(model_path, envs, Model, 2, device)
+    return _noisy_actor_returns(actor, envs, eval_episodes, exploration_noise, device, max_steps)
+
+
+def evaluate_ddpg(model_path, make_env, env_id, eval_episodes, run_name, Model, device=torch.device("cuda"),
+                  capture_video=True, exploration_noise=0.1, envs=None, max_steps=1000000):
+    """Noisy deterministic rollout of a saved DDPG actor (cleanrl_utils/evals/ddpg_eval.py): the file holds
+    ``(actor.state_dict(), qf1.state_dict())``; ``Model = (Actor, QNetwork)``; the rollout is ``evaluate_td3``'s."""
+    envs = envs if envs is not None else _gymnasium_env(make_env, env_id, capture_video, run_name)
+    actor = _load_actor_and_critics(model_path, envs, Model, 1, device)
+    return _noisy_actor_returns(actor, envs, eval_episodes, exploration_noise, device, max_steps)

@@ -1285,6 +1285,9 @@ def sacc_actor_bwd(params, B, obs_dim, act_dim, head, eps, scale, dact, q, log_p
 
 
 def sacc_wgrad(critic, B, obs_dim, act_dim, x, h1, h2, dz1, dz2, dout, grad, net_stride=0):
+    """Weight and bias gradients into the flat ``grad``: of the twin critics (``critic`` True, ``net_stride`` apart:
+    dz1 / dz2 / h1 / h2 [2, B, 256], ``dout`` = dq [2, B]) or, with ``net_stride`` 0, of one critic (DDPG: [1, B, 256],
+    dq [B]); of the tanh-Gaussian actor (False) or of the deterministic actor (``SACC_TD3_ACTOR``)."""
     rc = _lib.load().b200rl_sacc_wgrad_f32(
         _net_kind(critic), int(B), int(obs_dim), int(act_dim), _ptr(x, _F32, "x"), _ptr(h1, _F32, "h1"),
         _ptr(h2, _F32, "h2"), _ptr(dz1, _F32, "dz1"), _ptr(dz2, _F32, "dz2"), _ptr(dout, _F32, "dout"),
@@ -1324,3 +1327,31 @@ def td3_actor_bwd(params, B, obs_dim, act_dim, y, scale, dact, q, h1, h2, dhead,
         _ptr(dhead, _F32, "dhead"), _ptr(dz1, _F32, "dz1"), _ptr(dz2, _F32, "dz2"), _ptr(stats, _F32, "stats"),
         workspace.data_ptr(), workspace.numel(), _stream())
     _lib.check(rc, "td3_actor_bwd")
+
+
+# ------------------------------------------------------------------ DDPG (ddpg_continuous_action.py), one critic
+DDPG_CRITIC_STAT_NAMES = ("qf1_values", "qf1_loss")
+
+
+def ddpg_critic_loss_bwd(params, B, obs_dim, act_dim, q_next, q, rewards, dones, gamma, h1, h2, rows=None, y=None,
+                         dq=None, dz1=None, dz2=None, stats=None, workspace=None):
+    """The one-critic step of ddpg_continuous_action.py:222-229 in one launch: y = r + (1 - d) gamma q_next, dq [B] of
+    F.mse_loss(q, y) and the critic's data gradients dz1 / dz2 [B, 256] from its kept h1 / h2; ``stats`` [2] =
+    ``DDPG_CRITIC_STAT_NAMES``.  ``q_next`` / ``q`` are [B] (or [1, B]); ``rewards`` / ``dones`` 1-D (strided) views
+    read at ``rows``.  Returns (stats, dq, dz1, dz2)."""
+    dev = q.device
+    z = lambda *s: torch.empty(*s, dtype=_F32, device=dev)   # noqa: E731
+    dq = z(B) if dq is None else dq
+    dz1 = z(B, 256) if dz1 is None else dz1
+    dz2 = z(B, 256) if dz2 is None else dz2
+    stats = torch.zeros(2, dtype=_F32, device=dev) if stats is None else stats
+    ws = sacc_workspace(B, dev) if workspace is None else workspace
+    if rewards.stride() != dones.stride():
+        raise ValueError("ddpg_critic_loss_bwd: rewards and dones need the same stride")
+    rc = _lib.load().b200rl_ddpg_critic_loss_bwd_f32(
+        _ptr(params, _F32, "params"), int(B), int(obs_dim), int(act_dim), _ptr(q_next, _F32, "q_next"),
+        _ptr(q, _F32, "q"), _ptr(rewards, _F32, "rewards"), _ptr(dones, _F32, "dones"), rewards.stride(0), _rows(rows),
+        float(gamma), _ptr(h1, _F32, "h1"), _ptr(h2, _F32, "h2"), _o(y, "y"), _ptr(dq, _F32, "dq"),
+        _ptr(dz1, _F32, "dz1"), _ptr(dz2, _F32, "dz2"), _ptr(stats, _F32, "stats"), ws.data_ptr(), ws.numel(), _stream())
+    _lib.check(rc, "ddpg_critic_loss_bwd")
+    return stats, dq, dz1, dz2

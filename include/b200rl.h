@@ -604,7 +604,7 @@ int b200rl_sac_actor_loss_f32(const float* logits, int64_t ld, const float* q1, 
  * b200rl_sacc_wgrad_f32: weight and bias gradients of all three layers of both critics (critic 1: dz1 / dz2 [2, B,
  *   256], dout = dq [2, B], x [B, K], h1 / h2 [2, B, 256]), of the actor (critic 0: dout = dhead [B, 2D]) or of the TD3
  *   actor (critic 2: dout = dhead [B, D]) into grad (flat layout, overwritten), summed over rows in row order, no
- *   atomics.
+ *   atomics.  Critic 1 with net_stride 0: one critic (DDPG), dz1 / dz2 / h1 / h2 [1, B, 256], dout = dq [B].
  * b200rl_sacc_soft_update_f32: dst = tau * src + (1 - tau) * dst, two products and one sum each rounded.
  *
  * cleanrl/td3_continuous_action.py's deterministic Actor (kind 2) on the same trunk, critics and limits:
@@ -615,6 +615,12 @@ int b200rl_sac_actor_loss_f32(const float* logits, int64_t ld, const float* q1, 
  * b200rl_td3_actor_bwd_f32: actor_loss = -mean(q) (q [B] of qf1 on the actor's action, dact [B, D] its gradient from
  *   the single-network critic backward) back through the head: dhead [B, D] = (dact scale) (1 - y^2), then dz2 / dz1
  *   [B, 256]; stats[0] = actor_loss.  Workspace as above.
+ *
+ * cleanrl/ddpg_continuous_action.py: the TD3 actor and one critic (net_stride 0 everywhere), plus
+ * b200rl_ddpg_critic_loss_bwd_f32: the one-critic step in one launch.  y = r + ((1 - d) gamma) q_next (r / d read
+ *   through rows, NULL: 0..B-1; q_next [B] of the target critic), dq [B] = 2 (q - y) / B, then, as the critic step of
+ *   b200rl_sacc_critic_bwd_f32, dz1 / dz2 [B, 256] from the critic's kept h1 / h2 [B, 256]; y may be NULL;
+ *   stats[0..1] = mean q (qf1_values), qf1_loss.  Workspace as above.
  */
 int64_t b200rl_sacc_param_count(int obs_dim, int act_dim, int critic);
 size_t b200rl_sacc_workspace_bytes(int64_t B);
@@ -651,6 +657,11 @@ int b200rl_td3_actor_bwd_f32(const float* params, int64_t B, int obs_dim, int ac
                              const float* scale, const float* dact, const float* q, const float* h1, const float* h2,
                              float* dhead, float* dz1, float* dz2, float* stats, void* workspace,
                              size_t workspace_bytes, void* stream);
+int b200rl_ddpg_critic_loss_bwd_f32(const float* params, int64_t B, int obs_dim, int act_dim, const float* q_next,
+                                    const float* q, const float* rewards, const float* dones, int64_t ld_rd,
+                                    const int64_t* rows, double gamma, const float* h1, const float* h2, float* y,
+                                    float* dq, float* dz1, float* dz2, float* stats, void* workspace,
+                                    size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }
