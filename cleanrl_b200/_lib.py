@@ -37,6 +37,8 @@ SIGNATURES = {
     "b200rl_ppo_loss_gaussian_workspace_bytes": (_sz, [_i64]),
     "b200rl_ppo_loss_gaussian_f32": (_i, [_p, _i64, _p, _p, _i64, _p, _p, _p, _p, _p, _p, _i64, _i, _d, _d, _d, _i, _i,
                                           _p, _i64, _p, _p, _i64, _p, _p, _sz, _p]),
+    "b200rl_ppo_loss_gaussian_shift_f32": (_i, [_p, _i64, _p, _p, _i64, _p, _p, _p, _p, _p, _p, _p, _i64, _i64, _i, _d,
+                                                _d, _d, _i, _i, _p, _i64, _p, _p, _i64, _p, _p, _sz, _p]),
     "b200rl_clip_adam_workspace_bytes": (_sz, [_i64]),
     "b200rl_clip_adam_f32": (_i, [_p, _p, _p, _p, _i64, _i64, _d, _d, _d, _d, _d, _i, _p, _p, _sz, _p]),
     "b200rl_adam_step_scalars": (_i, [_i64, _d, _d, _d, _p]),

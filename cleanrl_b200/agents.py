@@ -826,7 +826,7 @@ class ContinuousMLPAgent(KernelAgent):
         eps = noise if noise is not None else self.noise_fn(n, D, mean.device)
         ops.gaussian_sample(mean, self._logstd(), eps, value, out=(actions_out, logprobs_out, None, values_out))
 
-    def loss_backward(self, policy_out, value, mb_inds, b, a, stats_row, scratch):
+    def loss_backward(self, policy_out, value, mb_inds, b, a, stats_row, scratch, mean_shift=None):
         M, D = policy_out.shape
         dev = policy_out.device
         if scratch.get("M") != M:
@@ -836,7 +836,7 @@ class ContinuousMLPAgent(KernelAgent):
         ops.ppo_loss_gaussian(policy_out, self._logstd(), value, mb_inds, b["actions"], b["logprobs"], b["advantages"],
                               b["returns"], b["values"], a.clip_coef, a.ent_coef, a.vf_coef, a.norm_adv, a.clip_vloss,
                               dmean=scratch["dmean"], dlogstd=self.actor_logstd.grad.view(-1), dvalue=scratch["dv"][:, 0],
-                              stats=stats_row)
+                              stats=stats_row, mean_shift=mean_shift)
         self.a_chain.bwd(scratch["dmean"])
         self.c_chain.bwd(scratch["dv"])
 
@@ -850,6 +850,51 @@ class ContinuousMLPAgent(KernelAgent):
         else:
             logprob, entropy = ops.gaussian_eval(mean, self._logstd(), action)
             v = value.clone() if not value.is_contiguous() else value
+        return action, logprob, entropy, v.reshape(-1, 1)
+
+
+class RPOAgent(ContinuousMLPAgent):
+    """Robust policy optimization (reference: cleanrl/rpo_continuous_action.py:108-144): the continuous PPO agent (same
+    modules, initialisation and state_dict keys) whose update evaluates the stored actions under
+    ``Normal(mean + z, std)``, with z ~ U(-rpo_alpha, rpo_alpha) per row and action dimension from the CPU generator.
+
+    The reference draws one [M, D] z per minibatch and copies it to the device.  ``begin_update_epoch`` draws the
+    epoch's whole [B, D] instead, into the epoch's pinned slot, and uploads it with one asynchronous copy; minibatch
+    ``mb_start`` reads rows [mb_start, mb_start + M).  CPU ``uniform_`` fills a tensor in order, so one [B, D] draw is
+    the concatenation of the reference's per-minibatch draws, and the reference tests ``target_kl`` only after a whole
+    epoch, so no draw is made that the reference would not make."""
+
+    def __init__(self, envs, rpo_alpha):
+        super().__init__(envs)
+        self.rpo_alpha = rpo_alpha
+        self._z_h = None       # pinned [update_epochs, B, D]: one slot per epoch, never rewritten while its copy is queued
+        self._z = None         # device [B, D]: the current epoch's draws
+
+    def begin_update_epoch(self, epoch, num_epochs, batch_size):
+        """Draw and upload the mean shifts of update epoch ``epoch`` (PPOEngine calls it before the epoch's minibatches)."""
+        D = self.action_dim
+        if self._z_h is None or tuple(self._z_h.shape) != (num_epochs, batch_size, D):
+            z_h = torch.empty(num_epochs, batch_size, D, dtype=torch.float32)
+            self._z_h = z_h.pin_memory() if torch.cuda.is_available() else z_h
+            self._z = torch.empty(batch_size, D, dtype=torch.float32, device=self.actor_logstd.device)
+        self._z_h[epoch].uniform_(-self.rpo_alpha, self.rpo_alpha)
+        self._z.copy_(self._z_h[epoch], non_blocking=True)
+
+    def loss_backward(self, policy_out, value, mb_inds, b, a, stats_row, scratch, mb_start=0):
+        if self._z is None:
+            raise RuntimeError("RPOAgent.loss_backward: no mean shifts drawn; call begin_update_epoch first")
+        M = policy_out.shape[0]
+        super().loss_backward(policy_out, value, mb_inds, b, a, stats_row, scratch,
+                              mean_shift=self._z[mb_start:mb_start + M])
+
+    def get_action_and_value(self, x, action=None):
+        if action is None:
+            return super().get_action_and_value(x)
+        self.flat
+        mean, value = self._forward_heads(x)
+        z = torch.empty(mean.shape, dtype=torch.float32).uniform_(-self.rpo_alpha, self.rpo_alpha).to(mean.device)
+        logprob, entropy = ops.gaussian_eval(mean + z, self._logstd(), action)
+        v = value.clone() if not value.is_contiguous() else value
         return action, logprob, entropy, v.reshape(-1, 1)
 
 

@@ -183,6 +183,15 @@ def ppo_continuous_action_args(exp_name="ppo_continuous_action"):
     return _make("Args", common + algo + _RUNTIME + _EXTRA)
 
 
+def rpo_continuous_action_args(exp_name="rpo_continuous_action"):
+    """cleanrl/rpo_continuous_action.py:17-80: ppo_continuous_action.py's fields without save_model / upload_model /
+    hf_entity, total_timesteps 8e6, and rpo_alpha after target_kl."""
+    algo = _override(_ALGO, env_id="HalfCheetah-v4", total_timesteps=8000000, learning_rate=3e-4, num_envs=1,
+                     num_steps=2048, num_minibatches=32, update_epochs=10, ent_coef=0.0)
+    algo += [("rpo_alpha", float, 0.5, "the alpha parameter for RPO")]
+    return _make("Args", _override(_COMMON, exp_name=exp_name) + algo + _RUNTIME + _EXTRA)
+
+
 def dqn_atari_args(exp_name="dqn_atari"):
     """cleanrl/dqn_atari.py:27-80."""
     common = list(_override(_COMMON, exp_name=exp_name))

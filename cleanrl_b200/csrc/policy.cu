@@ -259,14 +259,24 @@ __global__ void __launch_bounds__(kLossThreads) ppo_loss_kernel(LossParams P) {
 constexpr int kMaxD = 32;
 constexpr float kLogSqrt2Pi = 0.9189385332046727f;   // math.log(math.sqrt(2*math.pi)) of torch/distributions/normal.py
 
+// The mean of row component d: ``mean[d]``, or with a shift (rpo_continuous_action.py:140-141, ``action_mean + z``)
+// ``mean[d] + shift[d]`` rounded once, as the reference's separate fp32 add.
+template <bool kShift>
+__device__ __forceinline__ float row_mean(const float* __restrict__ mean, const float* __restrict__ shift, int d) {
+    if constexpr (kShift) return __fadd_rn(mean[d], shift[d]);
+    else return mean[d];
+}
+
+template <bool kShift = false>
 __device__ __forceinline__ void gaussian_row(const float* __restrict__ mean, const float* __restrict__ logstd,
-                                             const float* __restrict__ a, int D, float& logprob, float& entropy) {
+                                             const float* __restrict__ a, int D, float& logprob, float& entropy,
+                                             const float* __restrict__ shift = nullptr) {
     float lp = 0.f, ent = 0.f;
     for (int d = 0; d < D; ++d) {
         const float std = expf(logstd[d]);
         const float var = std * std;
         const float ls = logf(std);
-        const float diff = a[d] - mean[d];
+        const float diff = a[d] - row_mean<kShift>(mean, shift, d);
         lp += -(diff * diff) / (2.f * var) - ls - kLogSqrt2Pi;
         ent += 0.5f + kLogSqrt2Pi + ls;
     }
@@ -309,6 +319,7 @@ struct GLossParams {
     const int64_t* inds;
     const float* b_actions;      // [B, D]
     const float* b_logprobs; const float* b_adv; const float* b_ret; const float* b_val;
+    const float* shift; int64_t lds;   // [M, D] mean shift in minibatch row order (ppo_loss_gaussian_kernel<true> only)
     int64_t M; int D;
     float clip, ent_coef, vf_coef;
     int norm_adv, clip_vloss;
@@ -321,6 +332,9 @@ struct GLossParams {
     unsigned int* ticket;
 };
 
+// kShift: every use of the mean is the shifted mean mu = mean + shift (row_mean).  The gradient w.r.t. the network's
+// mean output equals the gradient w.r.t. mu, so dmean keeps its meaning.  kShift = false is the unshifted kernel.
+template <bool kShift>
 __global__ void __launch_bounds__(kLossThreads) ppo_loss_gaussian_kernel(GLossParams P) {
     __shared__ float red[32];
     __shared__ bool is_last;
@@ -331,13 +345,15 @@ __global__ void __launch_bounds__(kLossThreads) ppo_loss_gaussian_kernel(GLossPa
     for (int k = 0; k < 6; ++k) acc[k] = 0.f;
     float g_lp = 0.f;
     const float* m = nullptr;
+    const float* z = nullptr;
     const float* a = nullptr;
     if (i < P.M) {
         const int64_t j = P.inds ? P.inds[i] : i;
         m = P.mean + i * P.ld;
+        if constexpr (kShift) z = P.shift + i * P.lds;
         a = P.b_actions + j * D;
         float newlogprob, ent;
-        gaussian_row(m, P.logstd, a, D, newlogprob, ent);
+        gaussian_row<kShift>(m, P.logstd, a, D, newlogprob, ent, z);
         const float logratio = newlogprob - P.b_logprobs[j];
         const float ratio = expf(logratio);
         float adv = P.b_adv[j];
@@ -378,7 +394,7 @@ __global__ void __launch_bounds__(kLossThreads) ppo_loss_gaussian_kernel(GLossPa
         float* dm = P.dmean + i * P.ldd;
         for (int d = 0; d < D; ++d) {
             const float std = expf(P.logstd[d]);
-            dm[d] = g_lp * (a[d] - m[d]) / (std * std);
+            dm[d] = g_lp * (a[d] - row_mean<kShift>(m, z, d)) / (std * std);
         }
         P.dvalue[i * P.lddv] = P.vf_coef * 0.5f * invM * gv;
     }
@@ -392,7 +408,7 @@ __global__ void __launch_bounds__(kLossThreads) ppo_loss_gaussian_kernel(GLossPa
         float t = 0.f;
         if (i < P.M) {
             const float std = expf(P.logstd[d]);
-            const float diff = a[d] - m[d];
+            const float diff = a[d] - row_mean<kShift>(m, z, d);
             t = g_lp * (diff * diff / (std * std) - 1.f);
         }
         const float s = block_sum(t, red);
@@ -550,6 +566,51 @@ extern "C" size_t b200rl_ppo_loss_gaussian_workspace_bytes(int64_t M) {
     return 32 + (size_t)ceil_div(M > 0 ? M : 1, kLossThreads) * (kNumStats + kMaxD) * sizeof(float);
 }
 
+namespace b200rl {
+// The shared body of b200rl_ppo_loss_gaussian_f32 / _shift_f32 (``name`` prefixes the messages and names the ProfScope).
+static int ppo_loss_gaussian_launch(const char* name, const float* new_mean, int64_t ld_mean, const float* logstd,
+                                    const float* new_value, int64_t ld_value, const int64_t* mb_inds,
+                                    const float* b_actions, const float* b_logprobs,
+                                    const float* b_advantages, const float* b_returns, const float* b_values,
+                                    const float* mean_shift, int64_t ld_shift,
+                                    int64_t M, int D, double clip_coef, double ent_coef, double vf_coef,
+                                    int norm_adv, int clip_vloss,
+                                    float* dmean, int64_t ld_dmean, float* dlogstd, float* dvalue, int64_t ld_dvalue,
+                                    float* stats, void* workspace, size_t workspace_bytes, void* stream) {
+    B200RL_REQUIRE(M >= 1, "%s: M must be >= 1", name);
+    B200RL_REQUIRE(!norm_adv || M >= 2, "%s: norm_adv needs M >= 2", name);
+    B200RL_REQUIRE(D >= 1 && D <= kMaxD, "%s: D=%d outside [1,%d]", name, D, kMaxD);
+    B200RL_REQUIRE(new_mean && logstd && new_value && b_actions && b_logprobs && b_advantages && b_returns && b_values,
+                   "%s: null input pointer", name);
+    B200RL_REQUIRE(dmean && dlogstd && dvalue && stats, "%s: null output pointer", name);
+    B200RL_REQUIRE(ld_mean >= D && ld_dmean >= D && ld_value >= 1 && ld_dvalue >= 1, "%s: bad strides", name);
+    B200RL_REQUIRE(workspace && aligned(workspace, 16), "%s: workspace null or misaligned", name);
+    if (workspace_bytes < b200rl_ppo_loss_gaussian_workspace_bytes(M))
+        return fail(B200RL_ERR_WORKSPACE, "%s: workspace %zu < %zu bytes", name, workspace_bytes,
+                    b200rl_ppo_loss_gaussian_workspace_bytes(M));
+    cudaStream_t s = (cudaStream_t)stream;
+    float* adv_stats = reinterpret_cast<float*>(workspace);
+    unsigned int* ticket = reinterpret_cast<unsigned int*>(reinterpret_cast<char*>(workspace) + 16);
+    float* partials = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 32);
+    ProfScope ps(s, name, 0, (double)M * (48.0 + 12.0 * D + (mean_shift ? 4.0 * D : 0.0)));
+    cudaError_t e = cudaMemsetAsync(ticket, 0, sizeof(unsigned int), s);
+    if (e != cudaSuccess) return fail(B200RL_ERR_CUDA, "%s: memset: %s", name, cudaGetErrorString(e));
+    if (norm_adv) { note_launches(1); adv_stats_kernel<<<1, 1024, 0, s>>>(b_advantages, mb_inds, M, adv_stats); }
+    GLossParams P;
+    P.mean = new_mean; P.ld = ld_mean; P.logstd = logstd; P.value = new_value; P.ldv = ld_value; P.inds = mb_inds;
+    P.b_actions = b_actions; P.b_logprobs = b_logprobs; P.b_adv = b_advantages; P.b_ret = b_returns; P.b_val = b_values;
+    P.shift = mean_shift; P.lds = ld_shift;
+    P.M = M; P.D = D; P.clip = (float)clip_coef; P.ent_coef = (float)ent_coef; P.vf_coef = (float)vf_coef;
+    P.norm_adv = norm_adv; P.clip_vloss = clip_vloss;
+    P.dmean = dmean; P.ldd = ld_dmean; P.dlogstd = dlogstd; P.dvalue = dvalue; P.lddv = ld_dvalue;
+    P.stats = stats; P.adv_stats = adv_stats; P.partials = partials; P.ticket = ticket;
+    const unsigned blocks = (unsigned)ceil_div(M, kLossThreads);
+    if (mean_shift) ppo_loss_gaussian_kernel<true><<<blocks, kLossThreads, 0, s>>>(P);
+    else ppo_loss_gaussian_kernel<false><<<blocks, kLossThreads, 0, s>>>(P);
+    return check_launch(name);
+}
+}  // namespace b200rl
+
 extern "C" int b200rl_ppo_loss_gaussian_f32(const float* new_mean, int64_t ld_mean, const float* logstd,
                                             const float* new_value, int64_t ld_value, const int64_t* mb_inds,
                                             const float* b_actions, const float* b_logprobs,
@@ -558,33 +619,27 @@ extern "C" int b200rl_ppo_loss_gaussian_f32(const float* new_mean, int64_t ld_me
                                             int norm_adv, int clip_vloss,
                                             float* dmean, int64_t ld_dmean, float* dlogstd, float* dvalue, int64_t ld_dvalue,
                                             float* stats, void* workspace, size_t workspace_bytes, void* stream) {
-    using namespace b200rl;
-    B200RL_REQUIRE(M >= 1, "ppo_loss_gaussian: M must be >= 1");
-    B200RL_REQUIRE(!norm_adv || M >= 2, "ppo_loss_gaussian: norm_adv needs M >= 2");
-    B200RL_REQUIRE(D >= 1 && D <= kMaxD, "ppo_loss_gaussian: D=%d outside [1,%d]", D, kMaxD);
-    B200RL_REQUIRE(new_mean && logstd && new_value && b_actions && b_logprobs && b_advantages && b_returns && b_values,
-                   "ppo_loss_gaussian: null input pointer");
-    B200RL_REQUIRE(dmean && dlogstd && dvalue && stats, "ppo_loss_gaussian: null output pointer");
-    B200RL_REQUIRE(ld_mean >= D && ld_dmean >= D && ld_value >= 1 && ld_dvalue >= 1, "ppo_loss_gaussian: bad strides");
-    B200RL_REQUIRE(workspace && aligned(workspace, 16), "ppo_loss_gaussian: workspace null or misaligned");
-    if (workspace_bytes < b200rl_ppo_loss_gaussian_workspace_bytes(M))
-        return fail(B200RL_ERR_WORKSPACE, "ppo_loss_gaussian: workspace %zu < %zu bytes", workspace_bytes,
-                    b200rl_ppo_loss_gaussian_workspace_bytes(M));
-    cudaStream_t s = (cudaStream_t)stream;
-    float* adv_stats = reinterpret_cast<float*>(workspace);
-    unsigned int* ticket = reinterpret_cast<unsigned int*>(reinterpret_cast<char*>(workspace) + 16);
-    float* partials = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 32);
-    ProfScope ps(s, "ppo_loss_gaussian", 0, (double)M * (48.0 + 12.0 * D));
-    cudaError_t e = cudaMemsetAsync(ticket, 0, sizeof(unsigned int), s);
-    if (e != cudaSuccess) return fail(B200RL_ERR_CUDA, "ppo_loss_gaussian: memset: %s", cudaGetErrorString(e));
-    if (norm_adv) { note_launches(1); adv_stats_kernel<<<1, 1024, 0, s>>>(b_advantages, mb_inds, M, adv_stats); }
-    GLossParams P;
-    P.mean = new_mean; P.ld = ld_mean; P.logstd = logstd; P.value = new_value; P.ldv = ld_value; P.inds = mb_inds;
-    P.b_actions = b_actions; P.b_logprobs = b_logprobs; P.b_adv = b_advantages; P.b_ret = b_returns; P.b_val = b_values;
-    P.M = M; P.D = D; P.clip = (float)clip_coef; P.ent_coef = (float)ent_coef; P.vf_coef = (float)vf_coef;
-    P.norm_adv = norm_adv; P.clip_vloss = clip_vloss;
-    P.dmean = dmean; P.ldd = ld_dmean; P.dlogstd = dlogstd; P.dvalue = dvalue; P.lddv = ld_dvalue;
-    P.stats = stats; P.adv_stats = adv_stats; P.partials = partials; P.ticket = ticket;
-    ppo_loss_gaussian_kernel<<<(unsigned)ceil_div(M, kLossThreads), kLossThreads, 0, s>>>(P);
-    return check_launch("ppo_loss_gaussian");
+    return b200rl::ppo_loss_gaussian_launch("ppo_loss_gaussian", new_mean, ld_mean, logstd, new_value, ld_value, mb_inds,
+                                            b_actions, b_logprobs, b_advantages, b_returns, b_values, nullptr, 0, M, D,
+                                            clip_coef, ent_coef, vf_coef, norm_adv, clip_vloss, dmean, ld_dmean, dlogstd,
+                                            dvalue, ld_dvalue, stats, workspace, workspace_bytes, stream);
+}
+
+extern "C" int b200rl_ppo_loss_gaussian_shift_f32(const float* new_mean, int64_t ld_mean, const float* logstd,
+                                                  const float* new_value, int64_t ld_value, const int64_t* mb_inds,
+                                                  const float* b_actions, const float* b_logprobs,
+                                                  const float* b_advantages, const float* b_returns,
+                                                  const float* b_values, const float* mean_shift, int64_t ld_shift,
+                                                  int64_t M, int D, double clip_coef, double ent_coef, double vf_coef,
+                                                  int norm_adv, int clip_vloss,
+                                                  float* dmean, int64_t ld_dmean, float* dlogstd, float* dvalue,
+                                                  int64_t ld_dvalue, float* stats, void* workspace,
+                                                  size_t workspace_bytes, void* stream) {
+    B200RL_REQUIRE(mean_shift, "ppo_loss_gaussian_shift: null mean_shift");
+    B200RL_REQUIRE(ld_shift >= D, "ppo_loss_gaussian_shift: ld_shift < D");
+    return b200rl::ppo_loss_gaussian_launch("ppo_loss_gaussian_shift", new_mean, ld_mean, logstd, new_value, ld_value,
+                                            mb_inds, b_actions, b_logprobs, b_advantages, b_returns, b_values, mean_shift,
+                                            ld_shift, M, D, clip_coef, ent_coef, vf_coef, norm_adv, clip_vloss, dmean,
+                                            ld_dmean, dlogstd, dvalue, ld_dvalue, stats, workspace, workspace_bytes,
+                                            stream);
 }

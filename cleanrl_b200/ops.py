@@ -971,8 +971,10 @@ def gaussian_eval(mean, logstd, action):
 
 def ppo_loss_gaussian(new_mean, logstd, new_value, mb_inds, b_actions, b_logprobs, b_advantages, b_returns, b_values,
                       clip_coef, ent_coef, vf_coef, norm_adv=True, clip_vloss=True, dmean=None, dlogstd=None, dvalue=None,
-                      stats=None):
-    """Continuous-action PPO loss + gradients (reference: ppo_continuous_action.py:262-300)."""
+                      stats=None, mean_shift=None):
+    """Continuous-action PPO loss + gradients (reference: ppo_continuous_action.py:262-300).  ``mean_shift`` [M, D]
+    (minibatch row order): evaluate ``Normal(new_mean + mean_shift, std)`` instead, as RPO's update does
+    (rpo_continuous_action.py:138-142); ``dmean`` stays the gradient w.r.t. ``new_mean``."""
     lib = _lib.load()
     M, D = new_mean.shape
     dev = new_mean.device
@@ -988,15 +990,23 @@ def ppo_loss_gaussian(new_mean, logstd, new_value, mb_inds, b_actions, b_logprob
     if stats is None:
         stats = torch.zeros(16, dtype=f, device=dev)
     ws = _workspace(dev, "gloss", lib.b200rl_ppo_loss_gaussian_workspace_bytes(M))
-    rc = lib.b200rl_ppo_loss_gaussian_f32(
-        _ptr(new_mean, f, "new_mean"), new_mean.stride(0), _ptr(logstd, f, "logstd"),
-        _ptr(new_value, f, "new_value"), new_value.stride(0), _ptr(mb_inds, torch.int64, "mb_inds", True),
-        _ptr(b_actions, f, "b_actions"), _ptr(b_logprobs, f, "b_logprobs"), _ptr(b_advantages, f, "b_advantages"),
-        _ptr(b_returns, f, "b_returns"), _ptr(b_values, f, "b_values"), M, D, float(clip_coef), float(ent_coef),
-        float(vf_coef), int(bool(norm_adv)), int(bool(clip_vloss)), _ptr(dmean, f, "dmean"), dmean.stride(0),
-        _ptr(dlogstd, f, "dlogstd"), _ptr(dv2, f, "dvalue"), dv2.stride(0), _ptr(stats, f, "stats"),
-        ws.data_ptr(), ws.numel(), _stream())
-    _lib.check(rc, "ppo_loss_gaussian")
+    inputs = (_ptr(new_mean, f, "new_mean"), new_mean.stride(0), _ptr(logstd, f, "logstd"),
+              _ptr(new_value, f, "new_value"), new_value.stride(0), _ptr(mb_inds, torch.int64, "mb_inds", True),
+              _ptr(b_actions, f, "b_actions"), _ptr(b_logprobs, f, "b_logprobs"), _ptr(b_advantages, f, "b_advantages"),
+              _ptr(b_returns, f, "b_returns"), _ptr(b_values, f, "b_values"))
+    rest = (M, D, float(clip_coef), float(ent_coef), float(vf_coef), int(bool(norm_adv)), int(bool(clip_vloss)),
+            _ptr(dmean, f, "dmean"), dmean.stride(0), _ptr(dlogstd, f, "dlogstd"), _ptr(dv2, f, "dvalue"), dv2.stride(0),
+            _ptr(stats, f, "stats"), ws.data_ptr(), ws.numel(), _stream())
+    if mean_shift is None:
+        rc = lib.b200rl_ppo_loss_gaussian_f32(*inputs, *rest)
+        _lib.check(rc, "ppo_loss_gaussian")
+    else:
+        if tuple(mean_shift.shape) != (M, D) or mean_shift.stride(1) != 1:
+            raise ValueError(f"ppo_loss_gaussian: mean_shift must be [{M}, {D}] with unit column stride, "
+                             f"got {tuple(mean_shift.shape)} strides {mean_shift.stride()}")
+        rc = lib.b200rl_ppo_loss_gaussian_shift_f32(*inputs, _ptr(mean_shift, f, "mean_shift"), mean_shift.stride(0),
+                                                    *rest)
+        _lib.check(rc, "ppo_loss_gaussian_shift")
     return stats, dmean, dlogstd, dvalue
 
 

@@ -729,6 +729,8 @@ class PPOEngine:
                    and self.agent.uses_tc_plan()
                    and (self.world_size == 1 or os.environ.get("CLEANRL_B200_UPDATE_GRAPHS_DP", "0") == "1"))
         self._upd_iters += 1
+        # optional per-epoch agent work before the epoch's minibatches (outside any capture), e.g. RPOAgent's mean shifts
+        epoch_hook = getattr(self.agent, "begin_update_epoch", None)
         if graphed:
             hy = self.hyper_h.numpy()
             for j in range(E * nmb):                 # the scalars of every update of this iteration (host, double, as clip_adam)
@@ -744,6 +746,8 @@ class PPOEngine:
             self.b_inds_h[epoch].copy_(torch.from_numpy(b_inds_np))        # one pinned slot per epoch: never rewritten in flight
             self.b_inds[epoch].copy_(self.b_inds_h[epoch], non_blocking=True)
             self.h2d_bytes += B * 8
+            if epoch_hook is not None:
+                epoch_hook(epoch, E, B)
             if graphed:
                 g = self._upd_graphs.get(epoch)
                 if g is None:
@@ -779,8 +783,10 @@ class PPOEngine:
             # same minibatch SETS as the reference's shuffle; rows visited in ascending address order so the frames gathered
             # by conv1 share DRAM pages / TLB entries (the sums over a minibatch are order-independent up to fp rounding)
             self.b_inds[epoch].copy_(torch.sort(self.b_inds[epoch].view(nmb, M), dim=1).values.view(B))
+        offsets = hasattr(self.agent, "begin_update_epoch")     # the agent reads per-epoch rows at the minibatch's offset
         for start in range(0, B, M):
-            self.minibatch_update(self.b_inds[epoch, start:start + M], lr, k, dyn=self.hyper[k] if dyn else None)
+            self.minibatch_update(self.b_inds[epoch, start:start + M], lr, k, dyn=self.hyper[k] if dyn else None,
+                                  **({"mb_start": start} if offsets else {}))
             k += 1
         return k
 
@@ -800,10 +806,11 @@ class PPOEngine:
         return g
 
     @torch.no_grad()
-    def minibatch_update(self, mb_inds, lr, k=0, dyn=None):
+    def minibatch_update(self, mb_inds, lr, k=0, dyn=None, mb_start=None):
         """ONE fused update on the rollout rows ``mb_inds`` (device int64): forward with the row gather folded in,
         loss + its gradient, hand-written backward, DP gradient exchange, clip + Adam (ppo.py:250-290,
-        ppo_atari_multigpu.py:360-377).  ``stats[k]`` receives the logged scalars."""
+        ppo_atari_multigpu.py:360-377).  ``stats[k]`` receives the logged scalars.  ``mb_start``: the minibatch's row
+        offset within its epoch, passed on to ``loss_backward`` when given (agents with ``begin_update_epoch``)."""
         a, agent, flat, B = self.args, self.agent, self.flat, self.B
         b_obs = self.obs.view((B,) + tuple(self.obs.shape[2:]))
         b = {"actions": self.actions.view((B,) + tuple(self.actions.shape[2:])), "logprobs": self.logprobs.view(B),
@@ -814,7 +821,10 @@ class PPOEngine:
             policy_out, value = agent.forward_train(b_obs, mb_inds, aux=self.obs_t.view(B, 64, 448))
         else:
             policy_out, value = agent.forward_train(b_obs, mb_inds)
-        agent.loss_backward(policy_out, value, mb_inds, b, a, self.stats[k], self._scratch)
+        if mb_start is None:
+            agent.loss_backward(policy_out, value, mb_inds, b, a, self.stats[k], self._scratch)
+        else:
+            agent.loss_backward(policy_out, value, mb_inds, b, a, self.stats[k], self._scratch, mb_start=mb_start)
         if self.world_size > 1:
             self._exchange_gradients()
         if dyn is not None:      # captured: the (step, lr) scalars of update k come from the device table

@@ -148,6 +148,21 @@ int b200rl_ppo_loss_gaussian_f32(const float* new_mean, int64_t ld_mean, const f
                                  int norm_adv, int clip_vloss,
                                  float* dmean, int64_t ld_dmean, float* dlogstd, float* dvalue, int64_t ld_dvalue,
                                  float* stats, void* workspace, size_t workspace_bytes, void* stream);
+/* The same loss with the policy mean shifted per row (cleanrl/rpo_continuous_action.py:138-142: Normal(mean + z, std)
+ * when the update re-evaluates stored actions).  mean_shift f32 [M, D] (row stride ld_shift >= D, minibatch row
+ * order, not gathered through mb_inds); each row uses mu = fl(new_mean + mean_shift) wherever the loss above uses
+ * new_mean.  dmean is d loss / d new_mean (== d loss / d mu).  Same launches, workspace and other arguments as
+ * b200rl_ppo_loss_gaussian_f32; a null mean_shift is refused. */
+int b200rl_ppo_loss_gaussian_shift_f32(const float* new_mean, int64_t ld_mean, const float* logstd,
+                                       const float* new_value, int64_t ld_value, const int64_t* mb_inds,
+                                       const float* b_actions, const float* b_logprobs,
+                                       const float* b_advantages, const float* b_returns, const float* b_values,
+                                       const float* mean_shift, int64_t ld_shift,
+                                       int64_t M, int D, double clip_coef, double ent_coef, double vf_coef,
+                                       int norm_adv, int clip_vloss,
+                                       float* dmean, int64_t ld_dmean, float* dlogstd, float* dvalue,
+                                       int64_t ld_dvalue, float* stats, void* workspace, size_t workspace_bytes,
+                                       void* stream);
 
 /* ------------------------------------------------- grad clip + Adam step ---
  * One fused optimiser step over a FLAT f32 parameter vector: optional DP
