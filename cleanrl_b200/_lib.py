@@ -138,6 +138,16 @@ SIGNATURES = {
     "b200rl_td3_actor_bwd_f32": (_i, [_p, _i64, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p]),
     "b200rl_ddpg_critic_loss_bwd_f32": (_i, [_p, _i64, _i, _i, _p, _p, _p, _p, _i64, _p, _d, _p, _p, _p, _p, _p, _p,
                                              _p, _p, _sz, _p]),
+    "b200rl_radam_step_scalars": (_i, [_i64, _d, _d, _d, _p]),
+    "b200rl_clip_radam_f32": (_i, [_p, _p, _p, _p, _i64, _i64, _d, _d, _d, _d, _d, _p, _p, _sz, _p]),
+    "b200rl_clip_radam_dyn_f32": (_i, [_p, _p, _p, _p, _i64, _p, _d, _d, _d, _d, _p, _p, _sz, _p]),
+    "b200rl_pqn_param_count": (_i64, [_i, _i]),
+    "b200rl_pqn_workspace_bytes": (_sz, [_i64]),
+    "b200rl_pqn_act_f32": (_i, [_p, _p, _i64, _i64, _i, _i, _p, _p, _d, _p, _p, _p, _p, _p, _i64, _p]),
+    "b200rl_pqn_forward_f32": (_i, [_p, _p, _i64, _i64, _i, _i, _p, _p]),
+    "b200rl_pqn_loss_bwd_f32": (_i, [_p, _p, _i64, _p, _p, _p, _i64, _i, _i, _p, _p, _sz, _p]),
+    "b200rl_pqn_wgrad_f32": (_i, [_p, _i64, _p, _p, _i64, _i, _i, _p, _sz, _p, _p]),
+    "b200rl_qlambda_f32": (_i, [_p, _p, _p, _p, _p, _p, _i64, _i64, _d, _d, _p]),
 }
 
 

@@ -1749,3 +1749,43 @@ def ddpg_update(state, ring, batch, global_step, args, graph=None):
     _replay_update_graph(st, key, lambda: _ddpg_update_body(st, *views, buf["rows"], buf, actor_step, args.gamma,
                                                             args.tau))
     return st
+
+
+# ---------------------------------------------------------- PQN (cleanrl/pqn.py)
+class PQNQNetwork(nn.Module):
+    """pqn.py:89-104: ``network`` = Linear(obs, 120), LayerNorm(120), ReLU, Linear(120, 84), LayerNorm(84), ReLU,
+    Linear(84, A), with ``layer_init``'s orthogonal initialisation in the reference's layer order (a seed gives the
+    reference's weights) and its state_dict keys.  ``forward(x)`` runs the fp32 LayerNorm kernel on the parameters'
+    flat buffer (``flat``, a ``nets.FlatParams`` built on first use on their CUDA device)."""
+
+    def __init__(self, env):
+        super().__init__()
+        self.obs_dim = int(np.array(env.single_observation_space.shape).prod())
+        self.n_actions = int(env.single_action_space.n)
+        ops.pqn_param_count(self.obs_dim, self.n_actions)          # refuses shapes outside the kernels' limits
+        self.network = nn.Sequential(
+            layer_init(nn.Linear(np.array(env.single_observation_space.shape).prod(), 120)),
+            nn.LayerNorm(120),
+            nn.ReLU(),
+            layer_init(nn.Linear(120, 84)),
+            nn.LayerNorm(84),
+            nn.ReLU(),
+            layer_init(nn.Linear(84, env.single_action_space.n)),
+        )
+        self._flat = None
+
+    @property
+    def flat(self):
+        p = next(self.parameters())
+        f = self._flat
+        if f is None or f.flat.device != p.device or p.data_ptr() != f.flat.data_ptr():
+            if p.device.type != "cuda":
+                raise RuntimeError("cleanrl_b200 agents execute on CUDA only (libb200rl kernels); there is no CPU fallback.")
+            self._flat = nets.FlatParams(list(self.parameters()), p.device)
+        return self._flat
+
+    @torch.no_grad()
+    def forward(self, x):
+        flat = self.flat.flat
+        x = x.float().reshape(x.shape[0], -1).contiguous()
+        return ops.pqn_forward(flat, x, self.obs_dim, self.n_actions)

@@ -348,6 +348,28 @@ def ddpg_continuous_action_args(exp_name="ddpg_continuous_action"):
     return _make("Args", common + algo + extra)
 
 
+def pqn_args(exp_name="pqn"):
+    """cleanrl/pqn.py:17-64."""
+    algo = [
+        ("env_id", str, "CartPole-v1", "the id of the environment"),
+        ("total_timesteps", int, 500000, "total timesteps of the experiments"),
+        ("learning_rate", float, 2.5e-4, "the learning rate of the optimizer"),
+        ("num_envs", int, 4, "the number of parallel game environments"),
+        ("num_steps", int, 128, "the number of steps to run for each environment per update"),
+        ("num_minibatches", int, 4, "the number of mini-batches"),
+        ("update_epochs", int, 4, "the K epochs to update the policy"),
+        ("anneal_lr", bool, True, "Toggle learning rate annealing"),
+        ("gamma", float, 0.99, "the discount factor gamma"),
+        ("start_e", float, 1, "the starting epsilon for exploration"),
+        ("end_e", float, 0.05, "the ending epsilon for exploration"),
+        ("exploration_fraction", float, 0.5, "the fraction of `total_timesteps` it takes from start_e to end_e"),
+        ("max_grad_norm", float, 10.0, "the maximum norm for the gradient clipping"),
+        ("q_lambda", float, 0.65, "the lambda for Q(lambda)"),
+    ]
+    extra = [r for r in _EXTRA if r[0] == "synthetic_env"]
+    return _make("Args", _override(_COMMON, exp_name=exp_name) + algo + extra)
+
+
 def parse(cls, argv=None):
     return tyro.cli(cls, args=argv)
 

@@ -85,12 +85,21 @@ struct AdamScalars {
     int do_clip;
 };
 
+// The moment updates Adam and RAdam share (torch/optim/adam.py and radam.py, the same two lines).  CPU torch's
+// addcmul_ is one fused multiply-add, fma(value * t1, t2, self), which RAdam follows (kFmaAddcmul) to stay bitwise
+// equal to CPU torch.optim.RAdam; Adam keeps its separately rounded sum.
+template <bool kFmaAddcmul>
+__device__ __forceinline__ void adam_moments(float g, float& m, float& v, float w1, float beta2, float w2) {
+    m = fmaf(w1, g - m, m);                         // exp_avg.lerp_(grad, 1-beta1)
+    v = v * beta2;                                  // exp_avg_sq.mul_(beta2)
+    if (kFmaAddcmul) v = fmaf(__fmul_rn(w2, g), g, v);     // .addcmul_(grad, grad, value=1-beta2)
+    else v = __fadd_rn(v, __fmul_rn(__fmul_rn(w2, g), g));
+}
+
 __device__ __forceinline__ void adam_one(float& p, float g, float& m, float& v, const AdamScalars& a, float coef) {
     if (a.divide_world) g = g / a.world;
     if (a.do_clip) g = g * coef;
-    m = fmaf(a.w1, g - m, m);                       // exp_avg.lerp_(grad, 1-beta1)
-    v = v * a.beta2;                                // exp_avg_sq.mul_(beta2)
-    v = __fadd_rn(v, __fmul_rn(__fmul_rn(a.w2, g), g));   // .addcmul_(grad, grad, value=1-beta2)
+    adam_moments<false>(g, m, v, a.w1, a.beta2, a.w2);
     const float denom = __fadd_rn(__fdiv_rn(sqrtf(v), a.bc2_sqrt), a.eps);
     p = __fadd_rn(p, __fmul_rn(a.neg_step_size, __fdiv_rn(m, denom)));   // addcdiv_(m, denom, -step_size)
 }
@@ -358,4 +367,131 @@ extern "C" int b200rl_clip_adam_ranges_dyn_f32(float* params, const float* grads
     B200RL_REQUIRE(step_scalars, "clip_adam_ranges_dyn: null scalar table");
     return b200rl::clip_adam_ranges_impl(params, grads, exp_avg, exp_avg_sq, P, 0, 0.0, ranges, nranges, 0, 0.0, step_scalars,
                                          frozen, beta1, beta2, eps, max_norm, norm_out, workspace, workspace_bytes, stream);
+}
+
+// ---- clip + RAdam (torch/optim/radam.py _single_tensor_radam, no weight decay).  The four step-dependent scalars stay
+// separate, each rounded to f32 where the tensor operation that uses it rounds it:
+//   rho_t <= 5: p -= (m / bc1) * lr
+//   rho_t >  5: p -= (((m / bc1) * lr) * (reciprocal(sqrt(v) + eps) * sqrt(bc2))) * rect
+namespace b200rl {
+struct RAdamScalars {
+    float w1, beta2, w2, eps;
+    float bc1, lr, bc2_sqrt, rect;   // rect <= 0: rho_t <= 5 (no rectification)
+    int do_clip;
+};
+
+__device__ __forceinline__ void radam_one(float& p, float g, float& m, float& v, const RAdamScalars& a, float coef) {
+    if (a.do_clip) g = g * coef;
+    adam_moments<true>(g, m, v, a.w1, a.beta2, a.w2);
+    const float u = __fmul_rn(__fdiv_rn(m, a.bc1), a.lr);                 // bias_corrected_exp_avg * lr
+    if (a.rect > 0.f) {
+        const float adaptive = __fmul_rn(__frcp_rn(__fadd_rn(sqrtf(v), a.eps)), a.bc2_sqrt);   // bc2**0.5 / (sqrt(v)+eps)
+        p = __fsub_rn(p, __fmul_rn(__fmul_rn(u, adaptive), a.rect));
+    } else {
+        p = __fsub_rn(p, u);
+    }
+}
+
+__global__ void __launch_bounds__(kOptThreads) radam_kernel(
+    float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
+    int64_t P, RAdamScalars a, const OptScratch* sc, const float* __restrict__ dyn) {
+    if (dyn) { a.bc1 = __ldg(dyn); a.lr = __ldg(dyn + 1); a.bc2_sqrt = __ldg(dyn + 2); a.rect = __ldg(dyn + 3); }
+    const float coef = a.do_clip ? sc->coef : 1.f;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t P4 = P >> 2;
+    float4* p4 = reinterpret_cast<float4*>(p);
+    const float4* g4 = reinterpret_cast<const float4*>(g);
+    float4* m4 = reinterpret_cast<float4*>(m);
+    float4* v4 = reinterpret_cast<float4*>(v);
+    for (int64_t i = tid; i < P4; i += stride) {
+        float4 pp = p4[i], gg = __ldg(g4 + i), mm = m4[i], vv = v4[i];
+        radam_one(pp.x, gg.x, mm.x, vv.x, a, coef);
+        radam_one(pp.y, gg.y, mm.y, vv.y, a, coef);
+        radam_one(pp.z, gg.z, mm.z, vv.z, a, coef);
+        radam_one(pp.w, gg.w, mm.w, vv.w, a, coef);
+        p4[i] = pp; m4[i] = mm; v4[i] = vv;
+    }
+    for (int64_t i = (P4 << 2) + tid; i < P; i += stride) {
+        float pp = p[i], mm = m[i], vv = v[i];
+        radam_one(pp, g[i], mm, vv, a, coef);
+        p[i] = pp; m[i] = mm; v[i] = vv;
+    }
+}
+
+// the scalar algebra of _single_tensor_radam in double, as python runs it (x ** 0.5 is C pow)
+static void radam_step_scalars(int64_t step, double lr, double beta1, double beta2, float* out4) {
+    const double st = (double)step;
+    const double bc1 = 1.0 - pow(beta1, st);
+    const double bc2 = 1.0 - pow(beta2, st);
+    const double rho_inf = 2.0 / (1.0 - beta2) - 1.0;
+    const double rho_t = rho_inf - 2.0 * st * pow(beta2, st) / bc2;
+    out4[0] = (float)bc1;
+    out4[1] = (float)lr;
+    out4[2] = (float)pow(bc2, 0.5);
+    out4[3] = rho_t > 5.0 ? (float)pow((rho_t - 4.0) * (rho_t - 2.0) * rho_inf / ((rho_inf - 4.0) * (rho_inf - 2.0) * rho_t), 0.5)
+                          : 0.f;
+}
+
+// dyn == nullptr: (step, lr) by value; else the four step-dependent scalars are read from device memory
+static int clip_radam_impl(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, int64_t P, int64_t step,
+                           double lr, const float* dyn, double beta1, double beta2, double eps, double max_norm,
+                           float* norm_out, void* workspace, size_t workspace_bytes, void* stream) {
+    B200RL_REQUIRE(P >= 0, "clip_radam: negative P");
+    if (P == 0) return B200RL_OK;
+    B200RL_REQUIRE(params && grads && exp_avg && exp_avg_sq, "clip_radam: null pointer");
+    B200RL_REQUIRE(aligned(params, 16) && aligned(grads, 16) && aligned(exp_avg, 16) && aligned(exp_avg_sq, 16),
+                   "clip_radam: buffers must be 16-B aligned (float4 path)");
+    B200RL_REQUIRE(dyn || step >= 1, "clip_radam: step is 1-based (got %lld)", (long long)step);
+    B200RL_REQUIRE(!dyn || aligned(dyn, 4), "clip_radam: misaligned scalar table");
+    B200RL_REQUIRE(workspace && aligned(workspace, 16), "clip_radam: workspace null or misaligned");
+    if (workspace_bytes < b200rl_clip_adam_workspace_bytes(P))
+        return fail(B200RL_ERR_WORKSPACE, "clip_radam: workspace %zu < %zu bytes", workspace_bytes,
+                    b200rl_clip_adam_workspace_bytes(P));
+    cudaStream_t s = (cudaStream_t)stream;
+    OptScratch* sc = reinterpret_cast<OptScratch*>(workspace);
+    double* partials = reinterpret_cast<double*>(reinterpret_cast<char*>(workspace) + sizeof(OptScratch));
+    const unsigned blocks = opt_blocks(P);
+    ProfScope ps(s, "clip_radam", 0, 32.0 * P);
+    if (max_norm >= 0.0 || norm_out) {
+        cudaError_t e = cudaMemsetAsync(&sc->ticket, 0, sizeof(unsigned int), s);
+        if (e != cudaSuccess) return fail(B200RL_ERR_CUDA, "clip_radam: memset: %s", cudaGetErrorString(e));
+        grad_sumsq_kernel<<<blocks, kOptThreads, 0, s>>>(grads, P, 0.f, 1.f, (float)max_norm, sc, partials, norm_out);
+        int rc = check_launch("clip_radam/sumsq");
+        if (rc) return rc;
+    }
+    RAdamScalars a;
+    a.w1 = (float)(1.0 - beta1);
+    a.beta2 = (float)beta2;
+    a.w2 = (float)(1.0 - beta2);
+    a.eps = (float)eps;
+    float s4[4] = {1.f, 0.f, 1.f, 0.f};
+    if (!dyn) radam_step_scalars(step, lr, beta1, beta2, s4);
+    a.bc1 = s4[0]; a.lr = s4[1]; a.bc2_sqrt = s4[2]; a.rect = s4[3];
+    a.do_clip = max_norm >= 0.0;
+    radam_kernel<<<blocks, kOptThreads, 0, s>>>(params, grads, exp_avg, exp_avg_sq, P, a, sc, dyn);
+    return check_launch("clip_radam/radam");
+}
+}  // namespace b200rl
+
+extern "C" int b200rl_radam_step_scalars(int64_t step, double lr, double beta1, double beta2, float* out4) {
+    B200RL_REQUIRE(out4 && step >= 1, "radam_step_scalars: bad arguments");
+    b200rl::radam_step_scalars(step, lr, beta1, beta2, out4);
+    return B200RL_OK;
+}
+
+extern "C" int b200rl_clip_radam_f32(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, int64_t P,
+                                     int64_t step, double lr, double beta1, double beta2, double eps, double max_norm,
+                                     float* norm_out, void* workspace, size_t workspace_bytes, void* stream) {
+    return b200rl::clip_radam_impl(params, grads, exp_avg, exp_avg_sq, P, step, lr, nullptr, beta1, beta2, eps, max_norm,
+                                   norm_out, workspace, workspace_bytes, stream);
+}
+
+extern "C" int b200rl_clip_radam_dyn_f32(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, int64_t P,
+                                         const float* step_scalars, double beta1, double beta2, double eps,
+                                         double max_norm, float* norm_out, void* workspace, size_t workspace_bytes,
+                                         void* stream) {
+    B200RL_REQUIRE(step_scalars, "clip_radam_dyn: null scalar table");
+    return b200rl::clip_radam_impl(params, grads, exp_avg, exp_avg_sq, P, 0, 0.0, step_scalars, beta1, beta2, eps,
+                                   max_norm, norm_out, workspace, workspace_bytes, stream);
 }

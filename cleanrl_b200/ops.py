@@ -1365,3 +1365,137 @@ def ddpg_critic_loss_bwd(params, B, obs_dim, act_dim, q_next, q, rewards, dones,
         _ptr(dz1, _F32, "dz1"), _ptr(dz2, _F32, "dz2"), _ptr(stats, _F32, "stats"), ws.data_ptr(), ws.numel(), _stream())
     _lib.check(rc, "ddpg_critic_loss_bwd")
     return stats, dq, dz1, dz2
+
+
+# ------------------------------------------------------------------------------ RAdam (torch/optim/radam.py)
+def radam_step_scalars(step, lr, beta1=0.9, beta2=0.999):
+    """(bc1, lr, bc2 ** 0.5, rect) as float32 (rect 0 where rho_t <= 5), computed by the library in double as
+    ``_single_tensor_radam`` computes them in python."""
+    import ctypes
+    out = (ctypes.c_float * 4)()
+    _lib.check(_lib.load().b200rl_radam_step_scalars(int(step), float(lr), float(beta1), float(beta2), out),
+               "radam_step_scalars")
+    return tuple(float(x) for x in out)
+
+
+def _radam_args(params, grads, exp_avg, exp_avg_sq):
+    P = params.numel()
+    for n_, t in (("params", params), ("grads", grads), ("exp_avg", exp_avg), ("exp_avg_sq", exp_avg_sq)):
+        _contig(t, n_)
+        assert t.numel() == P
+    return (_ptr(params, _F32, "params"), _ptr(grads, _F32, "grads"), _ptr(exp_avg, _F32, "exp_avg"),
+            _ptr(exp_avg_sq, _F32, "exp_avg_sq"), P)
+
+
+def clip_radam(params, grads, exp_avg, exp_avg_sq, step, lr, beta1=0.9, beta2=0.999, eps=1e-8, max_norm=10.0,
+               norm_out=None):
+    """In-place clip_grad_norm_ + RAdam step on flat f32 vectors (cleanrl/pqn.py:239-240); ``max_norm`` None: no clip."""
+    lib = _lib.load()
+    *ptrs, P = _radam_args(params, grads, exp_avg, exp_avg_sq)
+    ws = _workspace(params.device, "adam", lib.b200rl_clip_adam_workspace_bytes(P))
+    rc = lib.b200rl_clip_radam_f32(*ptrs, P, int(step), float(lr), float(beta1), float(beta2), float(eps),
+                                   -1.0 if max_norm is None else float(max_norm), _o(norm_out, "norm_out"),
+                                   ws.data_ptr(), ws.numel(), _stream())
+    _lib.check(rc, "clip_radam")
+    return params
+
+
+def clip_radam_dyn(params, grads, exp_avg, exp_avg_sq, step_scalars, beta1=0.9, beta2=0.999, eps=1e-8, max_norm=10.0,
+                   norm_out=None):
+    """``clip_radam`` with the four step scalars of ``radam_step_scalars`` in device memory (f32 [4]): what a captured
+    CUDA graph of the update replays."""
+    lib = _lib.load()
+    *ptrs, P = _radam_args(params, grads, exp_avg, exp_avg_sq)
+    assert step_scalars.numel() == 4 and step_scalars.is_contiguous()
+    ws = _workspace(params.device, "adam", lib.b200rl_clip_adam_workspace_bytes(P))
+    rc = lib.b200rl_clip_radam_dyn_f32(*ptrs, P, _ptr(step_scalars, _F32, "step_scalars"), float(beta1), float(beta2),
+                                       float(eps), -1.0 if max_norm is None else float(max_norm),
+                                       _o(norm_out, "norm_out"), ws.data_ptr(), ws.numel(), _stream())
+    _lib.check(rc, "clip_radam_dyn")
+    return params
+
+
+# ------------------------------------------------------------------------------ PQN (cleanrl/pqn.py)
+PQN_STAT_NAMES = ("td_loss", "q_values")
+
+
+def pqn_param_count(obs_dim, A):
+    n = _lib.load().b200rl_pqn_param_count(int(obs_dim), int(A))
+    if n < 0:
+        raise ValueError(f"pqn: obs_dim={obs_dim}, A={A} outside the kernels' limits (1 <= obs_dim <= 512, 2 <= A <= 64)")
+    return n
+
+
+def pqn_workspace(M, device):
+    """Zeroed update workspace of a minibatch of up to M rows (one loss_bwd and the wgrad after it)."""
+    return torch.zeros(int(_lib.load().b200rl_pqn_workspace_bytes(int(M))), dtype=torch.uint8, device=device)
+
+
+def _obs2d(obs, obs_dim):
+    if obs.dim() != 2 or obs.stride(1) != 1 or obs.shape[1] != obs_dim:
+        raise ValueError(f"pqn: obs must be row-major [n, {obs_dim}] with unit column stride")
+    return obs.stride(0)
+
+
+def pqn_act(params, obs, obs_dim, A, values, random_actions=None, u=None, eps=0.0, actions=None, obs_slot=None,
+            copy=None):
+    """The rollout step (pqn.py:180-189) on obs [n, obs_dim]: ``values`` [n] = max Q and, with ``random_actions`` /
+    ``u`` (the step's CPU draws), ``actions`` [n] int64 = u < eps ? random : argmax Q.  ``obs_slot`` [n, obs_dim] receives a
+    copy of the rows and ``copy`` = (src, dst) f32 tensors of equal size is copied in the same launch."""
+    n = obs.shape[0]
+    src, dst = copy if copy is not None else (None, None)
+    rc = _lib.load().b200rl_pqn_act_f32(
+        _ptr(params, _F32, "params"), _ptr(obs, _F32, "obs"), _obs2d(obs, obs_dim), n, int(obs_dim), int(A),
+        _rows(random_actions, "random_actions"), _o(u, "u"), float(eps), _o(obs_slot, "obs_slot"),
+        _rows(actions, "actions"), _ptr(values, _F32, "values"), _o(src, "copy_in"), _o(dst, "copy_out"),
+        0 if src is None else int(src.numel()), _stream())
+    _lib.check(rc, "pqn_act")
+    return actions, values
+
+
+def pqn_forward(params, obs, obs_dim, A, q=None):
+    """QNetwork.forward: q [n, A]."""
+    n = obs.shape[0]
+    q = torch.empty(n, A, dtype=_F32, device=obs.device) if q is None else q
+    rc = _lib.load().b200rl_pqn_forward_f32(_ptr(params, _F32, "params"), _ptr(obs, _F32, "obs"), _obs2d(obs, obs_dim), n,
+                                            int(obs_dim), int(A), _ptr(_contig(q, "q"), _F32, "q"), _stream())
+    _lib.check(rc, "pqn_forward")
+    return q
+
+
+def pqn_loss_bwd(params, obs, obs_dim, A, mb_inds, b_actions, b_returns, stats, workspace):
+    """One minibatch's loss, data backward and kept activations (pqn.py:233-238); ``stats`` [2] = ``PQN_STAT_NAMES``."""
+    M = int(mb_inds.numel())
+    rc = _lib.load().b200rl_pqn_loss_bwd_f32(
+        _ptr(params, _F32, "params"), _ptr(obs, _F32, "obs"), _obs2d(obs, obs_dim), _rows(mb_inds, "mb_inds"),
+        _rows(b_actions, "b_actions"), _ptr(_contig(b_returns, "b_returns"), _F32, "b_returns"), M, int(obs_dim), int(A),
+        _ptr(stats, _F32, "stats"), workspace.data_ptr(), workspace.numel(), _stream())
+    _lib.check(rc, "pqn_loss_bwd")
+    return stats
+
+
+def pqn_wgrad(obs, obs_dim, A, mb_inds, b_actions, workspace, grad):
+    """Every weight / bias / gamma / beta gradient of the minibatch the last ``pqn_loss_bwd`` on ``workspace`` saw."""
+    M = int(mb_inds.numel())
+    rc = _lib.load().b200rl_pqn_wgrad_f32(
+        _ptr(obs, _F32, "obs"), _obs2d(obs, obs_dim), _rows(mb_inds, "mb_inds"), _rows(b_actions, "b_actions"), M,
+        int(obs_dim), int(A), workspace.data_ptr(), workspace.numel(), _ptr(grad, _F32, "grad"), _stream())
+    _lib.check(rc, "pqn_wgrad")
+
+
+def qlambda(rewards, values, dones, next_value, next_done, gamma, q_lambda, returns=None):
+    """Q(lambda) returns (pqn.py:205-218), bit-identical to the reference loop."""
+    T, N = rewards.shape
+    for n_, t in (("rewards", rewards), ("values", values), ("dones", dones)):
+        _contig(t, n_)
+        assert t.shape == (T, N), f"{n_} shape {tuple(t.shape)} != {(T, N)}"
+    next_value = _contig(next_value.reshape(-1), "next_value")
+    next_done = _contig(next_done.reshape(-1), "next_done")
+    assert next_value.numel() == N and next_done.numel() == N
+    returns = torch.empty_like(rewards) if returns is None else returns
+    rc = _lib.load().b200rl_qlambda_f32(
+        _ptr(rewards, _F32, "rewards"), _ptr(values, _F32, "values"), _ptr(dones, _F32, "dones"),
+        _ptr(next_value, _F32, "next_value"), _ptr(next_done, _F32, "next_done"), _ptr(returns, _F32, "returns"), T, N,
+        float(gamma), float(q_lambda), _stream())
+    _lib.check(rc, "qlambda")
+    return returns

@@ -210,6 +210,23 @@ int b200rl_clip_adam_ranges_dyn_f32(float* params, const float* grads, float* ex
                                     double beta1, double beta2, double eps, double max_norm, float* norm_out,
                                     void* workspace, size_t workspace_bytes, void* stream);
 
+/* grad clip + RAdam (torch/optim/radam.py _single_tensor_radam op order, no weight decay; cleanrl/pqn.py:152,239-240).
+ * The clip norm, max_norm, norm_out, buffers and workspace are those of b200rl_clip_adam_f32 (world_size 1).  The
+ * step-dependent scalars are python doubles rounded to f32 where the tensor operation that uses each of them rounds it:
+ * with bc1 = 1 - beta1^step, bc2 = 1 - beta2^step and rho_t = rho_inf - 2 step beta2^step / bc2,
+ *   rho_t <= 5: p -= (m / bc1) * lr
+ *   rho_t >  5: p -= (((m / bc1) * lr) * (reciprocal(sqrt(v) + eps) * bc2^0.5)) * rect.
+ * The second moment is fma((1 - beta2) g, g, beta2 v), one rounding, as CPU torch's addcmul_ computes it.
+ * b200rl_radam_step_scalars writes out4 = (bc1, lr, bc2^0.5, rect) as f32, rect = 0 when rho_t <= 5; the _dyn entry point
+ * reads those four from DEVICE memory (step_scalars f32 [4]) so a captured CUDA graph replays for any step / lr. */
+int b200rl_radam_step_scalars(int64_t step, double lr, double beta1, double beta2, float* out4);
+int b200rl_clip_radam_f32(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, int64_t P,
+                          int64_t step, double lr, double beta1, double beta2, double eps, double max_norm,
+                          float* norm_out, void* workspace, size_t workspace_bytes, void* stream);
+int b200rl_clip_radam_dyn_f32(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, int64_t P,
+                              const float* step_scalars, double beta1, double beta2, double eps, double max_norm,
+                              float* norm_out, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ------------------------------------------------ phasic policy gradient: auxiliary loss ------
  * cleanrl/ppg_procgen.py:449-461 on the joint head output head_out [n][A + 2] = [logits | value | aux_value] (row stride
  * ld_head): kl_loss = mean KL(Categorical(old_logits) || Categorical(logits)), aux_value_loss = 0.5 mean (aux_value - R)^2,
@@ -677,6 +694,52 @@ int b200rl_ddpg_critic_loss_bwd_f32(const float* params, int64_t B, int obs_dim,
                                     const int64_t* rows, double gamma, const float* h1, const float* h2, float* y,
                                     float* dq, float* dz1, float* dz2, float* stats, void* workspace,
                                     size_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------ parallel Q-learning ---
+ * cleanrl/pqn.py, fp32: QNetwork obs (obs_dim) -> Linear 120 -> LayerNorm -> ReLU -> Linear 84 -> LayerNorm -> ReLU ->
+ * Linear A.  Shapes: 1 <= obs_dim <= 512, 2 <= A <= 64; any other shape is B200RL_ERR_INVALID_ARGUMENT.  Parameters are
+ * flat f32 in nn.Module order (network.0.weight [120, obs_dim], network.0.bias, network.1.weight / .bias (LN1 gamma /
+ * beta), network.3.*, network.4.*, network.6.weight [A, 84], network.6.bias).  obs rows have stride ld_obs floats.
+ * Every reduction runs in a fixed order: bitwise repeatable.
+ *
+ * b200rl_pqn_param_count: floats in the network; -1 for a shape outside the limits.
+ * b200rl_pqn_act_f32: the rollout step (pqn.py:180-189) on n rows: Q, max_action = argmax Q (first maximum; a NaN counts
+ *   as the maximum), values_slot [n] = Q[max_action].  With random_actions i64 [n] and u f32 [n] (the step's CPU draws,
+ *   together or neither) actions_slot i64 [n] = u < eps ? random_actions : max_action, eps rounded to f32 as torch's
+ *   `tensor < python_float` rounds it; without them actions_slot (may then be NULL) = max_action, and values_slot is
+ *   the greedy bootstrap max Q (pqn.py:209).  obs_slot [n, obs_dim] (dense) may be NULL: a copy of the rows.  The same
+ *   launch copies copy_n floats copy_in -> copy_out (the step's done / reward bookkeeping; copy_n 0: none).
+ * b200rl_pqn_forward_f32: Q values q [n, A] (QNetwork.forward).
+ * b200rl_pqn_loss_bwd_f32: one minibatch (pqn.py:233-238): rows obs[mb_inds] (NULL: 0..M-1), q = Q[b_actions[mb_inds]],
+ *   loss = mean((b_returns[mb_inds] - q)^2), dq = F.mse_loss's backward for its target argument, and the data backward
+ *   through the head, LN2 + ReLU and LN1 + ReLU (dz = rstd (dxhat - mean(dxhat) - xhat mean(dxhat xhat))).  It keeps in
+ *   the workspace what the weight gradient reads; stats f32 [2] = td_loss, mean(q).
+ * b200rl_pqn_wgrad_f32: every weight, bias, gamma and beta gradient of that minibatch into grad (flat layout,
+ *   overwritten) from the workspace loss_bwd left, summed over rows in row order, no atomics.  Same obs / mb_inds /
+ *   b_actions / M as the loss_bwd call before it.
+ * Workspace: b200rl_pqn_workspace_bytes(M) bytes, 16-byte aligned, zeroed once; it serves a loss_bwd and the wgrad
+ *   after it, and any smaller M.
+ * b200rl_qlambda_f32: Q(lambda) returns (pqn.py:205-218) over rewards / values / dones f32 [T, N], next_value /
+ *   next_done f32 [N] into returns [T, N].  One thread per env, every operation separately rounded: bit-identical to the
+ *   reference loop.  gamma, q_lambda and 1 - q_lambda (in double) round to f32; the last step is
+ *   r + ((gamma nv) (1 - next_done)), the others r + ((gamma ((ql R') + ((1 - ql) v'))) (1 - d')).
+ */
+int64_t b200rl_pqn_param_count(int obs_dim, int A);
+size_t b200rl_pqn_workspace_bytes(int64_t M);
+int b200rl_pqn_act_f32(const float* params, const float* obs, int64_t ld_obs, int64_t n, int obs_dim, int A,
+                       const int64_t* random_actions, const float* u, double eps, float* obs_slot,
+                       int64_t* actions_slot, float* values_slot, const float* copy_in, float* copy_out,
+                       int64_t copy_n, void* stream);
+int b200rl_pqn_forward_f32(const float* params, const float* obs, int64_t ld_obs, int64_t n, int obs_dim, int A,
+                           float* q, void* stream);
+int b200rl_pqn_loss_bwd_f32(const float* params, const float* obs, int64_t ld_obs, const int64_t* mb_inds,
+                            const int64_t* b_actions, const float* b_returns, int64_t M, int obs_dim, int A,
+                            float* stats, void* workspace, size_t workspace_bytes, void* stream);
+int b200rl_pqn_wgrad_f32(const float* obs, int64_t ld_obs, const int64_t* mb_inds, const int64_t* b_actions, int64_t M,
+                         int obs_dim, int A, const void* workspace, size_t workspace_bytes, float* grad, void* stream);
+int b200rl_qlambda_f32(const float* rewards, const float* values, const float* dones, const float* next_value,
+                       const float* next_done, float* returns, int64_t T, int64_t N, double gamma, double q_lambda,
+                       void* stream);
 
 #ifdef __cplusplus
 }
